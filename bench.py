@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — rendered megapixels/s (fwd+bwd) of the RGCA shade+splat hot path on B200.
+"""bench.py — rendered megapixels/s (fwd+bwd) of the RGCA shade+splat hot path on H100.
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched by torch.distributed.run)
   python bench.py --impl reference ...                     CPU restatement of the same path on the host cores
@@ -50,15 +50,38 @@ def parse():
     ap.add_argument("--no-graph", action="store_true", help="sync-free path without CUDA-graph capture")
     ap.add_argument("--mvp-density", type=float, default=2000.0, help="template alpha scale of the --ext-compare MVP scene")
     ap.add_argument("--decoder", action="store_true",
-                    help="time the RGCA PrimDecoder forward at native size (1024^2 Gaussians): towers on tcgen05 vs SIMT, "
+                    help="time the RGCA PrimDecoder forward at native size (1024^2 Gaussians): towers on the tensor cores (wgmma) vs SIMT, "
                          "fused heads kernel; prints its own JSON line")
     ap.add_argument("--decoder-library", action="store_true",
                     help="time the same decoder tower the reference's way (library conv_transpose2d + bias + LeakyReLU "
                          "passes, cuDNN); run under `timeout`: cuDNN may compile engines for minutes on a fresh box")
     ap.add_argument("--ext-compare", action="store_true",
-                    help="time the reference's own extensions rebuilt for sm_100a (oracle/_ref) against ours: SG shade, "
+                    help="time the reference's own extensions rebuilt for sm_90a (oracle/_ref) against ours: SG shade, "
                          "raydirs, MVP raymarch (BASELINE config 4 shape); prints its own JSON line")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (images and the gradient of "
+                         "each decoded Gaussian field) as DIR/<name>.npy, float32, at most 64 MB in all")
     return ap.parse_args()
+
+
+DUMP_BYTES = 60_000_000  # below 64 MB in either reading, .npy headers included
+
+
+def dump_outputs(out_dir, arrays):
+    """Write {name: tensor} as float32 .npy files under out_dir.  When the arrays together exceed DUMP_BYTES, each is
+    reduced to a fixed, seeded sample of its flattened elements, proportional to its size, so that two runs with the
+    same arguments write the same elements."""
+    os.makedirs(out_dir, exist_ok=True)
+    header = 128  # bytes of a .npy header for these shapes
+    total = sum(t.numel() * 4 + header for t in arrays.values())
+    for i, (name, t) in enumerate(sorted(arrays.items())):
+        a = t.detach().float().cpu().numpy()
+        if total > DUMP_BYTES:
+            flat = a.reshape(-1)
+            keep = max(1, int(flat.size * ((DUMP_BYTES - header * len(arrays)) / total)) - 1)
+            idx = np.sort(np.random.default_rng(1000 + i).choice(flat.size, keep, replace=False))
+            a = flat[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 FIELDS = (("primpos", 3), ("primqvec", 4), ("primscale", 3), ("opacity", 1), ("diff_color", 3), ("lobe_dirs", 3),
@@ -92,8 +115,8 @@ def unpack(flat, G=None):
 
 
 # ------------------------------------------------------------------------------------------ GPU arm
-# measured (profiles/r02_bench_head_shade_stream.json): the side stream costs 9 us per step on this workload — the shade is
-# done before the latency-bound part of the binning starts, and the fork/join edges are not free; off by default
+# the shade is done before the latency-bound part of the binning starts, and the fork/join edges are not free: the side
+# stream is off by default
 SHADE_STREAM = os.environ.get("GOLIATH_B200_SHADE_STREAM", "0") != "0"
 HIGH_PRIO = os.environ.get("GOLIATH_B200_RENDER_PRIO", "0") != "0"
 
@@ -186,9 +209,10 @@ def sample_clocks_stop(p, path):
     return out
 
 
-def kernel_roofline(dev, packed, cam, flush, sm_mhz=None):
+def kernel_roofline(dev, packed, cam, flush):
     """Time the blend kernels alone through the C ABI (CUDA events on the launch stream, L2 flushed between
-    launches) and report achieved ALGORITHMIC bytes/s (SURVEY.md §8d formulas) against the measured HBM peak."""
+    launches) and report achieved ALGORITHMIC bytes/s (SURVEY.md §8d formulas) against the H100 data-sheet HBM
+    bandwidth."""
     from goliath_b200 import _lib
     from goliath_b200.gsplat import project_gaussians
     from goliath_b200.gsplat import utils as gu
@@ -323,13 +347,7 @@ def kernel_roofline(dev, packed, cam, flush, sm_mhz=None):
     # binning: keys/ranks of G Gaussians through 4 radix passes + bbox reads twice, one rank written and read per
     # intersection, sorted id written and read, record gather + write
     bytes_bin = G * (4 * 16 + 2 * 16) + I * (8 + 8) + I * (24 + 4 * C) + I * 48
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    which = "measured" if "hbm_gbs" in peaks else "fallback"
+    peak = 3350.0  # HBM3 of the H100 SXM, NVIDIA data sheet (GB/s)
     mode = int(L.gb_get_blend_mode())
     list_fwd = os.environ.get("GOLIATH_B200_BLEND_FWD", "list") != "rounds"
     fwd_name = ("blend_fwd_packed_kernel<4>", "blend_fwd_pipe_kernel<4>", "blend_fwd_pipe_kernel<4>",
@@ -353,31 +371,8 @@ def kernel_roofline(dev, packed, cam, flush, sm_mhz=None):
             "ms": t_binr, "alg_bytes": bytes_binr, "gbs": bytes_binr / t_binr / 1e6}
     in_step = (lambda k: k.endswith(", 1, 1>") or k.endswith("<4, 1>")) if ranked else (lambda k: True)
     dom = max((k for k in ks if k.startswith("blend") and in_step(k)), key=lambda k: ks[k]["ms"])
-    # DRAM bytes and warp instructions per launch of the dominant kernel come from the committed `ncu --set full`
-    # capture of the same scene (profiles/r02_traffic.json, written by scripts/ncu_summary.py traffic; neither is
-    # measurable live).  The blend is not HBM-bound at this operating point (DESIGN.md section 4): the second figure is
-    # the bound that does apply, warp instructions / (SMs x 4 schedulers x SM clock x the live duration).
-    traffic, ncu_note, issue = None, None, None
-    for fname in ("r02_traffic.json", "r01_traffic.json"):
-        try:
-            caps = json.load(open(os.path.join(ROOT, "profiles", fname)))["kernels"]
-            cap = caps[dom]
-        except Exception:
-            continue
-        traffic = cap["dram_bytes"]
-        ncu_note = {k: cap[k] for k in ("issue_active_pct", "sm_cycles_active_over_elapsed", "top_stalls") if k in cap}
-        ncu_note["capture"] = "profiles/" + fname
-        if cap.get("warp_inst") and sm_mhz:
-            sms = torch.cuda.get_device_properties(dev).multi_processor_count
-
-            def slot_frac(k):
-                return caps[k]["warp_inst"] / (sms * 4 * sm_mhz * 1e6 * ks[k]["ms"] * 1e-3)
-
-            issue = {"warp_inst": int(cap["warp_inst"]), "sm_mhz": sm_mhz, "sms": sms, "frac": slot_frac(dom),
-                     "kernels": {k: slot_frac(k) for k in ks if k in caps and caps[k].get("warp_inst")}}
-        break
     roof = {"bound": "hbm", "kernel": dom, "achieved": ks[dom]["gbs"], "peak": peak, "unit": "GB/s",
-            "frac": ks[dom]["gbs"] / peak, "traffic": traffic, "issue_slot": issue, "ncu": ncu_note, "peak_source": which, "intersections": int(I),
+            "frac": ks[dom]["gbs"] / peak, "peak_source": "H100 SXM data sheet", "intersections": int(I),
             "kernels": ks}
     return roof
 
@@ -504,10 +499,7 @@ def run_ours(args):
     dev = torch.device("cuda", local)
     if world > 1:
         # The two 22.8 MB collectives of a step run UNDER the neighbouring renders; what they cost the step is the SMs
-        # NCCL's CTAs take from the blend, not their own duration.  Measured at N = 4 (profiles/r02_nccl_ctas_n4.txt):
-        # 8 CTAs lengthen them to 0.15 + 0.20 ms (still hidden under the 0.4 ms render) and shorten the step by 5 %.
-        # At N = 2 the library default is better by 2 % (profiles/r02_exchange_n2.txt); at N = 8 a cap of 16 gives 11 107
-        # MP/s, 8 gives 9 797 and 4 gives 7 390 (profiles/r02_nccl_ctas_n8.txt): two CTAs per peer from N = 4.
+        # NCCL's CTAs take from the blend, not their own duration: from N = 4 they are capped at two CTAs per peer.
         if world >= 4:
             os.environ.setdefault("NCCL_MAX_CTAS", str(2 * world))
         dist.init_process_group("nccl", device_id=dev)
@@ -524,7 +516,7 @@ def run_ours(args):
     flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
 
     def flush():
-        flush_buf.fill_(1)  # > 126 MB L2
+        flush_buf.fill_(1)  # > 50 MB L2
 
     resident = host_packed.to(dev)
     cap = wl.cap
@@ -571,11 +563,14 @@ def run_ours(args):
         build_graph()
 
     # ---------------------------------------------------------------- N = 1 paths
+    last = {}
+
     def timed_single(e2e, n_steps, n_warm):
         """per-step event pairs; e2e: the table comes from pinned host memory and the images go back, serially."""
         def one():
             static_in.copy_(host_packed if e2e else resident, non_blocking=True)
-            imgs, _ = run_step()
+            imgs, grad = run_step()
+            last["imgs"], last["grad"] = imgs, grad
             if e2e:
                 for dst, src_t in zip(host_out, imgs):
                     dst.copy_(src_t, non_blocking=True)
@@ -751,6 +746,11 @@ def run_ours(args):
     collectives = None
     if world == 1:
         ms_total, per_step, wall = timed_single(False, steps, warmup)
+        if args.dump_outputs:
+            torch.cuda.synchronize()
+            outs = dict(zip(("rgb", "alpha", "depth"), last["imgs"]))
+            outs.update({"grad_" + k: v for k, v in unpack(last["grad"], G).items()})
+            dump_outputs(args.dump_outputs, outs)
         ms_e2e_serial = timed_single(True, e2e_steps, 3)[0] * steps / e2e_steps
         ms_e2e = timed_e2e_streamed_single(steps, warmup)
         h2d_rank = host_packed.numel() * 4
@@ -789,7 +789,7 @@ def run_ours(args):
         overflow = check_overflow(dev)
     roof = cpu = dec = None
     if rank == 0 and wl.key == "head":
-        roof = kernel_roofline(dev, resident, wl.cam, flush, (clocks or {}).get("sm_mhz"))
+        roof = kernel_roofline(dev, resident, wl.cam, flush)
         if world == 1 and not args.no_cpu_baseline:
             cpu = cpu_baseline(args, steps=3, warmup=3)
             try:
@@ -885,7 +885,7 @@ def _ref_ext(name):
 
 def _raymarch_kernels_alone(dev, raypos, raydir, tminmax, transf, template, step, reps=5):
     """forward / backward raymarch kernels alone through the extension-module API (ours and, when oracle/_ref holds it,
-    the reference's mvpraymarchlib rebuilt for sm_100a) on the same tensors: the extension-level ratio of north_star."""
+    the reference's mvpraymarchlib rebuilt for sm_90a) on the same tensors: the extension-level ratio of north_star."""
     from goliath_b200 import mvpraymarchlib
     from goliath_b200.mvpraymarch import _fixedorder_topology
 
@@ -931,17 +931,12 @@ def _mvp_roofline(N, K, T, P, ms_fwd, ms_bwd):
     vox = K * T[0] * T[1] * T[2]
     b_f = N * (vox * 16 + K * 60 + (2 * K - 1) * 24) + N * P * (32 + 16 + 12)
     b_b = N * (vox * 16 * 3 + K * 60 * 2 + (2 * K - 1) * 24) + N * P * (32 + 16 + 12 + 16)
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = 3350.0  # HBM3 of the H100 SXM, NVIDIA data sheet (GB/s)
     ks = {"raymarch_fwd_kernel": {"ms": ms_fwd, "alg_bytes": b_f, "gbs": b_f / ms_fwd / 1e6},
           "raymarch_bwd_kernel": {"ms": ms_bwd, "alg_bytes": b_b, "gbs": b_b / ms_bwd / 1e6}}
     dom = max(ks, key=lambda k: ks[k]["ms"])
     return {"bound": "hbm", "kernel": dom, "achieved": ks[dom]["gbs"], "peak": peak, "unit": "GB/s",
-            "frac": ks[dom]["gbs"] / peak, "traffic": None, "peak_source": "measured" if "hbm_gbs" in peaks else "fallback",
+            "frac": ks[dom]["gbs"] / peak, "peak_source": "H100 SXM data sheet",
             "note": "the march is L2/latency-bound (SURVEY.md section 8d): HBM fraction reported, not the target",
             "kernels": ks}
 
@@ -1343,8 +1338,7 @@ def run_reference(args):
     CPU implementation of the path is the oracle port, timed with all host threads.  Rank 0 only."""
     if int(os.environ.get("RANK", "0")) != 0:
         return
-    # honours --steps / --warmup (same counts as our arm asks for); one CPU step of this workload takes ~1 s on the
-    # host cores of a B200 box, so the default (no flags) is a bounded 5 + 3
+    # honours --steps / --warmup (same counts as our arm asks for); the default (no flags) is a bounded 5 + 3
     steps = 5 if args.steps is None else max(1, args.steps)
     warmup = 3 if args.warmup is None else max(0, args.warmup)
     cpu = cpu_baseline(args, steps=steps, warmup=warmup)
@@ -1379,7 +1373,7 @@ def decoder_summary(args, dev):
 
 def run_decoder(args, quick=False, dev=None):
     """Inference forward of the RGCA PrimDecoder at native size (B=1, 1024x1024 Gaussians, 162.8 M parameters,
-    random init): the two 7-layer towers on the tensor cores (tcgen05 + TMA) and on the SIMT kernels, then the fused heads
+    random init): the two 7-layer towers on the tensor cores (wgmma + TMA) and on the SIMT kernels, then the fused heads
     kernel and the SG shade.  Reports ms per part and the last layer's achieved HBM bandwidth on its mandatory bytes
     (SURVEY.md §8d: 2*Cout*H*W*4 + Cin*(H/2)*(W/2)*4)."""
     from goliath_b200 import nn as gnn
@@ -1475,7 +1469,7 @@ def run_decoder(args, quick=False, dev=None):
         res["frame_decode_shade_render_fwd_ms_graph"] = timeit(g_frame)
         res["frame_MP_per_s_fwd_graph"] = H * W / 1e6 / (res["frame_decode_shade_render_fwd_ms_graph"] * 1e-3)
         res["frame_intersection_overflow_graph"] = bool(check_overflow(dev))
-        # last layer on the tensor cores (pair-phase epilogue), for comparison with the FFMA2 kernel
+        # last layer on the tensor cores (pair-phase epilogue), for comparison with the wide SIMT kernel
         gnn.TC_MIN_CIN = 16
         for m_ in dec.vnocond_mod:
             if hasattr(m_, "_tc_cache"):
@@ -1573,7 +1567,7 @@ def run_decoder_library(args):
 
     res["last_layer_fwd_bwd_ms_library"] = timeit(last_fwd_bwd)
     # the same with TF32 disallowed: cuDNN's fp32 kernels, the precision class of this repo's SIMT backward (the TF32
-    # numbers above are the precision class of the 3xTF32 tcgen05 forward only up to the 3x split)
+    # numbers above are the precision class of the 3xTF32 wgmma forward only up to the 3x split)
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     try:
@@ -1589,7 +1583,7 @@ def run_decoder_library(args):
 # ------------------------------------------------------------------------------------------ extension-level comparison
 def run_ext_compare(args):
     """Reference arm at the EXTENSION level (SURVEY.md §8d): the reference's sgutilslib / utilslib / mvpraymarchlib
-    rebuilt for sm_100a by oracle/build_ref.py versus ours, same tensors, CUDA-event timing, L2 flushed between reps.
+    rebuilt for sm_90a by oracle/build_ref.py versus ours, same tensors, CUDA-event timing, L2 flushed between reps.
     gsplat cannot be compared: it is absent from the reference tree and from this image."""
     import importlib.util
 
@@ -1687,6 +1681,11 @@ def run_ext_compare(args):
 
 if __name__ == "__main__":
     a = parse()
+    if a.steps is not None and a.steps < 1:
+        sys.exit("--steps must be at least 1")
+    if a.dump_outputs and (a.gpus != 1 or a.impl != "ours" or a.config not in ("head", "olat") or a.decoder
+                           or a.decoder_library or a.ext_compare):
+        sys.exit("--dump-outputs: supported for the single-GPU head and olat configs of --impl ours")
     if a.decoder_library:
         run_decoder_library(a)
     elif a.decoder:

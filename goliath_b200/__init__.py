@@ -1,4 +1,4 @@
-"""goliath_b200 — B200-native (sm_100a) implementation of the goliath avatar render hot path.
+"""goliath_b200 — H100-native (sm_90a) implementation of the goliath avatar render hot path.
 
 Public surface (mirrors the reference's extension modules, SURVEY.md §8b):
   goliath_b200.sgutilslib / sgutils        — SG specular shade       (extensions/sgutils)

@@ -1,7 +1,7 @@
 """ctypes binding of libgoliath_b200.so — the thin C-ABI extension (include/goliath_b200.h).
 
 The product path has NO CPU fallback: if the CUDA library is missing, or a tensor is not on a CUDA
-device, every op raises.  Build with `python -m goliath_b200.build` (nvcc, sm_100a).
+device, every op raises.  Build with `python -m goliath_b200.build` (nvcc, sm_90a).
 """
 import ctypes
 import os

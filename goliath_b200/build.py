@@ -1,7 +1,7 @@
-"""In-tree build of libgoliath_b200.so: every CUDA translation unit compiled for sm_100a with nvcc.
+"""In-tree build of libgoliath_b200.so: every CUDA translation unit compiled for sm_90a with nvcc.
 
 `python -m goliath_b200.build` (or `__graft_entry__.build()`).  nvcc cross-compiles without a GPU; the
-resulting .so is git-ignored but travels with the repo snapshot to the GPU box.
+resulting .so is git-ignored.
 """
 import os
 import subprocess
@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libgoliath_b200.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 # per-file extra flags.  splat_project.cu carries the bit-exact binning contract: no FMA contraction.
 # sg_shade.cu mirrors the reference extension's own flag (extensions/sgutils/setup.py:31) for last-bit parity.

@@ -1,4 +1,4 @@
-// goliath_b200/csrc/common.cuh — shared device/host helpers for the sm_100a kernels.
+// goliath_b200/csrc/common.cuh — shared device/host helpers for the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -24,7 +24,7 @@ namespace gb {
 extern unsigned long long g_launch_count;
 inline void count_launches(int n) { __atomic_fetch_add(&g_launch_count, (unsigned long long)n, __ATOMIC_RELAXED); }
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 __host__ __device__ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }

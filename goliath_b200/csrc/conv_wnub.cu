@@ -1,5 +1,5 @@
 // goliath_b200/csrc/conv_wnub.cu — stride-1 KxK (K = 1 | 3, "same" padding) convolution with the reference's
-// weight-norm scale, tied or untied bias and LeakyReLU fused into the epilogue (sm_100a), forward and backward.
+// weight-norm scale, tied or untied bias and LeakyReLU fused into the epilogue (sm_90a), forward and backward.
 //
 // This is the layer the hand-MVP decoders are made of besides the transposed convolutions:
 //   TransDecoder       5 x la.Conv2dWNUB(.., 64, 64, 3, 1, 1) + LeakyReLU(0.2)   ca_code/models/hand_mvp.py:297-321

@@ -1,5 +1,5 @@
 // goliath_b200/csrc/deconv_wnub.cu — stride-2 4x4 transposed convolution with weight-norm scale, untied
-// (per-pixel) bias and LeakyReLU fused into the epilogue (sm_100a), forward.
+// (per-pixel) bias and LeakyReLU fused into the epilogue (sm_90a), forward.
 //
 // Replaces, for the layer type every RGCA / hand-MVP decoder tower is made of
 // (make_conv_trans(.., 4, 2, 1, "wn", LeakyReLU(0.2), ub=(H,W)), ca_code/models/rgca.py:408-456,
@@ -10,8 +10,8 @@
 //
 // Round-1 implementation: fp32 SIMT with the sub-pixel (4-phase) decomposition — each thread owns one input
 // position, i.e. a 2x2 output quad, for 8 output channels (32 accumulators); the 3x3 input neighbourhood and the
-// 8x16 weights of the current input channel come from shared memory (weights as broadcast float4).  The tcgen05
-// phase-GEMM version (TF32x3, TMA-fed) is the planned successor (DESIGN.md §7); the last layers are bound by the
+// 8x16 weights of the current input channel come from shared memory (weights as broadcast float4).  The tensor-core
+// phase-GEMM version (3xTF32, TMA-fed: csrc/deconv_tc.cu) serves the inference forward; the last layers are bound by the
 // untied-bias + output traffic (1.07 GB for 16->125 @1024^2), not by FLOPs.
 #include <cstdlib>
 #include <cstring>
@@ -113,11 +113,11 @@ __global__ void __launch_bounds__(TQ* TQ) deconv4x4s2_fwd_kernel(
 
 // ---------------------------------------------------------------------------------------------------------------
 // Wide variant for the high-resolution layers (Cin <= 32: 32->16 @512^2, 16->125 @1024^2 in the RGCA towers, every
-// layer of the hand-MVP content decoders).  ncu on the kernel above at 16->125 @1024^2: 720 M warp instructions for
-// 262 M FFMA-equivalents (shared-memory operand loads, per-co-block input re-staging), 1.07 ms, 13 % of DRAM peak,
-// and the epilogue's untied-bias loads sit exposed at the end of every CTA.  Here:
+// layer of the hand-MVP content decoders).  At 16->125 @1024^2 the kernel above spends most of its instructions on
+// shared-memory operand loads and per-co-block input re-staging rather than FMAs, and the epilogue's untied-bias loads
+// sit exposed at the end of every CTA.  Here:
 //  * a thread owns TWO horizontally adjacent quads (4 consecutive output columns x 2 rows -> 16-byte bias loads/stores);
-//  * output channels are processed in PAIRS with the packed FFMA2 instruction (fma.rn.f32x2): the x operand is stored
+//  * output channels are processed in PAIRS (ffma2 below): the x operand is stored
 //    duplicated in shared memory, the weights as [ci][tap][co] so that a channel pair is one 64-bit operand;
 //  * the input tile is staged once per CTA and reused for several blocks of output channels;
 //  * the bias of a block is loaded into registers BEFORE its FMA loop (4 channels per block keep that affordable)
@@ -126,9 +126,15 @@ constexpr int WQ_X = 32, WQ_Y = 16;       // input positions per CTA: 16 rows x 
 constexpr int W_CO = 4, W_CI = 16;
 constexpr int W_HX = WQ_X + 2, W_HY = WQ_Y + 2, W_HS = 36;  // halo tile; row stride in float2 (rows 16-byte aligned)
 
+// Hopper has no packed fma.rn.f32x2: a channel pair is two scalar fma.rn on the halves of the 64-bit operands (the
+// same rounding, so the results are identical to the packed form)
 __device__ __forceinline__ unsigned long long ffma2(unsigned long long a, unsigned long long b, unsigned long long c) {
   unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
+  asm("{\n\t.reg .f32 a0, a1, b0, b1, c0, c1;\n\t"
+      "mov.b64 {a0, a1}, %1;\n\tmov.b64 {b0, b1}, %2;\n\tmov.b64 {c0, c1}, %3;\n\t"
+      "fma.rn.f32 c0, a0, b0, c0;\n\tfma.rn.f32 c1, a1, b1, c1;\n\t"
+      "mov.b64 %0, {c0, c1};\n\t}"
+      : "=l"(d) : "l"(a), "l"(b), "l"(c));
   return d;
 }
 __device__ __forceinline__ void cp_async4_zfill(void* smem, const void* gmem, bool valid) {
@@ -315,7 +321,7 @@ GB_API int gb_deconv4x4s2_wnub_fwd(int B, int Cin, int Cout, int Hi, int Wi, con
                                    void* stream) {
   if (B <= 0 || Cin <= 0 || Cout <= 0 || Hi <= 0 || Wi <= 0) return 0;
   if (Cin <= 32 && Wi % 2 == 0 && Wi >= 32 && Hi >= 16) {
-    // high-resolution layers: wide FFMA2 kernel, several blocks of output channels per staged input tile
+    // high-resolution layers: wide kernel, several blocks of output channels per staged input tile
     const int tiles = gb::cdiv(Hi, WQ_Y) * gb::cdiv(Wi, WQ_X);
     const int nblk = gb::cdiv(Cout, W_CO);
     int per_cta = 1;  // grow while the grid still fills the machine a few times over
@@ -506,9 +512,9 @@ __global__ void __launch_bounds__(256) deconv4x4s2_bwd_weight_kernel(
 // Wide backward kernels for the high-resolution layers (Cin <= 32, the same layers as the wide forward).  The two
 // kernels above move one shared-memory operand per 2.7 (data) / 3.2 (weight) FMAs and re-stage the gz tile with scalar
 // loads; at 16->125 @1024^2 the layer's backward is 8.4 G FMA each way over a 524 MB gradient.  Here:
-//  data:   a thread owns TWO horizontally adjacent input positions x 16 input channels in FFMA2 pairs (32 sums in 16
+//  data:   a thread owns TWO horizontally adjacent input positions x 16 input channels in FMA pairs (32 sums in 16
 //          64-bit registers); per output channel it reads its 4x6 window of gz (3 loads per row) once, and every 16-byte
-//          weight load (two channel pairs of one tap) feeds 4 FFMA2.  gz tiles (4 output channels x 34 x 66, 16-byte
+//          weight load (two channel pairs of one tap) feeds 4 FMA pairs.  gz tiles (4 output channels x 34 x 66, 16-byte
 //          cp.async for the interior, zero-filled halo) and the weights are double-buffered.
 //  weight: lane = (4 input channels, 1 output channel, 16 taps) as above, but a step covers TWO adjacent positions: the
 //          6-wide gz rows are shared between them (12 loads + 4 x-pair loads for 128 FMAs), tiles are staged with
@@ -643,8 +649,8 @@ constexpr int WW_CO = 8, WW_CI = 16;
 constexpr int WW_GY = 2 * WW_Y + 2;                // 18 gz rows
 constexpr int WW_XS = 36;                          // x row stride in floats (32 + pad, rows 16-byte aligned)
 // plane strides = 16 bytes mod 128: the 4 channel groups (x, 8-byte loads) and the 8 output channels (gz, 16-byte loads)
-// that the lanes of a warp address in one instruction then fall into distinct banks.  (First version: strides of 0 / 64
-// bytes mod 128, 4-way conflicts on every operand load, 1.35 ms for the two wide layers.)
+// that the lanes of a warp address in one instruction then fall into distinct banks (strides of 0 / 64 bytes mod 128
+// would give 4-way conflicts on every operand load).
 constexpr int WW_XP = WW_Y * WW_XS + 4;            // 292 floats
 constexpr int WW_GP = WW_GY * DW_GS + 20;          // 1316 floats
 constexpr int WW_XBYTES = WW_CI * WW_XP * 4;              // 18688

@@ -1,4 +1,4 @@
-// goliath_b200/csrc/envmap_spec.cu — environment-map specular branch of the RGCA PrimDecoder (sm_100a).
+// goliath_b200/csrc/envmap_spec.cu — environment-map specular branch of the RGCA PrimDecoder (sm_90a).
 //
 // Replaces /root/reference/ca_code/models/rgca.py:548-556 (run_vis_relight.py's second loop, EnvSpinDecorator):
 //   ref_dirs = einsum("bxy,bny->bnx", lightrot, ref_dirs)                       rotate the reflection vector

@@ -1,4 +1,4 @@
-// goliath_b200/csrc/geom_uv.cu — mesh front end of the decoders: vertex normals and vertex -> UV gather (sm_100a).
+// goliath_b200/csrc/geom_uv.cu — mesh front end of the decoders: vertex normals and vertex -> UV gather (sm_90a).
 // SURVEY.md section 8f-4.  Replaces ca_code/utils/geom.py:308-346 as called by rgca.PrimDecoder.forward
 // (ca_code/models/rgca.py:478-491: postex = to_uv(geom); tn = normalize(to_uv(vn(geom)))):
 //   vert_normals   face normals (cross product, normalised with clamp(min=eps)) scatter-added to their three vertices,

@@ -1,4 +1,4 @@
-// goliath_b200/csrc/mvp_prims.cu — the two glue stages between the hand-MVP decoders and the raymarcher (sm_100a):
+// goliath_b200/csrc/mvp_prims.cu — the two glue stages between the hand-MVP decoders and the raymarcher (sm_90a):
 //
 //  1. slab -> primitive templates.  The reference turns the decoders' UV slabs into the raymarcher's template with
 //     five full-size passes: relu(25*rgb+100) (hand_mvp.py:472), relu(alpha) (:434), cat (:172), the

@@ -1,5 +1,5 @@
 // goliath_b200/csrc/mvp_raymarch.cu — Mixture-of-Volumetric-Primitives raymarcher, fwd + bwd, and the
-// fixed-order BVH bounds (sm_100a).
+// fixed-order BVH bounds (sm_90a).
 //
 // Replaces the reference extension extensions/mvpraymarch:
 //   raymarch_subset_forward_kernel   mvpraymarch_subset_kernel.h:7-112
@@ -13,7 +13,7 @@
 // the reference kernels to the last bits; the launch geometry (block (bx,by), 32 consecutive linear thread ids
 // per warp, edge threads clamped) is kept because hit lists are per-warp unions.
 //
-// What is different (B200 design):
+// What is different:
 //  * every hit primitive carries the warp-level [t_in, t_out] of its box; while marching, a primitive is
 //    touched only when the warp's current t-window overlaps that interval (warp-uniform test, no ballot), so
 //    the per-step cost follows the primitives actually overlapping the sample, not the whole hit list;
@@ -369,8 +369,8 @@ __global__ void raymarch_fwd_kernel(RMArgs a) {
 }
 
 // ------------------------------------------------------------------ forward, lane-compacted sampling (algo 0, no shadow)
-// ncu on the kernel above (profiles/r01_raymarch_fwd_ncu.txt): the sampling block — fade (3 pow + exp), trilinear setup,
-// 8 corner loads — runs with 6 of 32 lanes active, because a primitive overlaps only a few rays of the warp's 8x4
+// In the kernel above the sampling block — fade (3 pow + exp), trilinear setup, 8 corner loads — runs with few of the
+// 32 lanes active, because a primitive overlaps only a few rays of the warp's 8x4
 // footprint at a given step.  Here the warp ENQUEUES the (ray, primitive) pairs that are inside a primitive (local
 // coordinate + primitive id, compacted with a ballot) and SAMPLES them 32 at a time with every lane busy, whichever
 // ray or primitive an item belongs to; the results are then APPLIED in the original order — group by group (one group =
@@ -837,10 +837,11 @@ __global__ void __launch_bounds__(256) compute_aabb_kernel(int N, int K, const f
 }
 
 // bit 0: lane-compacted sampling queue in the forward march, bit 1: in the backward march (algo 0, no shadow splat).
-// Default 2 = queue in the BACKWARD only, from measurement on B200 (profiles/r02_bench_hand_mvp*.json): the backward, whose
-// per-item block carries the template-gradient REDs and the fade / position gradients, gains (9.9 -> 8.3 ms at config 4);
-// the forward is SLOWER with the queue (6.0 vs 5.0 ms at config 4, 17.3 vs 15.8 ms at config 5) — it is bound by
-// dependent-load latency (BVH walk, template corners), not by issue slots, and the queue adds shared-memory round trips.
+// Default 2 = queue in the BACKWARD only, from measurement: bench.py --config hand_mvp (decode + raymarch fwd+bwd) on an
+// H100 SXM at a 400 W power limit, two runs each: queue in the backward 34.72 / 34.72 ms per step, no queue 37.85 /
+// 37.96, both 35.65 / 35.90, forward only 38.94 / 38.93.  The backward, whose per-item block carries the template-gradient
+// REDs and the fade / position gradients, gains; the forward does not — it is bound by dependent-load latency (BVH walk,
+// template corners), not by issue slots, and the queue adds shared-memory round trips.
 int g_raymarch_mode = -1;
 int raymarch_mode() {
   if (g_raymarch_mode < 0) {
@@ -877,7 +878,7 @@ GB_API int gb_mvp_compute_aabb(int N, int K, const float* primpos, const float* 
   if (N <= 0 || K <= 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
   GB_CUDA(cudaMemsetAsync(workspace, 0, gb_mvp_aabb_workspace_bytes(N, K), s));
-  const int blocks = min(gb::cdiv(N * K, 256), 148 * 8);
+  const int blocks = min(gb::cdiv(N * K, 256), gb::kNumSMs * 8);
   compute_aabb_kernel<<<blocks, 256, 0, s>>>(N, K, primpos, primrot, primscale, sortedobjid, (const int2*)nodechildren,
                                              nodeparent, nodeaabb, (int*)workspace);
   gb::count_launches(1);

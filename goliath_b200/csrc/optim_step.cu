@@ -1,4 +1,4 @@
-// goliath_b200/csrc/optim_step.cu — gradient hygiene + global-norm clip + Adam/AdamW over a parameter list (sm_100a).
+// goliath_b200/csrc/optim_step.cu — gradient hygiene + global-norm clip + Adam/AdamW over a parameter list (sm_90a).
 // SURVEY.md section 8f-3.  Replaces, per train step, ca_code/utils/train.py:209-215
 //     p.grad[isnan(p.grad)] = 0; p.grad[isinf(p.grad)] = 0        (two masked writes per tensor)
 //     torch.nn.utils.clip_grad_norm_(params, 1.0)                 (norm pass + scale pass)

@@ -1,4 +1,4 @@
-// goliath_b200/csrc/photo_loss.cu — post-render chain + photometric losses of the RGCA train step, fused (sm_100a).
+// goliath_b200/csrc/photo_loss.cu — post-render chain + photometric losses of the RGCA train step, fused (sm_90a).
 // SURVEY.md section 8f-2.  Replaces, per frame, the eager chain
 //   rgb = cal(rgb, cam)                          ca_code/nn/color_cal.py:211-241  (CalV5: w * img + b; grey cameras: sum_c)
 //   rgb = rgb + (1 - alpha) * bg                 ca_code/models/rgca.py:226-230

@@ -1,4 +1,4 @@
-// goliath_b200/csrc/raydirs.cu — camera rays + unit-cube slab interval (sm_100a).
+// goliath_b200/csrc/raydirs.cu — camera rays + unit-cube slab interval (sm_90a).
 //
 // Replaces the reference kernel extensions/utils/utils_kernel.cu:11-51 (compute_raydirs_forward_kernel) behind
 // utilslib.compute_raydirs_forward (extensions/utils/utils.cpp:46-82).  Pure bandwidth: 8 B in / 32 B out per

@@ -1,4 +1,4 @@
-// goliath_b200/csrc/render_finish.cu — post-processing of one rendered view, one kernel each way (sm_100a).
+// goliath_b200/csrc/render_finish.cu — post-processing of one rendered view, one kernel each way (sm_90a).
 //
 // Replaces the ~20 small PyTorch kernels (and their autograd twins) of rgca.AutoEncoder.render after the rasteriser
 // (ca_code/models/rgca.py:136-151 with ca_code/utils/render_gsplat.py:79-108): HWC -> CHW of the colour image,

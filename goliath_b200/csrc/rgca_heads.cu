@@ -1,4 +1,4 @@
-// goliath_b200/csrc/rgca_heads.cu — RGCA Gaussian heads + SH diffuse + reflection direction, fused (sm_100a).
+// goliath_b200/csrc/rgca_heads.cu — RGCA Gaussian heads + SH diffuse + reflection direction, fused (sm_90a).
 //
 // Replaces the ~60 eager element-wise PyTorch ops of PrimDecoder.forward,
 // /root/reference/ca_code/models/rgca.py:506-546 (row R2 of SURVEY.md §8a; channel map SURVEY.md Appendix C),

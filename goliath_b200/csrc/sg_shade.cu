@@ -1,9 +1,9 @@
-// goliath_b200/csrc/sg_shade.cu — spherical-Gaussian specular shade, forward + backward (sm_100a).
+// goliath_b200/csrc/sg_shade.cu — spherical-Gaussian specular shade, forward + backward (sm_90a).
 //
 // Replaces the reference kernels extensions/sgutils/sg.cu:27-76 (fwd) and :78-175 (bwd) behind the
 // same argument meaning (C ABI in include/goliath_b200.h: gb_sg_evaluate_fwd / gb_sg_evaluate_bwd).
 //
-// Design (B200): one thread per Gaussian, the batch item's light table (position + value, 24 B/light)
+// Design: one thread per Gaussian, the batch item's light table (position + value, 24 B/light)
 // staged once per CTA in shared memory in chunks of kLightChunk, so the inner loop reads lights as
 // conflict-free broadcasts instead of the reference's per-pair global loads.  For L >= 4 the kernel is
 // FP32/SFU bound (acos + ex2 + rsqrt per pair), for L <= 2 it is a streaming HBM kernel (40 B in,

@@ -1,4 +1,4 @@
-// goliath_b200/csrc/splat_bin.cu — tile binning for the splat rasteriser (sm_100a):
+// goliath_b200/csrc/splat_bin.cu — tile binning for the splat rasteriser (sm_90a):
 //   inclusive int32 scan of num_tiles_hit -> (tile<<32 | depth-bits) intersection keys ->
 //   stable LSD radix sort of (u64 key, i32 Gaussian id) -> per-tile [first,last) bin edges.
 //
@@ -12,7 +12,7 @@
 // ceil(log2(#tiles))), and passes whose digit is identical for every key are skipped (typical for the
 // top depth byte).  Each pass = per-CTA digit histogram -> single-CTA exclusive scan over the
 // (digit-major) histogram table -> stable scatter with warp match-any ranking.  Everything stays in
-// the 126 MB L2 at the sizes of this path (1 M keys = 12 MB).
+// the 50 MB L2 at the sizes of this path (1 M keys = 12 MB).
 #include "common.cuh"
 
 namespace {

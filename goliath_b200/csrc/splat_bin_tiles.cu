@@ -1,4 +1,4 @@
-// goliath_b200/csrc/splat_bin_tiles.cu — tile binning for the fused render path, B200 formulation (sm_100a).
+// goliath_b200/csrc/splat_bin_tiles.cu — tile binning for the fused render path, sm_90a.
 //
 // Produces exactly what the key sort of csrc/splat_bin.cu produces for the fused render — per-tile
 // [first,last) bins, the Gaussian ids of every tile in front-to-back order (ties: ascending id), and the
@@ -10,7 +10,7 @@
 //                            intersection COUNT of every visible Gaussian.  Counts are privatised per CTA in
 //                            shared memory and flushed with one RED per (CTA, non-empty tile): the hot tiles
 //                            of a head scene take ~2000 hits each, which serialise on the L2 atomic unit when
-//                            issued one by one (measured: 118 us with one global RED per pair, 8 us privatised).
+//                            issued one by one.
 //   2. rank_scatter_kernel   x4: stable LSD radix sort of the G depth keys (8-bit digits).  One kernel per
 //                            pass: a CTA derives its own scatter bases from the per-CTA histogram table
 //                            (column prefix read from L2) and accumulates the NEXT pass's table with global
@@ -300,8 +300,8 @@ __global__ void __launch_bounds__(kRankBlock) rank_scatter_kernel(
 
 
 // ------------------------------------------------------------------ 2b. the whole rank sort as ONE cooperative kernel
-// Round-1 launch list (profiles/r01_launches_pipe.txt): 4 x 17-19 us for the four radix passes over 300k keys, each
-// a chain of L2 round trips at ~9 % issue utilisation with a kernel boundary in between.  Here the passes run inside
+// As separate launches, the four radix passes over 300k keys are each a chain of L2 round trips at low issue
+// utilisation with a kernel boundary in between.  Here the passes run inside
 // one cooperative launch (grid <= SM count, every CTA co-resident), separated by a grid barrier (an L2 counter), and
 // only the low bits in which the keys actually differ are sorted: depths of a head at ~1 m share their sign,
 // exponent and leading mantissa bits, so 3 passes (or 2) replace 4 and no launch gap remains.  Data written by other
@@ -377,7 +377,7 @@ __global__ void __launch_bounds__(kRankBlock) rank_sort_coop_kernel(
     // ---- phase A (passes > 0; pass 0's table was written by depth_keys_kernel): this pass's digit histogram of every
     // tile, from the keys as the previous pass left them.  No global atomics: round 2's first version accumulated the
     // next table with one RED per key while scattering, and the concentrated top digit of a head's depths put hundreds of
-    // REDs on the same address per tile (ncu: 6 % issue-active, 18 us per pass).
+    // REDs on the same address per tile.
     if (p > 0) {
       for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         const int warp_base = tile * kTile + warp * (32 * kItems);
@@ -469,11 +469,10 @@ __global__ void __launch_bounds__(kRankBlock) rank_sort_coop_kernel(
 }
 
 // ------------------------------------------------------------------ 2c. depth ranks by buckets (option, measured slower)
-// MEASURED (profiles/r02_launches_head_buckets.txt): steps (1)-(3) below take 8 + 5 + 12 us, but step (4), the n^2 in-bucket
-// ranking, executes 25.6 M warp instructions and takes 65 us at 300 k keys -- the cooperative sort stays the default; the
-// code is kept for GOLIATH_B200_RANKSORT=buckets and as the tested fallback protocol (device flag -> cooperative sort).
-// The idea: the cooperative LSD sort above is latency-bound: 147 CTAs of 8 warps walk 3 passes of dependent L2 round trips and
-// grid barriers (ncu: 6 % issue-active, 44 us for 300 k keys).  The ranks only have to order the VISIBLE Gaussians
+// Step (4) below, the n^2 in-bucket ranking, costs more than it saves on the bench scene (measurements at
+// rank_sort_mode below), so it is not the default; the code is kept for GOLIATH_B200_RANKSORT=buckets and as the tested fallback protocol (device flag -> cooperative sort).
+// The idea: the cooperative LSD sort above is latency-bound: one CTA per SM walks 3 passes of dependent L2 round trips
+// and grid barriers.  The ranks only have to order the VISIBLE Gaussians
 // by (depth bits, id), so: (1) the visible keys are dealt into 2048 buckets that split [min key, max key] evenly
 // (monotone in the key: bucket order == depth order), counts privatised per CTA; (2) one CTA scans the counts;
 // (3) the (key, id) pairs are scattered into their bucket (slots claimed per CTA, order inside a bucket arbitrary);
@@ -770,7 +769,7 @@ __global__ void __launch_bounds__(kSortThreads, 3) tile_sort_pack_kernel(
 // ------------------------------------------------------------------ 5b. the same in two kernels (default)
 // tile_sort_pack_kernel is bound by its heaviest tiles: one CTA walks bitmap clear -> bucket loads -> popcount scan ->
 // rank write-out -> rank read-back -> gid load -> 48-byte record gather -> store, eight dependent global round trips
-// per tile (profiles/r02_launches_head.txt: 51 us against ~12 us of traffic).  Split: the per-tile kernel stops after
+// per tile, far longer than its traffic needs.  Split: the per-tile kernel stops after
 // writing the SORTED RANKS in place over the tile's bucket; a grid-wide kernel then turns every intersection's rank
 // into its Gaussian id and its record, three threads per record (48 B = 3 x 16 B), fully parallel over the 1.08 M
 // intersections whatever the tile lengths are.
@@ -869,8 +868,9 @@ inline Layout make_layout(int G, int T, int64_t cap) {
   return l;
 }
 
-// 1: the four radix passes as separate launches (round 1), 0: one cooperative kernel (default), 2: 2048 key buckets +
-// in-bucket n^2 ranking (measured slower: 65 us for the in-bucket pass at 300k, profiles/r02_launches_head_buckets.txt).
+// 1: the four radix passes as separate launches (default), 0: one cooperative kernel, 2: 2048 key buckets + in-bucket
+// n^2 ranking.  bench.py (head config, 300k Gaussians) on an H100 SXM at a 400 W power limit, two runs each: passes
+// 0.596 / 0.597 ms per step, cooperative 0.605 / 0.606, buckets 0.609 / 0.610.
 // GOLIATH_B200_RANKSORT=passes|coop|buckets
 int g_tile_sort_mode = -1;  // 0: per-tile bitmap sort + grid-wide record gather (default), 1: one kernel per tile (round 1)
 int tile_sort_mode() {
@@ -880,11 +880,11 @@ int tile_sort_mode() {
   }
   return g_tile_sort_mode;
 }
-int g_rank_sort_mode = -1;  // 0: cooperative LSD sort, 1: four separate radix passes (round 1), 2: bucket ranking (+ fallback)
+int g_rank_sort_mode = -1;  // 0: cooperative LSD sort, 1: four separate radix passes, 2: bucket ranking (+ fallback)
 int rank_sort_mode() {
   if (g_rank_sort_mode < 0) {
     const char* e = getenv("GOLIATH_B200_RANKSORT");
-    g_rank_sort_mode = !e ? 0 : strcmp(e, "passes") == 0 ? 1 : strcmp(e, "buckets") == 0 ? 2 : 0;
+    g_rank_sort_mode = !e ? 1 : strcmp(e, "coop") == 0 ? 0 : strcmp(e, "buckets") == 0 ? 2 : 1;
   }
   return g_rank_sort_mode;
 }

@@ -1,11 +1,11 @@
-// goliath_b200/csrc/splat_blend.cu — per-tile alpha blending of sorted 2-D Gaussians, fwd + bwd (sm_100a).
+// goliath_b200/csrc/splat_blend.cu — per-tile alpha blending of sorted 2-D Gaussians, fwd + bwd (sm_90a).
 //
 // Replaces (third-party, absent from the reference tree) gsplat 0.1.11 rasterize_forward /
 // rasterize_backward_kernel as called from ca_code/utils/render_gsplat.py:65-78 (rgb) and :90-104
 // (depth-as-colour); semantics restated in SURVEY.md Appendix A and oracle/splat_oracle.c.
 //
 // One CTA per 16x16 tile (block_width <= 16 supported; CTA = roundup(bw*bw, 32) threads).
-// B200 design points:
+// Design points:
 //  * each warp owns a compact 8x4 pixel footprint (bw == 16), so "all lanes done" / "no lane hit"
 //    tests prune far more often than with the reference's 16x2 rows;
 //  * a batch of Gaussians (position, conic, opacity AND colours) is gathered once per CTA into shared

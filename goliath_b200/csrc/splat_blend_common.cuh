@@ -107,8 +107,8 @@ __device__ __forceinline__ float reduce10(const float (&v)[10], int lane, int& s
 //  sched == 1: `order` is a schedule written by gb_tile_schedule: position k*Q + q is the k-th item of queue q
 //  (Q = kSchedQueues = SM count), Q draw counters and a draw count follow at order[T ..].  The CTA draws the
 //  next item of the queue of the SM it runs on, so an SM blends the tiles of ITS queue whatever the block
-//  scheduler does, and the queues were filled with near-equal work (ncu on the launch-order kernels:
-//  sm__cycles_active.avg is only ~70 % of the elapsed cycles, the SMs finish far apart).  A CTA whose queue
+//  scheduler does, and the queues were filled with near-equal work (with the plain launch order the SMs can finish far
+//  apart).  A CTA whose queue
 //  is exhausted takes from the following queues (a grid of T CTAs draws exactly T items, one scan finds
 //  one), and the launch's last draw puts the counters back to zero for the next launch on this schedule.
 __device__ __forceinline__ int draw_tile(const int* order, int sched, int T) {

@@ -1,11 +1,10 @@
-// goliath_b200/csrc/splat_blend_mom.cu — third formulation of the packed blend (sm_100a), blend mode 3 (default).
+// goliath_b200/csrc/splat_blend_mom.cu — third formulation of the packed blend (sm_90a), blend mode 3 (default).
 //
 // Same records, same per-(pixel, Gaussian) arithmetic in the forward and the same gradients as
 // csrc/splat_blend_pipe.cu (gsplat 0.1.11 rasterize_forward / rasterize_backward_kernel, call sites
-// ca_code/utils/render_gsplat.py:65-78,90-104).  Round-1 ncu/SASS of the pipeline kernels (profiles/
-// r01_blend_pipe_ncu.txt, DESIGN.md section 4) showed both directions bound by the per-warp issue rate on the
-// heaviest tile: ~0.125 IPC per warp on a dependent chain of LDS -> FMA -> ex2 -> shuffles -> shared-memory CAS
-// atomics, 163 instructions per footprint hit in the backward.  What changes here:
+// ca_code/utils/render_gsplat.py:65-78,90-104).  The pipeline kernels are bound in both directions by the per-warp
+// issue rate on the heaviest tile: a dependent chain of LDS -> FMA -> ex2 -> shuffles -> shared-memory CAS atomics
+// per footprint hit in the backward.  What changes here:
 //
 //  cull      the 32-lane record test is the exact minimum of the Gaussian's quadratic form over the warp's 8x4
 //            pixel rectangle (a convex QP on a box: the minimiser lies on one of the two faces visible from the
@@ -234,9 +233,9 @@ __global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
       for (;;) {
         if (mbar_try(&s_full[s], par)) { st = 1; break; }
         if (all_done && *ndone >= kPixelWarps) { st = 2; break; }
-        // (ncu, profiles/r02_fwd_spin.txt: 25 % of this kernel's executed instructions are these single-lane probes, most
-        // of them saturated warps waiting at the producer's frontier.  Parking them with __nanosleep(32 / 200 ns) was
-        // measured SLOWER, 79.5 vs 74 us: the probes use issue slots nobody else wants, the wake-up latency is real.)
+        // (many of this kernel's executed instructions are these single-lane probes, mostly saturated warps waiting
+        // at the producer's frontier.  They are not parked with __nanosleep: the probes use issue slots nobody else
+        // wants, while the wake-up latency of a parked warp lands on the critical path.)
       }
     }
     st = __shfl_sync(0xffffffffu, st, 0);
@@ -770,9 +769,9 @@ __global__ void __launch_bounds__(kFwdThreads) blend_fwd_multi_kernel(
       for (;;) {
         if (mbar_try(&s_full[s], par)) { st = 1; break; }
         if (all_done && *ndone >= kPixelWarps) { st = 2; break; }
-        // (ncu, profiles/r02_fwd_spin.txt: 25 % of this kernel's executed instructions are these single-lane probes, most
-        // of them saturated warps waiting at the producer's frontier.  Parking them with __nanosleep(32 / 200 ns) was
-        // measured SLOWER, 79.5 vs 74 us: the probes use issue slots nobody else wants, the wake-up latency is real.)
+        // (many of this kernel's executed instructions are these single-lane probes, mostly saturated warps waiting
+        // at the producer's frontier.  They are not parked with __nanosleep: the probes use issue slots nobody else
+        // wants, while the wake-up latency of a parked warp lands on the critical path.)
       }
     }
     st = __shfl_sync(0xffffffffu, st, 0);

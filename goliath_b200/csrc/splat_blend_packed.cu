@@ -1,4 +1,4 @@
-// goliath_b200/csrc/splat_blend_packed.cu — the B200 blend path: packed per-intersection records streamed
+// goliath_b200/csrc/splat_blend_packed.cu — the packed blend path: packed per-intersection records streamed
 // with bulk async copies (TMA, cp.async.bulk + mbarrier), warp-level footprint culling, LPT tile order.
 //
 // Same arithmetic per (pixel, Gaussian) pair as csrc/splat_blend.cu (which restates gsplat 0.1.11
@@ -14,8 +14,8 @@
 //     instructions, the next batch is in flight while the current one is blended.
 //  3. each warp owns an 8x4 pixel footprint.  32 lanes test 32 records' boxes against the footprint in
 //     one step (ballot), then the warp walks only the set bits in order.  At the RGCA operating point
-//     (3-sigma radius ~6 px) this removes ~60 % of the per-pixel tests of the reference formulation, which
-//     ncu showed to be issue-bound, not HBM-bound (profiles/r01_blend_v1_ncu.txt).
+//     (3-sigma radius ~6 px) this removes most of the per-pixel tests of the reference formulation, which
+//     is issue-bound, not HBM-bound.
 //  4. tiles are launched longest-list-first (gb_tile_order), so the tail of the grid is made of short tiles.
 //  5. backward: the 10 per-Gaussian partial sums are reduced across the warp with a recursive-halving
 //     exchange (12 shuffles instead of 50), accumulated per CTA in shared memory, and flushed with one set

@@ -1,11 +1,9 @@
-// goliath_b200/csrc/splat_blend_pipe.cu — warp-decoupled formulation of the packed blend (sm_100a).
+// goliath_b200/csrc/splat_blend_pipe.cu — warp-decoupled formulation of the packed blend (sm_90a).
 //
 // Same records, same per-(pixel, Gaussian) arithmetic and same outputs as csrc/splat_blend_packed.cu (which
 // restates gsplat 0.1.11 rasterize_forward / rasterize_backward_kernel, call sites
 // ca_code/utils/render_gsplat.py:65-78,90-104); what changes is how the 8 pixel warps of a tile are
-// synchronised.  ncu on the CTA-synchronous kernels (profiles/r01_blend_packed_ncu.txt) shows the top stall
-// reason of both directions is the per-batch __syncthreads (3.9 warps parked at the barrier per issue-active
-// cycle): the warps of a tile see different numbers of footprint hits per batch, and every batch waits for
+// synchronised.  In the CTA-synchronous kernels the per-batch __syncthreads parks warps at the barrier: the warps of a tile see different numbers of footprint hits per batch, and every batch waits for
 // the slowest.  Here the warps never meet at a CTA barrier inside the walk:
 //
 //  forward   records stream through a 4-stage ring of 128-record (6 KB) buffers filled by cp.async.bulk.
@@ -24,8 +22,7 @@
 // order); gradients agree to the order of the floating-point atomics.
 //
 // Both kernels can also draw their tile from an SM-affine schedule (gb_tile_schedule, draw_tile below) instead of
-// taking order[blockIdx.x]; measured on the bench scene this does not beat the plain longest-first launch order
-// (DESIGN.md section 4), so it is an option (GOLIATH_B200_BLEND=affine), not the default.
+// taking order[blockIdx.x]; it is an option (GOLIATH_B200_BLEND=affine), not the default.
 #include <stdlib.h>
 #include <string.h>
 

@@ -1,4 +1,4 @@
-// goliath_b200/csrc/splat_project.cu — EWA projection of 3-D Gaussians, forward + backward (sm_100a).
+// goliath_b200/csrc/splat_project.cu — EWA projection of 3-D Gaussians, forward + backward (sm_90a).
 //
 // COMPILED WITH -fmad=false AND WITHOUT FAST-MATH: tile binning is a bit-exact contract
 // (BASELINE.json north_star), so every fp32 operation here is a single IEEE rounding in a fixed

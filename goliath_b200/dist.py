@@ -1,4 +1,4 @@
-"""View-sharded multi-GPU plumbing (SURVEY.md section 8e): one process per GPU, `torch.distributed` (NCCL on B200, gloo in
+"""View-sharded multi-GPU plumbing (SURVEY.md section 8e): one process per GPU, `torch.distributed` (NCCL on the GPUs, gloo in
 the CPU tests).  The path partitions by view — given the decoded Gaussians of a frame, project/bin/sort/blend of
 different views are independent — so the only exchange steps are a broadcast of the decoded table from the frame
 owner and a sum-reduction of its gradient.  The reference is single-GPU only (SURVEY.md section 2.4): nothing to match.

@@ -1,4 +1,4 @@
-"""Environment-map specular branch of the RGCA decoder (ca_code/models/rgca.py:548-556) as one sm_100a kernel each way
+"""Environment-map specular branch of the RGCA decoder (ca_code/models/rgca.py:548-556) as one sm_90a kernel each way
 (csrc/envmap_spec.cu): rotate the reflection vector by `lightrot`, `dir2uv` (ca_code/utils/envmap.py:284-292),
 `mipmap_grid_sample` of the pre-convolved pyramid at level `sigma * 5` (ca_code/utils/mipmap_sampler.py:13-66),
 `clamp(max=1) * spec_vis`.  Gradients: ref_dirs and spec_vis (the mip level is selected under no_grad upstream; the

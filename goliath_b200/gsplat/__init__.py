@@ -1,5 +1,5 @@
 """gsplat 0.1.11-compatible surface used by the reference (ca_code/utils/render_gsplat.py:10-11):
-`project_gaussians` and `rasterize_gaussians`, backed by hand-written sm_100a kernels.
+`project_gaussians` and `rasterize_gaussians`, backed by hand-written sm_90a kernels.
 
 gsplat is a third-party dependency that is not part of the reference tree; signatures and semantics are
 those of its 0.1.11 release as restated in SURVEY.md Appendix A.

@@ -23,8 +23,8 @@ BINNING = os.environ.get("GOLIATH_B200_BINNING", "buckets")
 SPLIT = os.environ.get("GOLIATH_B200_RENDER_SPLIT", "1") != "0"
 # records of the two-node path: "packed" (sorted 48-byte records materialised by the binning's gather, default) or "ranked"
 # (the blend stages records by depth rank from a per-Gaussian table with 16-byte cp.async gathers: the binning loses its
-# 31 us gather, but the forward goes from 74 to 132 us and the backward from 97 to 104 — measured, profiles/
-# r02_bench_head_ranked.json; kept as an option because it holds 4x less memory per view for the backward)
+# record gather, but the blend pays more for its scattered gathers; kept as an option because it holds 4x less memory
+# per view for the backward)
 RANKED = os.environ.get("GOLIATH_B200_RECORDS", "packed") == "ranked"
 
 

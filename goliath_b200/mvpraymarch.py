@@ -1,7 +1,7 @@
 """Host-side mirror of the reference wrapper extensions/mvpraymarch/mvpraymarch.py: `build_accel` (:21-84),
 `MVPRaymarch` (:87-311) and `mvpraymarch` (:314-418) with the same names, keyword arguments (ca_code/utils/
 render_raymarcher.py:59 introspects `mvpraymarch.__code__.co_varnames`), asserts and gradient wiring, calling the
-sm_100a kernels through `mvpraymarchlib`.
+sm_90a kernels through `mvpraymarchlib`.
 
 Differences that do not change results: the fixed-order heap topology (a function of N, K only) is cached per
 device instead of being rebuilt with torch ops on every call; bounds scratch is a cached workspace."""

@@ -3,7 +3,7 @@ checkpoints load (`weight_v`, `weight_g`, `bias`): `ConvTranspose2dWNUB`, `Linea
 `make_linear`.  Weight norm is the reference's non-standard one: g per output channel, norm of v over the WHOLE tensor
 (layers.py:200-204,468-480; SURVEY.md §0.6):  w = g * v / ||v||_F.
 
-The stride-2 4x4 transposed convolution + untied bias + LeakyReLU runs as ONE hand-written sm_100a kernel in the
+The stride-2 4x4 transposed convolution + untied bias + LeakyReLU runs as ONE hand-written sm_90a kernel in the
 forward, and its backward as three more (activation/bias gradient, data gradient, weight gradient) — no cuDNN
 (csrc/deconv_wnub.cu).  Round-1 status: fp32 SIMT kernels; LinearWN is a plain library GEMM (cuBLAS via F.linear)."""
 import math
@@ -262,7 +262,7 @@ def _tc_layer_ok(cin, cout):
 
 def tower_forward_tc(tower: nn.Sequential, x: torch.Tensor) -> torch.Tensor:
     """Inference forward of a deconv tower (Sequential of ConvTranspose2dWNUB [+ FusedLeakyReLU]) on the tensor cores
-    (csrc/deconv_tc.cu: tcgen05.mma kind::tf32 with 3xTF32 split, TMA-fed, TMEM accumulators).  Activations stay NHWC
+    (csrc/deconv_tc.cu: wgmma tf32 with 3xTF32 split, TMA-fed, register accumulators).  Activations stay NHWC
     (hi/lo split) between tensor-core layers (channels padded to 32, N padded to 16 inside the kernel); only layers
     with Cout > 256 would fall back to the SIMT kernel.
     No autograd: use the module's normal forward for training."""
@@ -276,8 +276,9 @@ def tower_forward_tc(tower: nn.Sequential, x: torch.Tensor) -> torch.Tensor:
         st = _lib.stream_ptr(dev)
         for i, layer in enumerate(layers):
             Cin, Cout = layer.in_channels, layer.out_channels
-            # measured on B200 (bench.py --decoder): with Cin = 16 the layer is pure output/bias bandwidth and the
-            # per-pixel NCHW epilogue of the tensor-core kernel loses to the SIMT kernel (4.2 vs 1.1 ms), so it stays SIMT
+            # with Cin = 16 the layer is pure output/bias bandwidth and the per-pixel NCHW epilogue of the tensor-core
+            # kernel loses to the SIMT kernel (bench.py decoder object, 16 -> 125 @ 1024^2 on an H100 SXM at 400 W:
+            # 0.92 ms SIMT, 1.05 ms tensor cores), so it stays SIMT
             tc_ok = _tc_layer_ok(Cin, Cout)
             nxt = layers[i + 1] if i + 1 < len(layers) else None
             nxt_tc = nxt is not None and _tc_layer_ok(nxt.in_channels, nxt.out_channels)

@@ -2,7 +2,7 @@
 (`render`) and of rgca.AutoEncoder.render's post-processing (ca_code/models/rgca.py:112-151).
 
 `render(...)` keeps the reference signature and call sequence (project, rasterise rgb, rasterise depth as
-colour) so that its results are comparable call-for-call; the kernels underneath are the sm_100a ones.
+colour) so that its results are comparable call-for-call; the kernels underneath are the sm_90a ones.
 """
 from typing import Optional
 
@@ -183,7 +183,7 @@ def render_views(width: int, height: int, K: th.Tensor, Rt: th.Tensor, preds, in
     if fused:
         # per view: one autograd node for project + bin/sort + pack + blend and one for the post-processing.  With several
         # views and the sync-free path the views are issued on a small pool of side streams (view_streams): independent
-        # views overlap on the device — one view's blend tail (SMs idle ~30 % of a blend launch) runs under the next
+        # views overlap on the device — one view's blend tail (SMs idle while the last tiles finish) runs under the next
         # view's projection / binning — and become parallel branches when the step is captured in a CUDA graph.
         from .gsplat.fused import render_fused
         rgbs, alphas, depths = [], [], []

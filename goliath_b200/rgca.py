@@ -1,4 +1,4 @@
-"""RGCA `PrimDecoder` (ca_code/models/rgca.py:372-620) assembled from the sm_100a pieces: the two 7-layer
+"""RGCA `PrimDecoder` (ca_code/models/rgca.py:372-620) assembled from the sm_90a pieces: the two 7-layer
 weight-normalised untied-bias deconv towers (rows R1, `goliath_b200.nn`), the fused Gaussian heads + SH diffuse
 (row R2, `goliath_b200.rgca_heads`) and the SG specular shade (row R3, `goliath_b200.sgutils`).
 
@@ -52,7 +52,7 @@ class PrimDecoder(nn.Module):
         gnn.glorot(self._last_deconv(self.vcond_mod), 1.0)
         rgb = color_mean / 255.0
         self.albedo = nn.Parameter((2.0 * rgb / 2.2974).permute(1, 2, 0).reshape(1, -1, 3))
-        # inference (no_grad) runs the towers on the tensor cores (tcgen05 + TMA, csrc/deconv_tc.cu); training uses
+        # inference (no_grad) runs the towers on the tensor cores (wgmma + TMA, csrc/deconv_tc.cu); training uses
         # the SIMT kernels that also provide the backward (csrc/deconv_wnub.cu)
         self.use_tensor_cores = True
 

@@ -1,5 +1,5 @@
 """Row R2 (SURVEY.md §8a): the Gaussian heads + SH diffuse + reflection direction block of the RGCA PrimDecoder
-(ca_code/models/rgca.py:506-546) and the colour compose (:557-575) as ONE fused sm_100a kernel per direction
+(ca_code/models/rgca.py:506-546) and the colour compose (:557-575) as ONE fused sm_90a kernel per direction
 (csrc/rgca_heads.cu) instead of ~60 eager element-wise kernels and a [B,G,3,81] temporary.
 
 `gaussian_heads(...)` returns a dict with the reference's `preds` key names and shapes (rgca.py:574-588);

@@ -1,6 +1,6 @@
 """Python surface of the SG specular shade with the names and argument meaning of the reference wrapper
 (extensions/sgutils/sgutils.py: `EvaluateGaussian` :17-63, `evaluate_gaussian` :65-98), written against the
-sm_100a kernels of csrc/sg_shade.cu (through `sgutilslib`).
+sm_90a kernels of csrc/sg_shade.cu (through `sgutilslib`).
 
 Contract kept from the reference: lobe directions are normalised in PyTorch so autograd owns that derivative
 (:74-75); only lobe_dirs, lobe_sigmas and light_values receive gradients — light_pts, prim_pts and n_lights are

@@ -1,7 +1,7 @@
 """Drop-in for the reference's pybind module `sgutilslib` (extensions/sgutils/sg.cu:280-283).
 
 Same function names, positional arguments, in-place output convention (caller allocates, returns [])
-and RuntimeError behaviour as the reference binding; the work is done by the sm_100a kernels in
+and RuntimeError behaviour as the reference binding; the work is done by the sm_90a kernels in
 csrc/sg_shade.cu through the C ABI.
 """
 import torch

@@ -1,5 +1,5 @@
 /*
- * include/goliath_b200.h — C ABI of libgoliath_b200.so (hand-written sm_100a kernels).
+ * include/goliath_b200.h — C ABI of libgoliath_b200.so (hand-written sm_90a kernels).
  *
  * The drop-in boundary of the goliath render hot path (SURVEY.md §8b).  Every entry point
  *   - takes raw DEVICE pointers (fp32 / int32 / int64, contiguous, layouts exactly as the reference's
@@ -103,7 +103,7 @@ int gb_rasterize_bwd(int img_h, int img_w, int block_width, int channels, const 
                      const int32_t* final_idx, const float* v_output, const float* v_output_alpha, float* v_xy,
                      float* v_conic, float* v_colors, float* v_opacity, void* stream);
 
-/* ---- B200 blend path (block_width == 16): same results as gb_rasterize_fwd/bwd, different work distribution.
+/* ---- packed blend path (block_width == 16): same results as gb_rasterize_fwd/bwd, different work distribution.
  * These have no counterpart in gsplat's binding; they sit behind the same rasterize_gaussians call
  * (ca_code/utils/render_gsplat.py:65-78,90-104). */
 
@@ -441,7 +441,7 @@ int gb_deconv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Hi, int Wi, const floa
                             const float* scale, const float* out, const float* gout, float slope, int apply_act,
                             float* gz, float* g_bias, float* gx, float* gw, void* stream);
 
-/* ---- tensor-core (tcgen05 + TMA + TMEM) forward of the same layer, inference path; Cin_pad % 32 == 0,
+/* ---- tensor-core (wgmma + TMA) forward of the same layer, inference path; Cin_pad % 32 == 0,
  * Cout % 16 == 0, 16 <= Cout <= 256.  Activations are NHWC split into a tf32 "hi" part and the fp32 remainder "lo"
  * (3xTF32 accumulation keeps the 1e-4 bar).  Same reference lines as gb_deconv4x4s2_wnub_fwd.
  * v may be NULL when w_scratch still holds the matrices prepared by an earlier call with the same weight_v

@@ -7,10 +7,10 @@ numpy-in / numpy-out wrappers over ``liboracle.so`` (plain C, built by ``oracle/
 ``-ffp-contract=off``).  Each C function cites the reference file:line it restates.
 
 Parity status per path (also in DESIGN.md):
-  * SG shade (sg_oracle.c)        — pinned on the GPU box against the reference kernels rebuilt into oracle/_ref
-  * splat path (splat_oracle.c)   — PARITY UNPINNED: gsplat==0.1.11 is a third-party dependency absent from
-                                    /root/reference; restated from its published algorithm (SURVEY.md App. A)
-  * raydirs / raymarch            — pinned against oracle/_ref (reference kernels) on the GPU box and against the
+  * SG shade (sg_oracle.c)        — pinned against stored outputs of the reference's own kernels (tests/golden)
+  * splat path (splat_oracle.c)   — PARITY UNPINNED: gsplat==0.1.11 is a third-party dependency outside the
+                                    reference tree; restated from its published algorithm (SURVEY.md App. A)
+  * raydirs / raymarch            — pinned against stored outputs of the reference's own kernels and against the
                                     reference's inline PyTorch raymarcher fixtures (tests/golden)
 """
 import ctypes

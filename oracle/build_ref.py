@@ -1,8 +1,8 @@
-"""Build the REFERENCE's own CUDA extensions for sm_100a into oracle/_ref/ (git-ignored, shipped to the GPU box).
+"""Build the REFERENCE's own CUDA extensions for sm_90a into oracle/_ref/ (git-ignored).
 
 TEST INFRASTRUCTURE ONLY.  Compiles the sources WHERE THEY LIE under /root/reference/extensions (nothing is copied
 into the repo) with the reference's own flags (setup.py of each extension: -use_fast_math where it says so,
--std=c++17, -lineinfo) except the gencode, which is sm_100a.  The outputs are the reference's pybind modules
+-std=c++17, -lineinfo) except the gencode, which is sm_90a.  The outputs are the reference's pybind modules
 `sgutilslib`, `utilslib`, `mvpraymarchlib`; tests load them from oracle/_ref as the GPU witness that pins the
 oracle and the product kernels (tests/test_ref_witness_gpu.py) and bench.py times them as the reference arm of
 the extension-level ratios.  gsplat is third-party and absent: it cannot be built here.
@@ -56,7 +56,7 @@ def build_one(name):
         obj = os.path.join(OUT, "obj", name + "_" + src.replace(".", "_") + ".o")
         objs.append(obj)
         if src.endswith(".cu"):
-            cmd = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-lineinfo", "-O3",
+            cmd = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-lineinfo", "-O3",
                    "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-D__CUDA_NO_HALF_OPERATORS__",
                    "-D__CUDA_NO_HALF_CONVERSIONS__", "-D__CUDA_NO_HALF2_OPERATORS__"] + \
                   (["-use_fast_math"] if spec["fast_math"] else []) + common + ["-c", path, "-o", obj]

@@ -172,9 +172,12 @@ def test_prim_decoder_end_to_end_small(cuda):
                                        ([(32, 48), (48, 16)], (40, 24)),
                                        # large enough for the pair-phase mode (one CTA, both column parities), first
                                        # layer -> NHWC pair stores, second -> NCHW float2 stores with Cout = 21 (padded N)
-                                       ([(32, 32), (32, 21)], (96, 200))])
+                                       ([(32, 32), (32, 21)], (96, 200)),
+                                       # Npad = 256 over enough tiles to keep the whole N dimension in one CTA: the
+                                       # widest accumulator (16 wgmma column blocks per warpgroup)
+                                       ([(32, 256)], (64, 64))])
 def test_tensor_core_tower_matches_simt(cuda, plan, size):
-    """csrc/deconv_tc.cu (tcgen05 + TMA + TMEM, 3xTF32) against the SIMT kernel on the same parameters: multi-layer
+    """csrc/deconv_tc.cu (wgmma + TMA, 3xTF32) against the SIMT kernel on the same parameters: multi-layer
     NHWC hi/lo chaining, channel padding (264 -> 288, 48 -> 64), partial tiles, and the SIMT tail for Cout % 16 != 0."""
     from goliath_b200 import nn as gnn
 

@@ -1,7 +1,6 @@
 """GPU parity of the SG shade kernels (csrc/sg_shade.cu) through the reference-shaped Python surface
-(goliath_b200.sgutils.evaluate_gaussian) against the CPU oracle, and — when oracle/_ref holds the reference's
-own sgutilslib rebuilt for sm_100a — against the reference kernels themselves on the same device."""
-import importlib.util
+(goliath_b200.sgutils.evaluate_gaussian) against the CPU oracle, and against the outputs of the reference's own
+sg.cu kernels (rebuilt for sm_90a, run on an H100) stored in tests/golden/ref_kernels_ref.npz."""
 import os
 
 import numpy as np
@@ -12,16 +11,7 @@ from test_oracle_sg import make
 from util import assert_close, t2n
 
 pytestmark = pytest.mark.gpu
-REF_SO = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "sgutilslib.so")
-
-
-def _ref_lib():
-    if not os.path.exists(REF_SO):
-        pytest.skip("oracle/_ref/sgutilslib.so not built (needs /root/reference at build time)")
-    spec = importlib.util.spec_from_file_location("sgutilslib", REF_SO)
-    m = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(m)
-    return m
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_kernels_ref.npz")
 
 
 @pytest.mark.parametrize("w_type", [0, 1, 2, 3])
@@ -53,33 +43,30 @@ def test_sg_vs_oracle(orc, cuda, w_type, shape):
 
 @pytest.mark.parametrize("w_type", [0, 1, 2, 3])
 def test_sg_vs_reference_kernels(cuda, w_type):
-    """Same inputs through the reference's sg.cu (rebuilt, -use_fast_math) and through ours."""
-    ref = _ref_lib()
+    """Same inputs as the reference's sg.cu (rebuilt, -use_fast_math) received when the golden file was made, through
+    ours; compared at the golden file's fixed sample of elements (tests/golden/make_ref_kernels_golden.py)."""
     from goliath_b200 import sgutilslib as ours
+    from golden.make_ref_kernels_golden import SAMPLE, sample_index, sg_case
 
-    N, D, L = 2, 20000, 32
-    dirs, sig, lv, lp, pp, nl = make(N=N, D=D, L=L, seed=123)
-    if w_type >= 2:
-        sig = sig * 0 + 0.3
-    c = lambda t: t.to(cuda).contiguous()
-    a = [c(dirs), c(sig), c(lv), c(lp), c(pp), c(nl)]
-    o_ref, o_our = torch.empty(N, D, 3, device=cuda), torch.empty(N, D, 3, device=cuda)
-    ref.evaluate_gaussian_fwd(*a, o_ref, w_type)
+    gold = np.load(GOLD)
+    ref = lambda k: gold["sg%d_%s" % (w_type, k)]
+    absmax = lambda k: float(gold["sg%d_%s_absmax" % (w_type, k)])
+    pick = lambda x: x.reshape(-1)[sample_index(x.size, SAMPLE, 100 + w_type)]
+    a, g, (N, D, L) = sg_case(cuda, w_type)
+    o_our = torch.empty(N, D, 3, device=cuda)
     ours.evaluate_gaussian_fwd(*a, o_our, w_type)
     torch.cuda.synchronize()
-    r = t2n(o_ref)
-    assert_close(t2n(o_our), r, rtol=1e-3, atol=1e-4 * float(np.abs(r).max()), frac=0.999, what="integral vs ref")
+    o = pick(t2n(o_our))
+    r = ref("integral")
+    assert_close(o, r, rtol=1e-3, atol=1e-4 * absmax("integral"), frac=0.999, what="integral vs ref")
     # same formula, same operation order, same -use_fast_math flag: the forward is bit-identical to sg.cu
-    assert (t2n(o_our).view(np.uint32) == r.view(np.uint32)).mean() >= 0.9999, "forward not bit-identical to the reference kernel"
-    g = c(torch.randn(N, D, 3, generator=torch.Generator().manual_seed(3)))
-    outs = []
-    for lib in (ref, ours):
-        gd, gs, gl = torch.zeros(N, D, 3, device=cuda), torch.zeros(N, D, device=cuda), torch.zeros(N, L, 3, device=cuda)
-        lib.evaluate_gaussian_bwd(*a, g, gd, gs, gl, w_type)
-        torch.cuda.synchronize()
-        outs.append((t2n(gd), t2n(gs), t2n(gl)))
-    for name, x, y in zip(("grad_dirs", "grad_sigmas", "grad_light_values"), outs[1], outs[0]):
-        assert_close(x, y, rtol=2e-3, atol=1e-4 * float(np.abs(y).max()), frac=0.999, what=name + " vs ref")
+    assert (o.view(np.uint32) == r.view(np.uint32)).mean() >= 0.9999, "forward not bit-identical to the reference kernel"
+    gd, gs, gl = torch.zeros(N, D, 3, device=cuda), torch.zeros(N, D, device=cuda), torch.zeros(N, L, 3, device=cuda)
+    ours.evaluate_gaussian_bwd(*a, g, gd, gs, gl, w_type)
+    torch.cuda.synchronize()
+    for name, x in zip(("grad_dirs", "grad_sigmas", "grad_light_values"), (gd, gs, gl)):
+        x, y = pick(t2n(x)), ref(name)
+        assert_close(x, y, rtol=2e-3, atol=1e-4 * absmax(name), frac=0.999, what=name + " vs ref")
         if name != "grad_light_values":  # that one is an atomics-order sum in both implementations
             assert (x.view(np.uint32) == y.view(np.uint32)).mean() >= 0.9999, name + " not bit-identical to the reference kernel"
 
