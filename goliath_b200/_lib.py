@@ -77,6 +77,8 @@ SIGNATURES = {
     "gb_deconv4x4s2_tc_fwd": (_i, [_i] * 6 + [_vp] * 6 + [_f, _i, _vp, _vp, _i, _vp, _vp]),
     "gb_deconv4x4s2_wnub_fwd": (_i, [_i] * 5 + [_vp] * 4 + [_f, _i, _vp, _vp]),
     "gb_deconv4x4s2_wnub_bwd": (_i, [_i] * 5 + [_vp] * 5 + [_f, _i] + [_vp] * 4 + [_vp]),
+    "gb_conv4x4s2_wnub_fwd": (_i, [_i] * 5 + [_vp] * 4 + [_f, _i, _vp, _vp]),
+    "gb_conv4x4s2_wnub_bwd": (_i, [_i] * 5 + [_vp] * 5 + [_f, _i] + [_vp] * 4 + [_vp]),
     "gb_conv2d_wnub_fwd": (_i, [_i] * 6 + [_vp] * 4 + [_i, _f, _i, _vp, _vp]),
     "gb_conv2d_wnub_bwd": (_i, [_i] * 6 + [_vp] * 5 + [_f, _i, _i] + [_vp] * 4 + [_vp]),
     "gb_mvp_slab_to_prims_fwd": (_i, [_i] * 6 + [_vp] * 3 + [_f, _f, _i, _vp, _vp]),

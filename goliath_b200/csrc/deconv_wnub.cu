@@ -25,6 +25,10 @@ constexpr int CO_T = 8;       // output channels per CTA pass
 constexpr int CI_CHUNK = 8;   // input channels staged per step
 constexpr int HALO = TQ + 2;
 
+// SCALE_IN = false: the weight-norm scale belongs to the output channel and is applied to the accumulator.
+// SCALE_IN = true : it belongs to the INPUT channel (the data gradient of the stride-2 convolution, where the conv's
+//                   output channels are this kernel's inputs): the weights are scaled while they are staged.
+template <bool SCALE_IN>
 __global__ void __launch_bounds__(TQ* TQ) deconv4x4s2_fwd_kernel(
     int Cin, int Cout, int Hi, int Wi, const float* __restrict__ x /* [B,Cin,Hi,Wi] */,
     const float* __restrict__ v /* [Cin,Cout,4,4] */, const float* __restrict__ scale /* [Cout] */,
@@ -61,7 +65,10 @@ __global__ void __launch_bounds__(TQ* TQ) deconv4x4s2_fwd_kernel(
     for (int i = tid; i < CI_CHUNK * CO_T * 16; i += TQ * TQ) {
       const int ci = i / (CO_T * 16), co = (i / 16) % CO_T, k = i % 16;
       float val = 0.f;
-      if (ci0 + ci < Cin && co0 + co < Cout) val = v[((size_t)(ci0 + ci) * Cout + (co0 + co)) * 16 + k];
+      if (ci0 + ci < Cin && co0 + co < Cout) {
+        val = v[((size_t)(ci0 + ci) * Cout + (co0 + co)) * 16 + k];
+        if (SCALE_IN) val *= scale[ci0 + ci];
+      }
       s_w[ci][co][k] = val;
     }
     __syncthreads();
@@ -93,7 +100,7 @@ __global__ void __launch_bounds__(TQ* TQ) deconv4x4s2_fwd_kernel(
   for (int c = 0; c < CO_T; ++c) {
     const int co = co0 + c;
     if (co >= Cout) break;
-    const float sc = scale[co];
+    const float sc = SCALE_IN ? 1.f : scale[co];
     float o00 = acc[c][0] * sc, o01 = acc[c][1] * sc, o10 = acc[c][2] * sc, o11 = acc[c][3] * sc;
     const size_t row0 = ((size_t)co * Ho + 2 * m) * Wo + 2 * n;
     if (bias) {
@@ -311,6 +318,15 @@ __global__ void __launch_bounds__(256, 2) deconv4x4s2_fwd_wide_kernel(
   }
 }
 
+// The round-1 forward kernel's launch (also the stride-2 convolution's data gradient, SCALE_IN = true)
+template <bool SCALE_IN>
+int launch_deconv_fwd(int B, int Cin, int Cout, int Hi, int Wi, const float* x, const float* v, const float* scale,
+                      const float* bias, float slope, int apply_act, float* out, cudaStream_t s) {
+  dim3 grid(gb::cdiv(Hi, TQ) * gb::cdiv(Wi, TQ), gb::cdiv(Cout, CO_T), B);
+  deconv4x4s2_fwd_kernel<SCALE_IN><<<grid, TQ * TQ, 0, s>>>(Cin, Cout, Hi, Wi, x, v, scale, bias, slope, apply_act, out);
+  return 1;
+}
+
 }  // namespace
 
 // Fused ConvTranspose2dWNUB(k=4, s=2, p=1) [+ LeakyReLU] forward.  x [B,Cin,Hi,Wi], v = weight_v [Cin,Cout,4,4],
@@ -339,10 +355,8 @@ GB_API int gb_deconv4x4s2_wnub_fwd(int B, int Cin, int Cout, int Hi, int Wi, con
     GB_CHECK_LAUNCH();
     return 0;
   }
-  const int tiles = gb::cdiv(Hi, TQ) * gb::cdiv(Wi, TQ);
-  dim3 grid(tiles, gb::cdiv(Cout, CO_T), B);
-  deconv4x4s2_fwd_kernel<<<grid, TQ * TQ, 0, (cudaStream_t)stream>>>(Cin, Cout, Hi, Wi, x, v, scale, bias, slope, apply_act, out);
-  gb::count_launches(1);
+  gb::count_launches(launch_deconv_fwd<false>(B, Cin, Cout, Hi, Wi, x, v, scale, bias, slope, apply_act, out,
+                                              (cudaStream_t)stream));
   GB_CHECK_LAUNCH();
   return 0;
 }
@@ -378,9 +392,20 @@ constexpr int BD_CO = 8;          // output channels staged per step
 constexpr int BD_CI = 8;          // input channels per CTA
 constexpr int BD_G = 2 * BD_T + 2;  // gz tile edge (34)
 
+// The same gather is the forward of the stride-2 4x4 convolution (gb_conv4x4s2_wnub_fwd): with CONV_FWD the kernel
+// reads the conv's input as `gz` (Cout here = the conv's Cin), v [Cin,Cout,4,4] as the conv weight [Cout_conv,Cin_conv,4,4]
+// and writes the conv's output as `gx` (Cin here = the conv's Cout).  The weight-norm scale then belongs to the
+// OUTPUT channel ci: it is applied to the accumulator, followed by the untied bias [Cin,Hi,Wi] and the activation.
+__device__ __forceinline__ float wn_bias_act(float a, float sc, float b, float slope, int apply_act) {
+  const float r = a * sc + b;
+  return apply_act ? (r > 0.f ? r : r * slope) : r;
+}
+
+template <bool CONV_FWD>
 __global__ void __launch_bounds__(BD_T* BD_T) deconv4x4s2_bwd_data_kernel(
     int Cin, int Cout, int Hi, int Wi, const float* __restrict__ gz /* [B,Cout,2Hi,2Wi] */,
-    const float* __restrict__ v, const float* __restrict__ scale, float* __restrict__ gx /* [B,Cin,Hi,Wi] */) {
+    const float* __restrict__ v, const float* __restrict__ scale, const float* __restrict__ bias, float slope,
+    int apply_act, float* __restrict__ gx /* [B,Cin,Hi,Wi] */) {
   __shared__ float s_g[BD_CO][BD_G][BD_G + 1];
   __shared__ __align__(16) float s_w[BD_CO][BD_CI][16];
   const int tiles_x = (Wi + BD_T - 1) / BD_T;
@@ -406,7 +431,10 @@ __global__ void __launch_bounds__(BD_T* BD_T) deconv4x4s2_bwd_data_kernel(
     for (int i = tid; i < BD_CO * BD_CI * 16; i += BD_T * BD_T) {
       const int co = i / (BD_CI * 16), ci = (i / 16) % BD_CI, k = i % 16;
       float val = 0.f;
-      if (co0 + co < Cout && ci0 + ci < Cin) val = v[((size_t)(ci0 + ci) * Cout + (co0 + co)) * 16 + k] * scale[co0 + co];
+      if (co0 + co < Cout && ci0 + ci < Cin) {
+        val = v[((size_t)(ci0 + ci) * Cout + (co0 + co)) * 16 + k];
+        if (!CONV_FWD) val *= scale[co0 + co];
+      }
       s_w[co][ci][k] = val;
     }
     __syncthreads();
@@ -432,8 +460,13 @@ __global__ void __launch_bounds__(BD_T* BD_T) deconv4x4s2_bwd_data_kernel(
   const int y = ty0 + py, x = tx0 + px;
   if (y >= Hi || x >= Wi) return;
 #pragma unroll
-  for (int ci = 0; ci < BD_CI; ++ci)
-    if (ci0 + ci < Cin) gx[(((size_t)b * Cin + ci0 + ci) * Hi + y) * Wi + x] = acc[ci];
+  for (int ci = 0; ci < BD_CI; ++ci) {
+    if (ci0 + ci >= Cin) continue;
+    float r = acc[ci];
+    if (CONV_FWD)
+      r = wn_bias_act(r, scale[ci0 + ci], bias ? bias[((size_t)(ci0 + ci) * Hi + y) * Wi + x] : 0.f, slope, apply_act);
+    gx[(((size_t)b * Cin + ci0 + ci) * Hi + y) * Wi + x] = r;
+  }
 }
 
 // weight gradient: warp tile = 16 ci x 8 co (lane: cig = lane>>3 -> 4 ci, co = lane&7 -> 16 taps), 8 warps split the
@@ -560,9 +593,11 @@ __device__ __forceinline__ void stage_gz_tile(float* s_g, const float* __restric
   }
 }
 
+template <bool CONV_FWD>  // as in deconv4x4s2_bwd_data_kernel
 __global__ void __launch_bounds__(256, 2) deconv4x4s2_bwd_data_wide_kernel(
     int Cin, int Cout, int Hi, int Wi, const float* __restrict__ gz /* [B,Cout,2Hi,2Wi] */, const float* __restrict__ v,
-    const float* __restrict__ scale, float* __restrict__ gx /* [B,Cin,Hi,Wi] */) {
+    const float* __restrict__ scale, const float* __restrict__ bias, float slope, int apply_act,
+    float* __restrict__ gx /* [B,Cin,Hi,Wi] */) {
   extern __shared__ __align__(16) unsigned char dsm[];
   const int tiles_x = (Wi + DW_X - 1) / DW_X;
   const int ty0 = (blockIdx.x / tiles_x) * DW_Y, tx0 = (blockIdx.x % tiles_x) * DW_X;
@@ -605,7 +640,7 @@ __global__ void __launch_bounds__(256, 2) deconv4x4s2_bwd_data_wide_kernel(
 #pragma unroll 1
     for (int co = 0; co < DW_CO; ++co) {
       if (blk * DW_CO + co >= Cout) break;
-      const float sc = scale[blk * DW_CO + co];
+      const float sc = CONV_FWD ? 1.f : scale[blk * DW_CO + co];
       unsigned long long G[4][6];  // rows 2m-1 .. 2m+2, columns 2n-1 .. 2n+4, scaled and duplicated
 #pragma unroll
       for (int r = 0; r < 4; ++r) {
@@ -638,9 +673,19 @@ __global__ void __launch_bounds__(256, 2) deconv4x4s2_bwd_data_wide_kernel(
 #pragma unroll
   for (int c = 0; c < DW_CI / 2; ++c) {
     const float2 a0 = unpack2(acc[0][c]), a1 = unpack2(acc[1][c]);
-    if (ci0 + 2 * c < Cin) *reinterpret_cast<float2*>(gxb + ((size_t)(ci0 + 2 * c) * Hi + m) * Wi + n) = make_float2(a0.x, a1.x);
-    if (ci0 + 2 * c + 1 < Cin)
-      *reinterpret_cast<float2*>(gxb + ((size_t)(ci0 + 2 * c + 1) * Hi + m) * Wi + n) = make_float2(a0.y, a1.y);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int ch = ci0 + 2 * c + h;
+      if (ch >= Cin) continue;
+      const size_t off = ((size_t)ch * Hi + m) * Wi + n;
+      float2 r = h ? make_float2(a0.y, a1.y) : make_float2(a0.x, a1.x);
+      if (CONV_FWD) {
+        const float sc = scale[ch];
+        const float2 bb = bias ? *reinterpret_cast<const float2*>(bias + off) : make_float2(0.f, 0.f);
+        r = make_float2(wn_bias_act(r.x, sc, bb.x, slope, apply_act), wn_bias_act(r.y, sc, bb.y, slope, apply_act));
+      }
+      *reinterpret_cast<float2*>(gxb + off) = r;
+    }
   }
 }
 
@@ -738,6 +783,64 @@ __global__ void __launch_bounds__(256, 1) deconv4x4s2_bwd_weight_wide_kernel(
   }
 }
 
+// The backward launches, shared by the transposed convolution and the stride-2 convolution (whose forward is this
+// data gradient and whose weight gradient is this weight gradient with the roles of x and gz swapped).  `wide` picks
+// the kernels for the high-resolution layers; the caller has checked Wi % 4 == 0, Wi >= 32, Hi >= 16.
+template <bool CONV_FWD>
+int launch_bwd_data(bool wide, int B, int Cin, int Cout, int Hi, int Wi, const float* gz, const float* v,
+                    const float* scale, const float* bias, float slope, int apply_act, float* gx, cudaStream_t s) {
+  if (wide) {
+    static bool configured = false;
+    if (!configured) {
+      GB_CUDA(cudaFuncSetAttribute(deconv4x4s2_bwd_data_wide_kernel<CONV_FWD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   DW_SMEM));
+      configured = true;
+    }
+    dim3 grid(gb::cdiv(Hi, DW_Y) * gb::cdiv(Wi, DW_X), gb::cdiv(Cin, DW_CI), B);
+    deconv4x4s2_bwd_data_wide_kernel<CONV_FWD><<<grid, 256, DW_SMEM, s>>>(Cin, Cout, Hi, Wi, gz, v, scale, bias, slope,
+                                                                          apply_act, gx);
+    return 1;
+  }
+  dim3 grid(gb::cdiv(Hi, BD_T) * gb::cdiv(Wi, BD_T), gb::cdiv(Cin, BD_CI), B);
+  deconv4x4s2_bwd_data_kernel<CONV_FWD><<<grid, BD_T * BD_T, 0, s>>>(Cin, Cout, Hi, Wi, gz, v, scale, bias, slope,
+                                                                     apply_act, gx);
+  return 1;
+}
+
+int launch_bwd_weight(bool wide, int B, int Cin, int Cout, int Hi, int Wi, const float* x, const float* gz, float* gw,
+                      cudaStream_t s) {
+  if (wide) {
+    static bool configured = false;
+    if (!configured) {
+      GB_CUDA(cudaFuncSetAttribute(deconv4x4s2_bwd_weight_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WW_SMEM));
+      configured = true;
+    }
+    const int total = B * gb::cdiv(Hi, WW_Y) * gb::cdiv(Wi, WW_X);
+    const int pairs = gb::cdiv(Cin, WW_CI) * gb::cdiv(Cout, WW_CO);
+    int split = (gb::kNumSMs * 2) / pairs;  // one CTA per SM at a time (120 KB of shared memory): two FULL waves
+    split = max(1, min(split, total));
+    dim3 grid(split, gb::cdiv(Cin, WW_CI), gb::cdiv(Cout, WW_CO));
+    deconv4x4s2_bwd_weight_wide_kernel<<<grid, 256, WW_SMEM, s>>>(B, Cin, Cout, Hi, Wi, x, gz, gw);
+    return 1;
+  }
+  const int total = B * gb::cdiv(Hi, BW_TY) * gb::cdiv(Wi, BW_TX);
+  const int pairs = gb::cdiv(Cin, BW_CI) * gb::cdiv(Cout, BW_CO);
+  int split = gb::cdiv(gb::kNumSMs * 3, pairs);  // ~3 CTAs per SM in total
+  split = max(1, min(split, total));
+  dim3 grid(split, gb::cdiv(Cin, BW_CI), gb::cdiv(Cout, BW_CO));
+  deconv4x4s2_bwd_weight_kernel<<<grid, 256, 0, s>>>(B, Cin, Cout, Hi, Wi, x, gz, gw);
+  return 1;
+}
+
+// gz = gout * act'(out) and the untied-bias gradient, unless gz aliases gout (no activation, no separate bias gradient)
+int launch_act_bwd(int B, long long per_item, const float* out, const float* gout, float slope, int apply_act, float* gz,
+                   float* g_bias, cudaStream_t s) {
+  if (gz == gout && !apply_act && !g_bias) return 0;
+  deconv_act_bwd_kernel<<<(unsigned)gb::cdiv64(per_item, 256), 256, 0, s>>>(B, per_item, gout, out, slope, apply_act, gz,
+                                                                            g_bias);
+  return 1;
+}
+
 }  // namespace
 
 // GOLIATH_B200_DECONV_BWD=narrow keeps the round-1 backward kernels on every layer (A/B timing, tests)
@@ -763,54 +866,61 @@ GB_API int gb_deconv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Hi, int Wi, con
   const long long per_item = (long long)Cout * 4 * Hi * Wi;
   // gz == gout with no activation and no separate bias gradient: the pre-activation gradient IS gout (the caller
   // aliases the untied-bias gradient to it when B == 1) — no 3 x 524 MB copy pass at the 16->125 @1024^2 layer
-  const bool alias = (gz == gout) && !apply_act && !g_bias;
-  int launches = 0;
-  if (!alias) {
-    deconv_act_bwd_kernel<<<(unsigned)gb::cdiv64(per_item, 256), 256, 0, s>>>(B, per_item, gout, out, slope, apply_act,
-                                                                              gz, g_bias);
-    launches = 1;
-  }
+  int launches = launch_act_bwd(B, per_item, out, gout, slope, apply_act, gz, g_bias, s);
   // high-resolution layers (the wide forward's condition, plus 16-byte staging: Wi % 4 == 0): wide backward kernels
   const bool wide = Cin <= 32 && Wi % 4 == 0 && Wi >= 32 && Hi >= 16 && wide_bwd_enabled();
-  if (wide) {
-    static bool configured = false;
-    if (!configured) {
-      GB_CUDA(cudaFuncSetAttribute(deconv4x4s2_bwd_data_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM));
-      GB_CUDA(cudaFuncSetAttribute(deconv4x4s2_bwd_weight_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WW_SMEM));
-      configured = true;
-    }
-    if (gx) {
-      dim3 grid(gb::cdiv(Hi, DW_Y) * gb::cdiv(Wi, DW_X), gb::cdiv(Cin, DW_CI), B);
-      deconv4x4s2_bwd_data_wide_kernel<<<grid, 256, DW_SMEM, s>>>(Cin, Cout, Hi, Wi, gz, v, scale, gx);
-      ++launches;
-    }
-    if (gw) {
-      const int total = B * gb::cdiv(Hi, WW_Y) * gb::cdiv(Wi, WW_X);
-      const int pairs = gb::cdiv(Cin, WW_CI) * gb::cdiv(Cout, WW_CO);
-      int split = (gb::kNumSMs * 2) / pairs;  // one CTA per SM at a time (120 KB of shared memory): two FULL waves
-      split = max(1, min(split, total));
-      dim3 grid(split, gb::cdiv(Cin, WW_CI), gb::cdiv(Cout, WW_CO));
-      deconv4x4s2_bwd_weight_wide_kernel<<<grid, 256, WW_SMEM, s>>>(B, Cin, Cout, Hi, Wi, x, gz, gw);
-      ++launches;
-    }
-    gb::count_launches(launches);
-    GB_CHECK_LAUNCH();
-    return 0;
-  }
-  if (gx) {
-    dim3 grid(gb::cdiv(Hi, BD_T) * gb::cdiv(Wi, BD_T), gb::cdiv(Cin, BD_CI), B);
-    deconv4x4s2_bwd_data_kernel<<<grid, BD_T * BD_T, 0, s>>>(Cin, Cout, Hi, Wi, gz, v, scale, gx);
-    ++launches;
-  }
-  if (gw) {
-    const int total = B * gb::cdiv(Hi, BW_TY) * gb::cdiv(Wi, BW_TX);
-    const int pairs = gb::cdiv(Cin, BW_CI) * gb::cdiv(Cout, BW_CO);
-    int split = gb::cdiv(gb::kNumSMs * 3, pairs);  // ~3 CTAs per SM in total
-    split = max(1, min(split, total));
-    dim3 grid(split, gb::cdiv(Cin, BW_CI), gb::cdiv(Cout, BW_CO));
-    deconv4x4s2_bwd_weight_kernel<<<grid, 256, 0, s>>>(B, Cin, Cout, Hi, Wi, x, gz, gw);
-    ++launches;
-  }
+  if (gx) launches += launch_bwd_data<false>(wide, B, Cin, Cout, Hi, Wi, gz, v, scale, nullptr, 1.f, 0, gx, s);
+  if (gw) launches += launch_bwd_weight(wide, B, Cin, Cout, Hi, Wi, x, gz, gw, s);
+  gb::count_launches(launches);
+  GB_CHECK_LAUNCH();
+  return 0;
+}
+
+// =====================================================================================================
+// Stride-2 4x4 convolution (k=4, s=2, p=1) with weight-norm scale, untied bias and LeakyReLU: the layer of the RGCA
+// texture encoder (ca_code/models/rgca.py:281-298, la.Conv2dWNUB(cin, cout, h, w, 4, 2, 1), layers.py:276-327).
+//   out[b,o,y,x] = act(scale[o] * sum_i sum_{ky,kx} x[b,i,2y-1+ky,2x-1+kx] v[o,i,ky,kx] + bias[o,y,x])
+// This is the transposed convolution with its two sides exchanged, so it runs on the kernels above:
+//   forward         = the deconv data gradient with the conv input as gz (CONV_FWD: scale on the output channel,
+//                     bias + activation epilogue);
+//   data gradient   = the (round-1) deconv forward of gz with v read as [Cin_d = Cout, Cout_d = Cin, 4, 4] (SCALE_IN:
+//                     the scale belongs to its input channel o);
+//   weight gradient = the deconv weight gradient with x and gz exchanged; its [Cin_d, Cout_d, 4, 4] output is the
+//                     conv weight layout [Cout, Cin, 4, 4].
+// Kernels are chosen by shape: the wide ones where the tile conditions hold and their grid still fills the machine.
+namespace {
+
+bool conv_wide_fwd(int B, int Cout, int Ho, int Wo) {
+  return Wo % 4 == 0 && Wo >= 32 && Ho >= 16 &&
+         (long long)gb::cdiv(Ho, DW_Y) * gb::cdiv(Wo, DW_X) * gb::cdiv(Cout, DW_CI) * B >= gb::kNumSMs;
+}
+
+}  // namespace
+
+// x [B,Cin,2Ho,2Wo], v = weight_v [Cout,Cin,4,4], scale [Cout] = weight_g / ||weight_v||_F, bias [Cout,Ho,Wo] or
+// NULL, out [B,Cout,Ho,Wo]; apply_act != 0 applies LeakyReLU(slope).
+GB_API int gb_conv4x4s2_wnub_fwd(int B, int Cin, int Cout, int Ho, int Wo, const float* x, const float* v,
+                                 const float* scale, const float* bias, float slope, int apply_act, float* out,
+                                 void* stream) {
+  if (B <= 0 || Cin <= 0 || Cout <= 0 || Ho <= 0 || Wo <= 0) return 0;
+  const int n = launch_bwd_data<true>(conv_wide_fwd(B, Cout, Ho, Wo), B, Cout, Cin, Ho, Wo, x, v, scale, bias, slope,
+                                      apply_act, out, (cudaStream_t)stream);
+  gb::count_launches(n);
+  GB_CHECK_LAUNCH();
+  return 0;
+}
+
+// Backward of gb_conv4x4s2_wnub_fwd, with the conventions of gb_deconv4x4s2_wnub_bwd: gz [B,Cout,Ho,Wo] scratch (may be
+// gout itself when apply_act == 0 and g_bias == NULL), g_bias [Cout,Ho,Wo] or NULL, gx [B,Cin,2Ho,2Wo] or NULL,
+// gw [Cout,Cin,4,4] ACCUMULATED at unit scale (gw[o,i,k] = sum gz * x); the caller applies the weight-norm chain rule.
+GB_API int gb_conv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Ho, int Wo, const float* x, const float* v,
+                                 const float* scale, const float* out, const float* gout, float slope, int apply_act,
+                                 float* gz, float* g_bias, float* gx, float* gw, void* stream) {
+  if (B <= 0 || Cin <= 0 || Cout <= 0 || Ho <= 0 || Wo <= 0) return 0;
+  cudaStream_t s = (cudaStream_t)stream;
+  int launches = launch_act_bwd(B, (long long)Cout * Ho * Wo, out, gout, slope, apply_act, gz, g_bias, s);
+  if (gx) launches += launch_deconv_fwd<true>(B, Cout, Cin, Ho, Wo, gz, v, scale, nullptr, 1.f, 0, gx, s);
+  if (gw) launches += launch_bwd_weight(Wo % 4 == 0 && Wo >= 32 && Ho >= 16, B, Cout, Cin, Ho, Wo, gz, x, gw, s);
   gb::count_launches(launches);
   GB_CHECK_LAUNCH();
   return 0;

@@ -5,7 +5,9 @@ checkpoints load (`weight_v`, `weight_g`, `bias`): `ConvTranspose2dWNUB`, `Linea
 
 The stride-2 4x4 transposed convolution + untied bias + LeakyReLU runs as ONE hand-written sm_90a kernel in the
 forward, and its backward as three more (activation/bias gradient, data gradient, weight gradient) — no cuDNN
-(csrc/deconv_wnub.cu).  Round-1 status: fp32 SIMT kernels; LinearWN is a plain library GEMM (cuBLAS via F.linear)."""
+(csrc/deconv_wnub.cu).  The stride-2 4x4 convolution of the RGCA encoder (`Conv2dWNUB(.., 4, 2, 1)`) runs on the same
+kernels with the two sides of the layer exchanged.  Round-1 status: fp32 SIMT kernels; LinearWN is a plain library
+GEMM (cuBLAS via F.linear)."""
 import math
 from typing import Optional
 
@@ -166,15 +168,82 @@ class _ConvS1WN(Function):
         return gx, gv, gg.view_as(g), gb, None
 
 
+class _Conv4x4s2WN(Function):
+    """stride-2 4x4 conv (padding 1) + weight-norm scale + untied bias [+ LeakyReLU], csrc/deconv_wnub.cu."""
+
+    @staticmethod
+    def forward(ctx, x, weight_v, weight_g, bias, slope):
+        x, weight_v = x.contiguous(), weight_v.contiguous()
+        _lib.check_input(x, "input")
+        _lib.check_input(weight_v, "weight_v")
+        B, Cin, H, W = x.shape
+        Cout = weight_v.shape[0]
+        if weight_v.shape != (Cout, Cin, 4, 4):
+            raise RuntimeError("weight_v must be [Cout, Cin, 4, 4]")
+        if H % 2 or W % 2:
+            raise RuntimeError("a k=4, s=2, p=1 layer needs an even input size (got %dx%d)" % (H, W))
+        Ho, Wo = H // 2, W // 2
+        b = None if bias is None else bias.contiguous()
+        if b is not None and b.shape != (Cout, Ho, Wo):
+            raise RuntimeError("untied bias must be [Cout, H/2, W/2]")
+        scale = (weight_g.reshape(-1) / weight_v.norm()).contiguous()
+        out = torch.empty(B, Cout, Ho, Wo, device=x.device, dtype=torch.float32)
+        with torch.cuda.device(x.device):
+            _lib.check(_lib.lib().gb_conv4x4s2_wnub_fwd(
+                B, Cin, Cout, Ho, Wo, _lib.ptr(x), _lib.ptr(weight_v), _lib.ptr(scale), _lib.ptr(b),
+                float(slope if slope is not None else 1.0), int(slope is not None), _lib.ptr(out),
+                _lib.stream_ptr(x.device)), "conv4x4s2_wnub_fwd")
+        ctx.save_for_backward(x, weight_v, weight_g, out)
+        ctx.slope = slope
+        ctx.has_bias = bias is not None
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, v, g, out = ctx.saved_tensors
+        B, Cin = x.shape[:2]
+        Cout, Ho, Wo = out.shape[1:]
+        dev = x.device
+        gout = gout.contiguous()
+        vnorm = v.norm()
+        scale = (g.reshape(-1) / vnorm).contiguous()
+        # as in _Deconv4x4s2WNUB: with B == 1 the untied-bias gradient is the pre-activation gradient, and without an
+        # activation that is gout itself
+        alias_bias = ctx.has_bias and B == 1
+        gz = gout if B == 1 and ctx.slope is None else torch.empty_like(out)
+        gb = None
+        if ctx.has_bias and not alias_bias:
+            gb = torch.empty(Cout, Ho, Wo, device=dev, dtype=torch.float32)
+        gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
+        gw = torch.zeros_like(v)                         # d L / d (effective weight), accumulated by the kernel
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().gb_conv4x4s2_wnub_bwd(
+                B, Cin, Cout, Ho, Wo, _lib.ptr(x), _lib.ptr(v), _lib.ptr(scale), _lib.ptr(out), _lib.ptr(gout),
+                float(ctx.slope if ctx.slope is not None else 1.0), int(ctx.slope is not None), _lib.ptr(gz), _lib.ptr(gb),
+                _lib.ptr(gx), _lib.ptr(gw), _lib.stream_ptr(dev)), "conv4x4s2_wnub_bwd")
+        if alias_bias:
+            gb = gz.view(Cout, Ho, Wo)
+        # weight-norm chain rule, g per OUTPUT channel (dim 0), norm over the whole tensor (as _ConvS1WN)
+        w = g * v / vnorm
+        gg = (gw * v).sum(dim=(1, 2, 3), keepdim=True) / vnorm
+        gv = g * gw / vnorm - (gw * w).sum() * v / (vnorm * vnorm)
+        return gx, gv, gg.view_as(g), gb, None
+
+
 class Conv2dWNUB(nn.Module):
-    """Conv2d (stride 1, k in {1,3}, "same" padding) with weight norm and untied bias (layers.py:276-327,472).
+    """Conv2d with weight norm and untied bias (layers.py:276-327,472): stride 1, k in {1,3}, "same" padding (hand-MVP
+    decoders), or k=4, s=2, p=1 (the RGCA encoder, rgca.py:281-298), where (height, width) is the OUTPUT size and the
+    input must be [B, Cin, 2*height, 2*width].
     Constructor argument order is the reference's: (in, out, height, width, kernel_size, stride, padding)."""
 
     def __init__(self, in_channels, out_channels, height, width, kernel_size=3, stride=1, padding=1, bias=True):
         super().__init__()
-        if stride != 1 or kernel_size not in (1, 3) or padding != (kernel_size - 1) // 2:
-            raise NotImplementedError("the fused kernel covers the hand-MVP decoders' stride-1 'same' 1x1 / 3x3 layers")
+        strided = (kernel_size, stride, padding) == (4, 2, 1)
+        if not strided and (stride != 1 or kernel_size not in (1, 3) or padding != (kernel_size - 1) // 2):
+            raise NotImplementedError("the fused kernels cover stride-1 'same' 1x1 / 3x3 layers and k=4, s=2, p=1 layers")
         self.in_channels, self.out_channels, self.kernel_size = in_channels, out_channels, (kernel_size, kernel_size)
+        self.stride = (stride, stride)
+        self._out_size = (height, width)
         self.weight_v = nn.Parameter(torch.empty(out_channels, in_channels, kernel_size, kernel_size))
         self.weight_g = nn.Parameter(torch.ones(out_channels, 1, 1, 1))
         self.bias = nn.Parameter(torch.zeros(out_channels, height, width)) if bias else None
@@ -189,6 +258,12 @@ class Conv2dWNUB(nn.Module):
 
     def forward(self, input, slope: Optional[float] = None):
         slope = self.fused_slope if slope is None else slope
+        if self.stride[0] == 2:
+            h, w = self._out_size
+            if input.dim() != 4 or tuple(input.shape[1:]) != (self.in_channels, 2 * h, 2 * w):
+                raise RuntimeError("input must be [B, %d, %d, %d] (got %s)" % (self.in_channels, 2 * h, 2 * w,
+                                                                              tuple(input.shape)))
+            return _Conv4x4s2WN.apply(input, self.weight_v, self.weight_g, self.bias, slope)
         return _ConvS1WN.apply(input, self.weight_v, self.weight_g, self.bias, slope)
 
 
@@ -196,6 +271,8 @@ class Conv2dWN(Conv2dWNUB):
     """th.nn.Conv2d with the reference's weight norm and a tied bias [Cout] (layers.py:470; ConvBlock.conv_resize)."""
 
     def __init__(self, in_channels, out_channels, kernel_size=1, stride=1, padding=0, bias=True):
+        if stride != 1:
+            raise NotImplementedError("the fused kernels cover stride-1 'same' 1x1 / 3x3 tied-bias layers")
         super().__init__(in_channels, out_channels, 1, 1, kernel_size, stride, padding, bias=False)
         self.bias = nn.Parameter(torch.zeros(out_channels)) if bias else None
 

@@ -8,8 +8,13 @@ as the reference module, so its checkpoints load: `viewmod.0.*`, `encmod.0.*`, `
 module can be exercised at small sizes.  The environment-map specular branch (`preconv_envmap`, rgca.py:548-556) is
 one texture-fetch kernel (csrc/envmap_spec.cu, `goliath_b200.envmap_spec`); the training-only random back-light
 outputs `cos_weight` / `color_rand` (rgca.py:590-618) come out of the heads kernel's pass over the diffuse planes
-(second light-SH table), so the reference's `backlit_reg` loss finds both keys."""
-from typing import Optional
+(second light-SH table), so the reference's `backlit_reg` loss finds both keys.
+
+The joint texture + geometry `Encoder` (rgca.py:256-332) and the coarse-geometry `GeomDecoder` (rgca.py:335-369) are
+mirrored with the same constructor arguments, state-dict keys and outputs; the encoder's eight stride-2 convolutions run
+on the fused sm_90a kernels (`goliath_b200.nn.Conv2dWNUB(.., 4, 2, 1)` with the LeakyReLU in their epilogue), the
+`LinearWN` layers, the input affine and the sampling noise are torch."""
+from typing import Dict, Optional
 
 import torch as th
 import torch.nn as nn
@@ -98,3 +103,66 @@ class PrimDecoder(nn.Module):
                 preds["cos_weight"] = (light_dir * preds["spec_nml"]).sum(dim=-1, keepdim=True)
             preds["color_rand"] = preds.pop("diff_color_rand").clamp(min=0.0)
         return preds
+
+
+class Encoder(nn.Module):
+    """A joint encoder for texture and geometry (rgca.Encoder): `geom` [B, n_verts_in, 3] and a 1024x1024 `color`
+    texture in [0, 255] -> `embs`, `embs_mu`, `embs_logvar` [B, n_embs]."""
+
+    def __init__(self, n_embs: int, n_verts_in: int, noise_std: float = 1.0, mean_scale: float = 0.1,
+                 logvar_scale: float = 0.01):
+        super().__init__()
+        self.noise_std = noise_std
+        self.n_embs = n_embs
+        self.mean_scale = mean_scale
+        self.logvar_scale = logvar_scale
+        self.n_verts_in = n_verts_in
+        self.geommod = nn.Sequential(gnn.LinearWN(self.n_verts_in * 3, 256), nn.LeakyReLU(0.2, inplace=True))
+        # 1024^2 -> 4^2: the texture size is fixed by the reshape to 256 * 4 * 4 below, as upstream
+        texmod = []
+        for cin, cout, size in ((3, 32, 512), (32, 32, 256), (32, 64, 128), (64, 64, 64), (64, 128, 32), (128, 128, 16),
+                                (128, 256, 8), (256, 256, 4)):
+            layer = gnn.Conv2dWNUB(cin, cout, size, size, 4, 2, 1)
+            layer.fused_slope = 0.2
+            texmod += [layer, gnn.FusedLeakyReLU()]
+        self.texmod = nn.Sequential(*texmod)
+        self.jointmod = nn.Sequential(gnn.LinearWN(256 + 256 * 4 * 4, 512), nn.LeakyReLU(0.2, inplace=True))
+        self.mean = gnn.LinearWN(512, self.n_embs)
+        self.logvar = gnn.LinearWN(512, self.n_embs)
+        self.apply(lambda m: gnn.glorot(m, 0.2))
+        gnn.glorot(self.mean, 1.0)
+        gnn.glorot(self.logvar, 1.0)
+
+    def forward(self, geom: th.Tensor, color: th.Tensor) -> Dict[str, th.Tensor]:
+        geomout = self.geommod(geom.view(geom.shape[0], -1))
+        texout = self.texmod(color / 255.0 - 0.5).view(-1, 256 * 4 * 4)
+        encout = self.jointmod(th.cat([geomout, texout], dim=1))
+        embs_mu = self.mean(encout) * self.mean_scale
+        embs_logvar = self.logvar(encout) * self.logvar_scale
+        # the noise is only applied to the input-conditioned values; its scale is exp(logvar), as upstream
+        if self.training:
+            noise = th.randn_like(embs_mu)
+            embs = embs_mu + th.exp(embs_logvar) * noise * self.noise_std
+        else:
+            embs = embs_mu.clone()
+        return dict(embs=embs, embs_mu=embs_mu, embs_logvar=embs_logvar)
+
+
+class GeomDecoder(nn.Module):
+    """A decoder for coarse geometry (rgca.GeomDecoder): `embs` [B, n_embs] -> `face_geom` [B, n_verts, 3]."""
+
+    def __init__(self, n_embs: int, verts_mean: th.Tensor, verts_std: float):
+        super().__init__()
+        self.verts_std: float = verts_std
+        self.register_buffer("verts_mean", verts_mean[None].float())
+        self.n_embs = n_embs
+        self.n_verts_out = verts_mean.shape[-2]
+        self.geommod = nn.Sequential(gnn.LinearWN(self.n_embs, 256), nn.LeakyReLU(0.2, inplace=True),
+                                     gnn.LinearWN(256, 3 * self.n_verts_out))
+        self.apply(lambda m: gnn.glorot(m, 0.2))
+        gnn.glorot(self.geommod[-1], 1.0)
+
+    def forward(self, embs: th.Tensor) -> Dict[str, th.Tensor]:
+        geom = self.geommod(embs).view(embs.shape[0], -1, 3)
+        geom = geom * self.verts_std + self.verts_mean
+        return dict(face_geom=geom)

@@ -441,6 +441,21 @@ int gb_deconv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Hi, int Wi, const floa
                             const float* scale, const float* out, const float* gout, float slope, int apply_act,
                             float* gz, float* g_bias, float* gx, float* gw, void* stream);
 
+/* replaces conv2d + untied-bias add (ca_code/nn/layers.py:276-327) + the LeakyReLU that follows each
+ * la.Conv2dWNUB(cin, cout, h, w, 4, 2, 1) of the RGCA texture encoder (ca_code/models/rgca.py:281-298) for k=4, s=2,
+ * p=1, with the weight-norm scale folded in: out = act(scale[co] * conv(x, v) + bias).  x [B,Cin,2Ho,2Wo],
+ * v [Cout,Cin,4,4], scale [Cout] = g / ||v||_F, bias [Cout,Ho,Wo] or NULL, out [B,Cout,Ho,Wo]; apply_act != 0 applies
+ * LeakyReLU(slope).  Runs on the kernels of gb_deconv4x4s2_wnub_bwd with the two sides of the layer exchanged. */
+int gb_conv4x4s2_wnub_fwd(int B, int Cin, int Cout, int Ho, int Wo, const float* x, const float* v,
+                          const float* scale, const float* bias, float slope, int apply_act, float* out, void* stream);
+
+/* backward of the above, with the conventions of gb_deconv4x4s2_wnub_bwd.  gz [B,Cout,Ho,Wo] scratch; g_bias
+ * [Cout,Ho,Wo] or NULL; gx [B,Cin,2Ho,2Wo] or NULL; gw [Cout,Cin,4,4] = dL/d(effective weight), ACCUMULATED (caller
+ * zeroes it and applies the weight-norm chain rule). */
+int gb_conv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Ho, int Wo, const float* x, const float* v,
+                          const float* scale, const float* out, const float* gout, float slope, int apply_act,
+                          float* gz, float* g_bias, float* gx, float* gw, void* stream);
+
 /* ---- tensor-core (wgmma + TMA) forward of the same layer, inference path; Cin_pad % 32 == 0,
  * Cout % 16 == 0, 16 <= Cout <= 256.  Activations are NHWC split into a tf32 "hi" part and the fp32 remainder "lo"
  * (3xTF32 accumulation keeps the 1e-4 bar).  Same reference lines as gb_deconv4x4s2_wnub_fwd.
