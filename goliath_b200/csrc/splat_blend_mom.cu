@@ -535,15 +535,16 @@ __global__ void __launch_bounds__(kBwdThreads, 3) blend_bwd_mom_kernel(
         M[(h0 + u) * kMStride + lane] = make_float2(fac, -ov[u] * v_alpha);  // (fac, v_sigma); zeros when not valid
       }
     }
+    if (RANKED) cp_async_wait_all();  // this lane's rank copies into the entries have landed (then the warp barrier)
     __syncwarp();
     {
       const int hh = lane & 15, half = lane >> 4;
       const int he = min(hh, n - 1);
       const float4 a0 = E[(base + he) * 3], a1 = E[(base + he) * 3 + 1];
-      // the Gaussian id is only needed by the REDs at the end: start its load now (padding entries: index 0)
+      // the Gaussian id is only needed by the REDs at the end: start its load now (padding entries: index 0 / rank 0)
       const int e_idx = __float_as_int(a1.z);
       const int e_safe = e_idx == 0x7fffffff ? range.x : e_idx;
-      const int g_id = RANKED ? gids_sorted[ranks[e_safe]] : gids_sorted[e_safe];
+      const int g_id = RANKED ? gids_sorted[__float_as_int(a1.w)] : gids_sorted[e_safe];
       const float2* Mrow = M + hh * kMStride + half * 16;
       const float4* V = VO + half * 16;
       float g[4] = {0.f, 0.f, 0.f, 0.f};
@@ -634,7 +635,16 @@ __global__ void __launch_bounds__(kBwdThreads, 3) blend_bwd_mom_kernel(
         const int pos = cnt + __popc(mask & ~((2u << lane) - 1u));
         const float4 q0 = sr[tj * 3], q1 = sr[tj * 3 + 1], q2 = sr[tj * 3 + 2];
         E[pos * 3 + 0] = make_float4(q0.x, q0.y, q1.x, q1.y);
-        E[pos * 3 + 1] = make_float4(q1.z, q1.w, __int_as_float(lo + tj), 0.f);
+        if constexpr (RANKED) {
+          // the entry's 4th word gets the hit's depth rank, copied asynchronously (chunk() waits for it before phase
+          // B): phase B then finds the Gaussian id with one dependent load, rank_to_gid[rank], instead of two
+          float* e1 = reinterpret_cast<float*>(&E[pos * 3 + 1]);
+          *reinterpret_cast<float2*>(e1) = make_float2(q1.z, q1.w);
+          e1[2] = __int_as_float(lo + tj);
+          cp_async4(e1 + 3, ranks + lo + tj);
+        } else {
+          E[pos * 3 + 1] = make_float4(q1.z, q1.w, __int_as_float(lo + tj), 0.f);
+        }
         E[pos * 3 + 2] = q2;
       }
       cnt += __popc(mask);

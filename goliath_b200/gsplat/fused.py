@@ -21,11 +21,15 @@ _OVERFLOW = {}
 BINNING = os.environ.get("GOLIATH_B200_BINNING", "buckets")
 # sync-free path as two autograd nodes (projection | binning + blend), see render_fused_split; "0" keeps the single node
 SPLIT = os.environ.get("GOLIATH_B200_RENDER_SPLIT", "1") != "0"
-# records of the two-node path: "packed" (sorted 48-byte records materialised by the binning's gather, default) or "ranked"
-# (the blend stages records by depth rank from a per-Gaussian table with 16-byte cp.async gathers: the binning loses its
-# record gather, but the blend pays more for its scattered gathers; kept as an option because it holds 4x less memory
-# per view for the backward)
-RANKED = os.environ.get("GOLIATH_B200_RECORDS", "packed") == "ranked"
+# records of the two-node path: "ranked" (default: the blend stages records by depth rank from the per-Gaussian table,
+# G x 48 B, with 16-byte cp.async gathers) or "packed" (sorted 48-byte records materialised by the binning's gather,
+# cap x 48 B).  On an H100 the by-rank table (14.4 MB at 300k Gaussians) stays in the 50 MB L2 between the binning and
+# the two blends, the sorted records (52 MB on the bench head scene) do not.  Measured on an H100 SXM at a 700 W power
+# limit (scripts/profile_head_step.py): the ranked blends cost ~2 us (forward) and ~10 us (backward) more than the
+# packed ones, the record gather they make unnecessary cost ~50 us, and the bench head step takes 0.557 instead of
+# 0.592 ms.  The ranked path also holds 4x less memory per view for the backward.  "packed" is kept for A/B timing; the
+# single-node path and OLAT always use packed records.
+RANKED = os.environ.get("GOLIATH_B200_RECORDS", "ranked") == "ranked"
 
 
 def _overflow_flag(dev):
@@ -274,8 +278,8 @@ class _BinBlend(Function):
             if colors_event is not None:
                 ev = colors_event.cuda_event
                 colors.record_stream(torch.cuda.current_stream(dev))
-            # rank-staged records (default with the mom blend, launch-order tiles): the blend gathers each stage from the
-            # by-rank table, the sorted 48-byte records are never materialised (csrc/splat_blend_mom.cu, RANKED)
+            # rank-staged records (the default with the mom blend and launch-order tiles): the blend gathers each stage
+            # from the by-rank table, the sorted 48-byte records are never materialised (csrc/splat_blend_mom.cu, RANKED)
             ranked = RANKED and not sched and L.gb_get_blend_mode() == 3
             if ranked:
                 gids = torch.empty(G, **i32)            # rank -> Gaussian id
