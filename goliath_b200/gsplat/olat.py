@@ -58,8 +58,10 @@ class _RenderShared(Function):
                 float(fy), float(cx), float(cy), H, W, BW, float(clip_thresh), _lib.ptr(cov3d), _lib.ptr(xys),
                 _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp), _lib.ptr(num_tiles_hit), st),
                 "project_gaussians_forward")
+            n_isect = None
             if capacity is None:  # reference-like exact buffers: one host sync for the intersection count
-                cap = max(int(num_tiles_hit.sum().item()), 1)
+                n_isect = int(num_tiles_hit.sum().item())
+                cap = max(n_isect, 1)
             else:
                 cap = int(capacity)
             tb = _tile_bounds(H, W, BW)
@@ -79,6 +81,10 @@ class _RenderShared(Function):
             ras_fwd = L.gb_rasterize_sched_fwd if sched else L.gb_rasterize_packed_fwd
             _lib.check(ras_fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(out4),
                                _lib.ptr(final_Ts), _lib.ptr(final_idx), st), "rasterize_packed_forward")
+            if n_isect == 0:
+                # as render_fused(capacity=None): the reference's final_Ts = 0 when nothing is drawn, so alpha = 1
+                final_Ts.zero_()
+                final_idx.zero_()
             rgb[0].copy_(out4[..., :3])
             multi = MODE == "multi" and C > 1
             wide = None
