@@ -61,7 +61,7 @@ __device__ __forceinline__ float exp_neg(float s) {
   return r;
 }
 
-// RANKED staging: the tile's list is a list of sorted depth RANKS (4 B) into the by-rank record table [G,12] written
+// RANKED staging: the tile's list is a list of sorted Gaussian ids (4 B) into the by-id record table [G,12] written
 // once per Gaussian by the binning; a stage is filled by 16-byte cp.async gathers (three per record) instead of one
 // bulk copy of materialised sorted records, which removes the binning's record gather (52 MB written + read per view).
 __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
@@ -377,7 +377,7 @@ constexpr int kBwdSmem = kSmRec + kSmEntries + kSmM + kSmVo;                // 7
 template <int C, bool RANKED>
 __global__ void __launch_bounds__(kBwdThreads, 3) blend_bwd_mom_kernel(
     int img_w, int img_h, int tbx, const int* order, int sched,
-    const int* __restrict__ gids_sorted /* RANKED: rank_to_gid */, const int* __restrict__ ranks /* RANKED only */,
+    const int* __restrict__ gids_sorted /* RANKED: unused */, const int* __restrict__ ranks /* RANKED only */,
     const int2* __restrict__ tile_bins, const float4* __restrict__ rec, const float* __restrict__ background,
     const float* __restrict__ final_Ts, const int* __restrict__ final_idx, const float* __restrict__ v_output,
     const float* __restrict__ v_output_alpha, float* __restrict__ v_xy, float* __restrict__ v_conic,
@@ -541,10 +541,10 @@ __global__ void __launch_bounds__(kBwdThreads, 3) blend_bwd_mom_kernel(
       const int hh = lane & 15, half = lane >> 4;
       const int he = min(hh, n - 1);
       const float4 a0 = E[(base + he) * 3], a1 = E[(base + he) * 3 + 1];
-      // the Gaussian id is only needed by the REDs at the end: start its load now (padding entries: index 0 / rank 0)
+      // the Gaussian id is only needed by the REDs at the end: start its load now (padding entries: index 0 / id 0)
       const int e_idx = __float_as_int(a1.z);
       const int e_safe = e_idx == 0x7fffffff ? range.x : e_idx;
-      const int g_id = RANKED ? gids_sorted[__float_as_int(a1.w)] : gids_sorted[e_safe];
+      const int g_id = RANKED ? __float_as_int(a1.w) : gids_sorted[e_safe];
       const float2* Mrow = M + hh * kMStride + half * 16;
       const float4* V = VO + half * 16;
       float g[4] = {0.f, 0.f, 0.f, 0.f};
@@ -636,8 +636,8 @@ __global__ void __launch_bounds__(kBwdThreads, 3) blend_bwd_mom_kernel(
         const float4 q0 = sr[tj * 3], q1 = sr[tj * 3 + 1], q2 = sr[tj * 3 + 2];
         E[pos * 3 + 0] = make_float4(q0.x, q0.y, q1.x, q1.y);
         if constexpr (RANKED) {
-          // the entry's 4th word gets the hit's depth rank, copied asynchronously (chunk() waits for it before phase
-          // B): phase B then finds the Gaussian id with one dependent load, rank_to_gid[rank], instead of two
+          // the entry's 4th word gets the hit's Gaussian id (the list entry), copied asynchronously (chunk() waits for
+          // it before phase B), so phase B needs no dependent load to find it
           float* e1 = reinterpret_cast<float*>(&E[pos * 3 + 1]);
           *reinterpret_cast<float2*>(e1) = make_float2(q1.z, q1.w);
           e1[2] = __int_as_float(lo + tj);
@@ -1243,9 +1243,9 @@ int launch_bwd_mom(int img_h, int img_w, int channels, const int32_t* gids_sorte
 
 }  // namespace gbblend
 
-// ---------------------------------------------------------------- blend straight from the by-rank record table, C ABI
-// ranks_sorted [cap] (per tile: depth ranks in blend order), rec_by_rank [G,12], rank_to_gid [G]: outputs of
-// gb_bin_tiles_ranked.  Same results as gb_rasterize_packed_fwd/bwd on the materialised records; final_idx indexes
+// ---------------------------------------------------------------- blend straight from the by-id record table, C ABI
+// ranks_sorted [cap] (per tile: Gaussian ids in blend order), rec_by_rank [G,12] (by id), rank_to_gid [G] (identity,
+// not read): outputs of gb_bin_tiles_ranked.  Same results as gb_rasterize_packed_fwd/bwd on the materialised records; final_idx indexes
 // ranks_sorted.  channels 3 or 4; tile_order as for the packed kernels (launch order, may be NULL).
 GB_API int gb_rasterize_ranked_fwd(int img_h, int img_w, int channels, const int32_t* tile_bins, const int32_t* tile_order,
                                    const int32_t* ranks_sorted, const float* rec_by_rank, const float* background,

@@ -21,9 +21,9 @@ _OVERFLOW = {}
 BINNING = os.environ.get("GOLIATH_B200_BINNING", "buckets")
 # sync-free path as two autograd nodes (projection | binning + blend), see render_fused_split; "0" keeps the single node
 SPLIT = os.environ.get("GOLIATH_B200_RENDER_SPLIT", "1") != "0"
-# records of the two-node path: "ranked" (default: the blend stages records by depth rank from the per-Gaussian table,
+# records of the two-node path: "ranked" (default: the blend stages records by Gaussian id from the per-Gaussian table,
 # G x 48 B, with 16-byte cp.async gathers) or "packed" (sorted 48-byte records materialised by the binning's gather,
-# cap x 48 B).  On an H100 the by-rank table (14.4 MB at 300k Gaussians) stays in the 50 MB L2 between the binning and
+# cap x 48 B).  On an H100 the by-id table (14.4 MB at 300k Gaussians) stays in the 50 MB L2 between the binning and
 # the two blends, the sorted records (52 MB on the bench head scene) do not.  Measured on an H100 SXM at a 700 W power
 # limit (scripts/profile_head_step.py): the ranked blends cost ~2 us (forward) and ~10 us (backward) more than the
 # packed ones, the record gather they make unnecessary cost ~50 us, and the bench head step takes 0.557 instead of
@@ -94,8 +94,8 @@ class _RenderFused(Function):
                 order = torch.empty(L.gb_tile_schedule_ints(T) if sched else T, **i32)
                 records = torch.empty(cap, 12, **f32)
                 if BINNING == "buckets" and L.gb_bin_tiles_supported(G):
-                    # depth ranks + per-tile buckets ordered by a rank bitmap (csrc/splat_bin_tiles.cu): same bins,
-                    # ids and records as the key sort below, without sorting the intersection keys
+                    # per-tile buckets, each sorted by (depth, id) in shared memory (csrc/splat_bin_tiles.cu): same
+                    # bins, ids and records as the key sort below, without sorting the intersection keys globally
                     bins = torch.empty(T, 2, **i32)
                     ws = _workspace(dev, L.gb_bin_tiles_workspace_bytes(G, T, cap))
                     _lib.check(L.gb_bin_tiles_pack(G, _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii),
@@ -278,13 +278,13 @@ class _BinBlend(Function):
             if colors_event is not None:
                 ev = colors_event.cuda_event
                 colors.record_stream(torch.cuda.current_stream(dev))
-            # rank-staged records (the default with the mom blend and launch-order tiles): the blend gathers each stage
-            # from the by-rank table, the sorted 48-byte records are never materialised (csrc/splat_blend_mom.cu, RANKED)
+            # id-staged records (the default with the mom blend and launch-order tiles): the blend gathers each stage
+            # from the by-id table, the sorted 48-byte records are never materialised (csrc/splat_blend_mom.cu, RANKED)
             ranked = RANKED and not sched and L.gb_get_blend_mode() == 3
             if ranked:
-                gids = torch.empty(G, **i32)            # rank -> Gaussian id
-                ranks = torch.empty(cap, **i32)         # per tile: depth ranks in blend order
-                records = torch.empty(G, 12, **f32)     # one record per Gaussian, by rank
+                gids = torch.empty(G, **i32)            # identity (the C ABI's rank_to_gid)
+                ranks = torch.empty(cap, **i32)         # per tile: Gaussian ids in blend order
+                records = torch.empty(G, 12, **f32)     # one record per Gaussian, by id
                 _lib.check(L.gb_bin_tiles_ranked(G, _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics),
                                                  _lib.ptr(colors), _lib.ptr(opacity), _lib.ptr(comp), H, W, BW, cap,
                                                  _lib.ptr(bins), _lib.ptr(order), sched, _lib.ptr(ranks),
@@ -345,7 +345,7 @@ class _BinBlend(Function):
 def render_fused_split(means3d, scales, glob_scale, quats, viewmat, fx, fy, cx, cy, img_height, img_width, opacity, colors,
                        background, clip_thresh, capacity, colors_event=None):
     """render_fused(capacity=N) as TWO autograd nodes — projection | binning + blend — with the same kernels.  What the
-    split buys: the projection, the depth ranks, the tile buckets and the per-tile sort do not read the colours, so a
+    split buys: the projection, the tile counts, the tile buckets and the per-tile sort do not read the colours, so a
     caller that runs its shade on a side stream (and passes the event recorded after it) gets them beside the shade
     forward; in the backward autograd finds the projection backward and the shade backward independent (both only need
     this node's gradients) and issues them on their own streams.  Requires the bucket binning and G >= 1."""

@@ -38,7 +38,7 @@ class _RenderShared(Function):
         dev = means3d.device
         L = _lib.lib()
         if not L.gb_bin_tiles_supported(G):
-            raise RuntimeError("render_shared: %d Gaussians exceed the bucket binning's shared-memory bitmap" % G)
+            raise RuntimeError("render_shared: %d Gaussians exceed the bucket binning's range (gb_bin_tiles_supported)" % G)
         f32 = dict(device=dev, dtype=torch.float32)
         i32 = dict(device=dev, dtype=torch.int32)
         cov3d, xys, depths = torch.empty(G, 6, **f32), torch.empty(G, 2, **f32), torch.empty(G, **f32)

@@ -162,13 +162,9 @@ int gb_pack_records_fused_dn(int64_t cap, const int32_t* n_dev, const int32_t* g
                              const float* conics, const float* colors3, const float* depths, const float* opacity,
                              const float* compensation, float* records, void* stream);
 
-/* depth ranks inside gb_bin_tiles_pack: 0 = one cooperative LSD kernel over the key bits that vary (default), 1 = four
- * radix passes as separate launches (round 1), 2 = 2048 key buckets + in-bucket ranking of the visible Gaussians (a
- * device flag hands degenerate depth distributions to the cooperative sort; measured slower).  Identical outputs.
- * GOLIATH_B200_RANKSORT=coop|passes|buckets. */
+/* gb_bin_tiles_pack has one formulation (per-tile buckets, each sorted by (depth, id) in shared memory): both getters
+ * return 0 and both setters accept and ignore any value.  Kept so that callers which label or select modes work. */
 int gb_get_rank_sort_mode(void);
-/* per-tile ordering inside gb_bin_tiles_pack: 0 = bitmap sort per tile + one grid-wide record gather (default), 1 = one
- * kernel per tile doing both (round 1).  Identical outputs.  GOLIATH_B200_TILESORT=split|fused. */
 int gb_get_tile_sort_mode(void);
 void gb_set_tile_sort_mode(int mode);
 void gb_set_rank_sort_mode(int mode);
@@ -176,12 +172,12 @@ void gb_set_rank_sort_mode(int mode);
 /* Bucket binning of the fused render (csrc/splat_bin_tiles.cu): replaces, for the fused path, the whole of gsplat
  * 0.1.11 bin_and_sort_gaussians (compute_cumulative_intersects, map_gaussian_to_intersects, torch.sort,
  * get_tile_bin_edges — call sites ca_code/utils/render_gsplat.py:65-78,90-104) plus the record packing, with the same
- * bit-exact outputs: Gaussians are depth-ranked once (G keys), intersections are bucketed per tile with atomics, and
- * each tile's bucket is ordered with a rank bitmap in shared memory.  Outputs: tile_bins [T,2], tile_order [T]
+ * bit-exact outputs: intersections are bucketed per tile with atomics (Gaussian ids), and one CTA per tile sorts its
+ * bucket by (depth key, id) with a radix sort in shared memory (tiles longer than 5120 entries: through global memory).  Outputs: tile_bins [T,2], tile_order [T]
  * (tile_sched = 1: an SM-affine schedule of gb_tile_schedule_ints(T) int32 instead, see gb_tile_schedule),
  * gids_sorted [cap], records [cap,12]; n_out (device int32, may be NULL) = true intersection count; *overflow = 1
  * when it exceeds cap (the excess is dropped).  Sync-free, never allocates, capturable in a CUDA graph. */
-int gb_bin_tiles_supported(int G); /* 1 if one tile's G-bit rank bitmap fits in shared memory */
+int gb_bin_tiles_supported(int G); /* 1 for 1 <= G <= 1.5 x 2^20 (1572864) Gaussians per view */
 size_t gb_bin_tiles_workspace_bytes(int G, int num_tiles, int64_t cap);
 int gb_bin_tiles_pack(int G, const float* xys, const float* depths, const int32_t* radii, const float* conics,
                       const float* colors3, const float* opacity, const float* compensation, int img_h, int img_w,
@@ -189,8 +185,8 @@ int gb_bin_tiles_pack(int G, const float* xys, const float* depths, const int32_
                       int32_t* gids_sorted, float* records, int32_t* n_out, int32_t* overflow, void* workspace,
                       void* stream);
 /* Same, with colors3 allowed to arrive late: colors_ready (cudaEvent_t recorded on the stream that writes colors3, or
- * NULL) is waited for on `stream` just before the first kernel that reads colors3 (with the split tile sort: a small
- * kernel after the per-tile sort), so ranks, buckets and the per-tile sort run beside the caller's shade (rgca.py:557-575 precedes
+ * NULL) is waited for on `stream` just before the first kernel that reads colors3 (a small kernel after the per-tile
+ * sort), so counts, buckets and the per-tile sort run beside the caller's shade (rgca.py:557-575 precedes
  * render_gsplat.py:65 in the reference; only the colours depend on it). */
 int gb_bin_tiles_pack_ev(int G, const float* xys, const float* depths, const int32_t* radii, const float* conics,
                          const float* colors3, const float* opacity, const float* compensation, int img_h, int img_w,
@@ -198,18 +194,19 @@ int gb_bin_tiles_pack_ev(int G, const float* xys, const float* depths, const int
                          int32_t* gids_sorted, float* records, int32_t* n_out, int32_t* overflow, void* workspace,
                          void* colors_ready, void* stream);
 
-/* Binning WITHOUT the sorted-record gather, for gb_rasterize_ranked_fwd/bwd: ranks_sorted [cap] (per tile, the depth ranks
- * in blend order), rec_by_rank [G,12] (one 48-byte record per visible Gaussian, at its depth rank) and rank_to_gid [G] are
- * written to the CALLER's arrays (they must live until the backward).  Everything else as gb_bin_tiles_pack_ev.  No
+/* Binning WITHOUT the sorted-record gather, for gb_rasterize_ranked_fwd/bwd: ranks_sorted [cap] (per tile, the Gaussian
+ * ids in blend order), rec_by_rank [G,12] (one 48-byte record per visible Gaussian, at its id) and rank_to_gid [G] (the
+ * identity: ranks_sorted already holds ids) are written to the CALLER's arrays (they must live until the backward).  Everything else as gb_bin_tiles_pack_ev.  No
  * counterpart in gsplat: it replaces the per-intersection sorted arrays of bin_and_sort_gaussians by per-Gaussian ones. */
 int gb_bin_tiles_ranked(int G, const float* xys, const float* depths, const int32_t* radii, const float* conics,
                         const float* colors3, const float* opacity, const float* compensation, int img_h, int img_w,
                         int block_width, int64_t cap, int32_t* tile_bins, int32_t* tile_order, int tile_sched,
                         int32_t* ranks_sorted, float* rec_by_rank, int32_t* rank_to_gid, int32_t* n_out, int32_t* overflow,
                         void* workspace, void* colors_ready, void* stream);
-/* Blend straight from the by-rank table (csrc/splat_blend_mom.cu, RANKED staging: 16-byte cp.async gathers by rank into
- * the stage ring instead of bulk copies of materialised sorted records).  Same results as gb_rasterize_packed_fwd/bwd;
- * final_idx indexes ranks_sorted.  channels 3 or 4; tile_order = launch order (gb_tile_order) or NULL. */
+/* Blend straight from the by-id table of gb_bin_tiles_ranked (csrc/splat_blend_mom.cu, RANKED staging: 16-byte cp.async
+ * gathers by list entry into the stage ring instead of bulk copies of materialised sorted records).  Same results as
+ * gb_rasterize_packed_fwd/bwd; final_idx indexes ranks_sorted.  The backward takes each hit's Gaussian id from
+ * ranks_sorted and does not read rank_to_gid (kept in the signature; gb_bin_tiles_ranked writes it as the identity).  channels 3 or 4; tile_order = launch order (gb_tile_order) or NULL. */
 int gb_rasterize_ranked_fwd(int img_h, int img_w, int channels, const int32_t* tile_bins, const int32_t* tile_order,
                             const int32_t* ranks_sorted, const float* rec_by_rank, const float* background,
                             float* out_img, float* final_Ts, int32_t* final_idx, void* stream);
