@@ -105,7 +105,10 @@ SIGNATURES = {
     "gb_ssim_l1_bwd": (_i, [_i, _i, _i] + [_vp] * 8 + [_f, _f, _vp, _vp]),
     "gb_envmap_spec_fwd": (_i, [_i, _i, _i] + [_vp] * 6 + [_f, _vp, _vp]),
     "gb_envmap_spec_bwd": (_i, [_i, _i, _i] + [_vp] * 6 + [_f, _vp, _vp, _vp, _vp]),
-    "gb_mvp_raymarch_bwd": (_i, [_i] * 4 + [_vp, _vp, _f] + [_vp] * 5 + [_i] * 3 + [_vp] + [_i] * 3 + [_vp] * 8
+    "gb_envmap_rotate": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp]),
+    "gb_envmap_compose_fwd": (_i, [_i] * 5 + [_vp] * 5 + [_i, _i, _vp, _vp, _vp]),
+    "gb_envmap_compose_bwd": (_i, [_i, _i, _i, _vp, _vp, _vp]),
+    "gb_mvp_raymarch_bwd":(_i, [_i] * 4 + [_vp, _vp, _f] + [_vp] * 5 + [_i] * 3 + [_vp] + [_i] * 3 + [_vp] * 8
                             + [_i, _f, _f, _i, _i, _vp]),
 }
 

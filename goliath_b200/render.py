@@ -238,3 +238,28 @@ def render_views(width: int, height: int, K: th.Tensor, Rt: th.Tensor, preds, in
     alpha = 1.0 - th.stack(Ts)
     depth = depth / alpha.clamp(0.05, 1.0)
     return rgb, alpha, depth
+
+
+def render_views_envmap(width: int, height: int, K: th.Tensor, headrel_Rt: th.Tensor, Rt: th.Tensor, preds, envbg,
+                        intrinsics_host=None, capacity=None):
+    """The environment-map frame of rgca.AutoEncoder.forward (rgca.py:221,232-245) with calibration, background and
+    learnable blur off (run_vis_relight's evaluation setting): three renders with identical geometry — preds["color"],
+    preds["diff_color"].clamp(0), preds["spec_color"].clamp(0) — the first composited over the environment
+    (goliath_b200.envmap.compose_envmap with the WORLD camera Rt; the renders use headrel_Rt, as the reference does).
+    The three colour sets go through gsplat.olat.render_views_shared: one projection and one binning per view instead
+    of the reference's three.  Returns rgb [B,3,H,3W] = cat(full, diffuse, specular, -1), alpha [B,1,H,W] (detached)
+    and depth [B,1,H,W].  With `capacity` and `intrinsics_host` ((fx, fy, cx, cy) per view) the frame runs without a
+    host synchronisation and can be captured in a CUDA graph.  Unlike the reference, which leaves preds["color"] set to
+    the specular colours, `preds` is not modified."""
+    from .envmap import compose_envmap
+    from .gsplat.olat import render_views_shared
+
+    B = headrel_Rt.shape[0]
+    if intrinsics_host is None:
+        intrinsics_host = [(K[b, 0, 0].item(), K[b, 1, 1].item(), K[b, 0, 2].item(), K[b, 1, 2].item()) for b in range(B)]
+    colors = th.stack([preds["color"].reshape(B, -1, 3), preds["diff_color"].reshape(B, -1, 3).clamp(min=0.0),
+                       preds["spec_color"].reshape(B, -1, 3).clamp(min=0.0)], 1)
+    geom = {k: preds[k] for k in ("primpos", "primqvec", "primscale", "opacity")}
+    rgb, alpha, depth = render_views_shared(width, height, headrel_Rt, geom, colors, intrinsics_host, capacity=capacity)
+    full = compose_envmap(rgb[:, 0], alpha, envbg, K, Rt)
+    return th.cat([full, rgb[:, 1], rgb[:, 2]], -1), alpha, depth

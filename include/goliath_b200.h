@@ -396,6 +396,30 @@ int gb_envmap_spec_bwd(int B, int G, int q, const float* const* levels, const in
                        const float* sigma, const float* spec_vis, const float* lightrot, float level_scale,
                        const float* g_spec, float* g_ref_dirs, float* g_spec_vis, void* stream);
 
+/* replaces rotate_envmap_mat (ca_code/utils/envmap.py:141-166), batched over B: texel grid
+ * theta = (i + 0.5) * 3.1415926 / He, phi = (j - We//2 + 0.5) * 3.1415926 * 2 / We, vec = (sin t sin p, cos t, sin t cos p),
+ * vec @ R^T (= R vec) clamped to [-1, 1] per component, dir2uv (np.pi), bilinear grid_sample (border padding,
+ * align_corners=False).  image / out [B,3,He,We], rot_mat [B,3,3] (row-major R). */
+int gb_envmap_rotate(int B, int He, int We, const float* image, const float* rot_mat, float* out, void* stream);
+/* replaces compose_envmap (ca_code/utils/envmap.py:325-345) with envmap_to_image (:169-227, focal_scale 0.2, blurbg,
+ * no fisheye D) and envmap_to_mirrorball (:230-248, 200x200):
+ *   rays d = ((x - K[0,2]) / (0.2 K[0,0]), (y - K[1,2]) / (0.2 K[1,1]), 1), rotated R^T d (einsum "bxy,bhwx->bhwy" with
+ *   R = Rt[:3,:3]), normalised, dir2uv; bicubic grid_sample (A = -0.75, border padding applied to each of the 16 taps,
+ *   align_corners=True); the 101x101 blur k(x)k / sum(k(x)k), k = exp(-linspace(-4, 4, 101)^2), zero padding 50, run as
+ *   two separable 101-tap passes; bg' = render + (1 - alpha) * clamp(bg, 0, 1); out = (1 - m) * bg' + m * mirror in the
+ *   bottom-right 200x200 corner, m = (zsq < 1) on torch's linspace(-1, 1, 200) grid, mirror colour unclamped.
+ * acos is taken without a clamp, as the reference does: where rounding (or a non-orthonormal Rt) pushes the y
+ * component past +-1, the sample is NaN, the blur spreads it over the 101x101 neighbourhood, and the mirror ball
+ * (whose reflected directions are not normalised) turns NaN at that pixel and, through m * NaN, at masked-out
+ * pixels of the corner too; clamp keeps NaN.
+ * render / out [B,3,H,W], alpha [B,1,H,W], envbg [B,3,He,We], K [B,3,3], Rt [B,rt_rows,rt_cols] (rt_rows, rt_cols >= 3),
+ * all in device memory (no host sync); hblur [B,3,H,W] scratch.  H, W >= 200. */
+int gb_envmap_compose_fwd(int B, int H, int W, int He, int We, const float* render, const float* alpha,
+                          const float* envbg, const float* K, const float* Rt, int rt_rows, int rt_cols, float* hblur,
+                          float* out, void* stream);
+/* the only gradient of compose_envmap (alpha detached, envbg / K / Rt data): g_render = (1 - m) * g_out [B,3,H,W]. */
+int gb_envmap_compose_bwd(int B, int H, int W, const float* g_out, float* g_render, void* stream);
+
 /* replaces the per-view post-processing of rgca.AutoEncoder.render (ca_code/models/rgca.py:136-151, with
  * render_gsplat.py:79-108): colour HWC -> CHW, alpha = 1 - final_T (detached), depth / alpha.clamp(0.05, 1).
  * out4 [H,W,4] = rgb + depth-as-colour, alpha [H,W] -> rgb [3,H,W], alpha_img [1,H,W], depth [1,H,W]. */
