@@ -20,12 +20,16 @@
 //                            one atomicAdd per (CTA, tile) on the global cursor, then shared-memory atomics hand out
 //                            the slots.  The same threads write the 48-byte blend record of their Gaussian into a
 //                            table indexed BY ID (cull box computed once per Gaussian, not once per intersection).
-//   4. tile_sort_kernel      one CTA per tile, in launch order: a stable LSD radix sort of the bucket on the 64-bit
-//                            key (depth bits - tile minimum) << id bits | (id - tile minimum), 9-bit digits, over the
-//                            bits that vary inside the tile only (CTA min/max reduction).  Buckets of up to
-//                            kSortCap entries are sorted in registers + shared memory; longer ones run the same
-//                            passes chunk by chunk through global memory (the bucket and the output array serve as
-//                            the ping-pong pair).  The sorted ids go to the output array.
+//   4. tile_sort_kernel      one CTA per tile, in launch order, on the 64-bit key (depth bits - tile minimum) << id
+//                            bits | (id - tile minimum), over the bits that vary inside the tile only (CTA min/max
+//                            reduction).  Buckets of up to kSortCap entries are spread over all warps and sorted in
+//                            registers + shared memory by stable LSD passes (9-bit digits) over the DEPTH bits only;
+//                            the id bits only break ties, and ties come in short runs (at most 3 entries on the bench
+//                            head), so the thread holding the first entry of each equal-depth run then sorts the run
+//                            by the full key in place.  A tile with a run longer than kTieRun runs the passes over the
+//                            full key instead.  Longer buckets run the full-key passes chunk by chunk through global
+//                            memory (the bucket and the output array serve as the ping-pong pair).  The sorted ids go
+//                            to the output array.
 //   5. gather_records_kernel (packed callers only) the sorted 48-byte records, copied from the by-id table.
 //
 // Integer/byte work with a BIT-EXACT contract: gids_sorted, tile_bins and records are identical to the
@@ -58,11 +62,14 @@ constexpr int kMaxGaussians = 3 << 19;
 // tiles (the counts above 6144 and above 4096) take the chunked path.
 constexpr int kSortThreads = 512;
 constexpr int kSortWarps = kSortThreads / 32;
-constexpr int kSortItems = 10;                        // entries per thread
+constexpr int kSortItems = 10;                        // entries per thread, at most
 constexpr int kSortCap = kSortThreads * kSortItems;
 constexpr int kDigitBits = 9;
 constexpr int kDigits = 1 << kDigitBits;              // == kSortThreads: thread t owns digit t in the scans
 static_assert(kDigits == kSortThreads, "one digit per thread");
+// Longest run of equal depth keys that one thread sorts by id in place after the depth passes.  The bench head's
+// tiles tie in ~70 % of tiles but in runs of at most 3 entries; a tile with a longer run re-sorts on the full key.
+constexpr int kTieRun = 16;
 
 // Gaussians per CTA of tile_count_kernel: 2048 up to ~400k Gaussians, 4096 beyond (fewer counter flushes)
 inline int count_items(int G) { return G <= 2048 * 192 ? 2 : 4; }
@@ -251,25 +258,32 @@ struct SortSmem {
   unsigned red[4];                            // min / max of the depth keys and of the ids
 };
 
-// Entry e of a chunk is held by warp e / (32 kSortItems), item (e / 32) % kSortItems, lane e % 32: "earlier in the
-// chunk" == (smaller warp, then smaller item, then smaller lane), which the per-warp ranking below preserves.
-__device__ __forceinline__ int entry_of(int j) {
-  return (threadIdx.x >> 5) * (32 * kSortItems) + j * 32 + (threadIdx.x & 31);
+// With ipt items per thread (ipt <= kSortItems), entry e of a chunk is held by warp e / (32 ipt), item (e / 32) % ipt,
+// lane e % 32: "earlier in the chunk" == (smaller warp, then smaller item, then smaller lane), which the per-warp
+// ranking below preserves.
+__device__ __forceinline__ int entry_of(int j, int ipt) {
+  return (threadIdx.x >> 5) * (32 * ipt) + j * 32 + (threadIdx.x & 31);
 }
 
+// item j of this thread is one of the m entries of the chunk
+__device__ __forceinline__ bool holds(int j, int ipt, int m) { return j < ipt && entry_of(j, ipt) < m; }
+
 // One stable counting pass on digit (key >> shift) & (kDigits - 1) over the m valid entries of a chunk held in
-// registers: dst[j] = destination of item j.  whole: the chunk is the whole list (bases = exclusive scan of this
-// chunk's counts); else the bases come from s.run, which is advanced by this chunk's counts.
-__device__ __forceinline__ void radix_positions(const unsigned long long (&k)[kSortItems], int m, int shift, bool whole,
-                                                SortSmem& s, int (&dst)[kSortItems]) {
+// registers, ipt per thread: dst[j] = destination of item j.  whole: the chunk is the whole list (bases = exclusive
+// scan of this chunk's counts); else the bases come from s.run, which is advanced by this chunk's counts.
+__device__ __forceinline__ void radix_positions(const unsigned long long (&k)[kSortItems], int m, int ipt, int shift,
+                                                bool whole, SortSmem& s, int (&dst)[kSortItems]) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  // items held by this warp and by this thread: item j is valid iff j < mine
+  const int wbase = warp * (32 * ipt);
+  const int ours = min(ipt, max(0, (m - wbase + 31) >> 5)), mine = min(ipt, max(0, (m - wbase - lane + 31) >> 5));
   for (int d = lane; d < kDigits; d += 32) s.whist[warp][d] = 0;
   __syncwarp();
 #pragma unroll
   for (int j = 0; j < kSortItems; ++j) {  // dst[j] = rank among the equal digits of this warp's earlier entries
     dst[j] = 0;
-    if (warp * (32 * kSortItems) + j * 32 >= m) continue;  // warp-uniform
-    const bool valid = entry_of(j) < m;
+    if (j >= ours) continue;  // warp-uniform
+    const bool valid = j < mine;
     const unsigned dgt = (unsigned)(k[j] >> shift) & (kDigits - 1);
     // lanes holding the same digit: one ballot per digit bit (__match_any_sync serialises over the ~30 distinct
     // digits a warp holds)
@@ -310,8 +324,24 @@ __device__ __forceinline__ void radix_positions(const unsigned long long (&k)[kS
 #pragma unroll
   for (int j = 0; j < kSortItems; ++j) {
     const unsigned dgt = (unsigned)(k[j] >> shift) & (kDigits - 1);
-    dst[j] = (entry_of(j) < m) ? s.base[dgt] + s.whist[warp][dgt] + dst[j] : -1;
+    dst[j] = (j < mine) ? s.base[dgt] + s.whist[warp][dgt] + dst[j] : -1;
   }
+}
+
+// One pass of the shared-memory sort: the n keys (ipt per thread) go to s_key in digit order, and every thread
+// reloads its items from there.
+__device__ __forceinline__ void smem_pass(unsigned long long (&k)[kSortItems], int n, int ipt, int shift, SortSmem& s,
+                                          unsigned long long* s_key) {
+  int dst[kSortItems];
+  radix_positions(k, n, ipt, shift, true, s, dst);
+#pragma unroll
+  for (int j = 0; j < kSortItems; ++j)
+    if (dst[j] >= 0) s_key[dst[j]] = k[j];
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < kSortItems; ++j)
+    if (holds(j, ipt, n)) k[j] = s_key[entry_of(j, ipt)];
+  // the next pass overwrites s_key only after the barriers inside radix_positions
 }
 
 __device__ __forceinline__ void minmax_to_smem(unsigned kmin, unsigned kmax, unsigned imin, unsigned imax, SortSmem& s) {
@@ -348,10 +378,11 @@ __global__ void __launch_bounds__(kSortThreads, 2) tile_sort_kernel(const int* _
   __syncthreads();
 
   if (n <= kSortCap) {
+    const int ipt = (n + kSortThreads - 1) / kSortThreads;  // the tile spread over all warps
     int id[kSortItems];
     unsigned dk[kSortItems];
 #pragma unroll
-    for (int j = 0; j < kSortItems; ++j) id[j] = (entry_of(j) < n) ? bucket[range.x + entry_of(j)] : -1;
+    for (int j = 0; j < kSortItems; ++j) id[j] = holds(j, ipt, n) ? bucket[range.x + entry_of(j, ipt)] : -1;
     unsigned kmin = 0xffffffffu, kmax = 0u, imin = 0xffffffffu, imax = 0u;
 #pragma unroll
     for (int j = 0; j < kSortItems; ++j) {
@@ -370,26 +401,53 @@ __global__ void __launch_bounds__(kSortThreads, 2) tile_sort_kernel(const int* _
 #pragma unroll
     for (int j = 0; j < kSortItems; ++j)
       k[j] = ((unsigned long long)(dk[j] - kmin) << bi) | (unsigned long long)((unsigned)id[j] - imin);
-    for (int shift = 0; shift < bits; shift += kDigitBits) {
-      int dst[kSortItems];
-      radix_positions(k, n, shift, true, s, dst);
+    // stable passes over the depth bits only: s_key ends in depth order, equal depth keys in bucket order
+    for (int shift = bi; shift < bits; shift += kDigitBits) smem_pass(k, n, ipt, shift, s, s_key);
+    if (bits == bi) {  // one depth key over the whole tile: no pass ran
 #pragma unroll
       for (int j = 0; j < kSortItems; ++j)
-        if (dst[j] >= 0) s_key[dst[j]] = k[j];
+        if (holds(j, ipt, n)) s_key[entry_of(j, ipt)] = k[j];
       __syncthreads();
+    }
+    // ties: find every run of equal depth keys (read only), then the thread holding its first entry sorts the run by
+    // id in place.  A run longer than kTieRun sends the whole tile through the passes on the full key instead.
+    static_assert(kTieRun < 32 && kSortItems * 5 <= 64, "run lengths are packed 5 bits per item");
+    unsigned long long runs = 0ull;  // 5 bits per item: length of the run it starts (0: none)
+    bool too_long = false;
 #pragma unroll
-      for (int j = 0; j < kSortItems; ++j)
-        if (entry_of(j) < n) k[j] = s_key[entry_of(j)];
-      // the next pass overwrites s_key only after the barriers inside radix_positions
+    for (int j = 0; j < kSortItems; ++j) {
+      const int e = j * kSortThreads + threadIdx.x;
+      if (j >= ipt || e >= n) continue;
+      const unsigned long long d = s_key[e] >> bi;
+      if (e > 0 && (s_key[e - 1] >> bi) == d) continue;  // not the first entry of its run
+      int len = 1;
+      while (len <= kTieRun && e + len < n && (s_key[e + len] >> bi) == d) ++len;
+      if (len > kTieRun) too_long = true;
+      else runs |= (unsigned long long)len << (5 * j);
+    }
+    if (__syncthreads_or(too_long)) {
+#pragma unroll
+      for (int j = 0; j < kSortItems; ++j) k[j] = holds(j, ipt, n) ? s_key[entry_of(j, ipt)] : 0ull;
+      for (int shift = 0; shift < bits; shift += kDigitBits) smem_pass(k, n, ipt, shift, s, s_key);
+    } else {
+#pragma unroll
+      for (int j = 0; j < kSortItems; ++j) {
+        const int e = j * kSortThreads + threadIdx.x, len = (int)(runs >> (5 * j)) & 31;
+        for (int a = e + 1; a < e + len; ++a) {  // insertion sort of s_key[e, e + len)
+          const unsigned long long v = s_key[a];
+          int b = a;
+          for (; b > e && s_key[b - 1] > v; --b) s_key[b] = s_key[b - 1];
+          s_key[b] = v;
+        }
+      }
+      __syncthreads();
     }
     const unsigned long long imask = (1ull << bi) - 1ull;
-#pragma unroll
-    for (int j = 0; j < kSortItems; ++j)
-      if (entry_of(j) < n) out[range.x + entry_of(j)] = (int)(imin + (unsigned)(k[j] & imask));
+    for (int e = threadIdx.x; e < n; e += kSortThreads) out[range.x + e] = (int)(imin + (unsigned)(s_key[e] & imask));
     return;
   }
 
-  // ---- long bucket: the same passes chunk by chunk (kSortCap entries in registers at a time) through global memory,
+  // ---- long bucket: the full-key passes chunk by chunk (kSortCap entries in registers at a time) through global memory,
   // ids ping-ponging between bucket and out (each pass recomputes the keys from the ids); one CTA, slow but exact
   {
     unsigned kmin = 0xffffffffu, kmax = 0u, imin = 0xffffffffu, imax = 0u;
@@ -425,9 +483,10 @@ __global__ void __launch_bounds__(kSortThreads, 2) tile_sort_kernel(const int* _
       const int m = min(kSortCap, n - c0);
       unsigned long long k[kSortItems];
 #pragma unroll
-      for (int j = 0; j < kSortItems; ++j) k[j] = (entry_of(j) < m) ? key_of(src[c0 + entry_of(j)]) : 0ull;
+      for (int j = 0; j < kSortItems; ++j)
+        k[j] = holds(j, kSortItems, m) ? key_of(src[c0 + entry_of(j, kSortItems)]) : 0ull;
       int dst[kSortItems];
-      radix_positions(k, m, shift, false, s, dst);
+      radix_positions(k, m, kSortItems, shift, false, s, dst);
 #pragma unroll
       for (int j = 0; j < kSortItems; ++j)
         if (dst[j] >= 0) dstp[dst[j]] = (int)(imin + (unsigned)(k[j] & imask));
