@@ -16,10 +16,12 @@
 //                            scatter cursors, total count, overflow flag.  Then the launch order of the tiles
 //                            (gb_tile_order, longest first, or the SM-affine schedule of gb_tile_schedule).
 //   3. tile_scatter_kernel   G threads: every (Gaussian, tile) pair drops the Gaussian's ID into the tile's bucket
-//                            (order inside the bucket arbitrary).  Slots are claimed per CTA: count in shared memory,
-//                            one atomicAdd per (CTA, tile) on the global cursor, then shared-memory atomics hand out
-//                            the slots.  The same threads write the 48-byte blend record of their Gaussian into a
-//                            table indexed BY ID (cull box computed once per Gaussian, not once per intersection).
+//                            (order inside the bucket arbitrary) and its depth key at the same slot of the output
+//                            array.  Slots are claimed per CTA: count in shared memory, one atomicAdd per (CTA, tile)
+//                            on the global cursor; the pairs are staged tile by tile in shared memory and written out
+//                            as runs of consecutive slots.  The same threads write the 48-byte blend record of their
+//                            Gaussian into a table indexed BY ID (cull box computed once per Gaussian, not once per
+//                            intersection), one contiguous span per warp.
 //   4. tile_sort_kernel      one CTA per tile, in launch order, on the 64-bit key (depth bits - tile minimum) << id
 //                            bits | (id - tile minimum), over the bits that vary inside the tile only (CTA min/max
 //                            reduction).  Buckets of up to kSortCap entries are spread over all warps and sorted in
@@ -28,8 +30,8 @@
 //                            head), so the thread holding the first entry of each equal-depth run then sorts the run
 //                            by the full key in place.  A tile with a run longer than kTieRun runs the passes over the
 //                            full key instead.  Longer buckets run the full-key passes chunk by chunk through global
-//                            memory (the bucket and the output array serve as the ping-pong pair).  The sorted ids go
-//                            to the output array.
+//                            memory (the bucket and the output array serve as the ping-pong pair, keys are gathered
+//                            by id).  The sorted ids overwrite the keys in the output array.
 //   5. gather_records_kernel (packed callers only) the sorted 48-byte records, copied from the by-id table.
 //
 // Integer/byte work with a BIT-EXACT contract: gids_sorted, tile_bins and records are identical to the
@@ -37,6 +39,8 @@
 
 #include "common.cuh"
 #include "splat_record.cuh"
+
+#include <algorithm>
 
 extern "C" int gb_tile_order(int num_tiles, const int32_t* tile_bins, int32_t* order, void* stream);
 extern "C" int gb_tile_schedule(int num_tiles, const int32_t* tile_bins, int32_t* sched, void* stream);
@@ -49,7 +53,7 @@ GB_API int gb_bin_tiles_pack_ev(int G, const float* xys, const float* depths, co
 namespace {
 
 constexpr int kGaussBlock = 1024;                     // threads of the per-Gaussian kernels
-constexpr int kScatItems = 2;                         // Gaussians per thread in tile_scatter_kernel
+constexpr int kScatItems = 3;                         // Gaussians per thread in tile_scatter_kernel, at most
 constexpr int kMaxSmemTiles = 20 * 1024;              // per-CTA tile counters (x2 in the scatter) in shared memory
 // Largest view the bucket binning takes (1.5 x 2^20 Gaussians, the native RGCA head has 2^20).  The sort itself has no
 // such bound; the range is what gb_bin_tiles_supported reports to callers, and the fused render (gsplat/fused.py) uses
@@ -188,54 +192,136 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(int T, long long cap, c
   }
 }
 
-// ------------------------------------------------------------------ 3. ids into the tile buckets + by-id records
-// smem_tiles = T: slots claimed per CTA through shared memory (s_cnt | s_base, 2*T ints); 0: one global atomic
-// per (Gaussian, tile).  kGaussBlock threads x kScatItems Gaussians per CTA (see tile_count_kernel).  The tile
+// ------------------------------------------------------------------ 3. ids + depth keys into the tile buckets, by-id records
+// Every (Gaussian, tile) pair puts the Gaussian's id at a slot of the tile's bucket (tile_ids) and its 32-bit depth key
+// at the same slot of `keys` (the caller's output array, which the sort overwrites with sorted ids), so the sort reads
+// both contiguously instead of gathering depth_keys[id].
+//
+// smem_tiles = T: slots claimed per CTA through shared memory; 0: one global atomic per (Gaussian, tile).
+// per_cta Gaussians per CTA (a multiple of 32, at most kScatItems x kGaussBlock; see scatter_per_cta).  The tile
 // rectangles come from tile_count_kernel, so both kernels walk the same tiles by construction.
+//
+// The kernel's time went into stores, not atomics.  On the bench head (H100 80GB HBM3, 700 W, 1980 MHz max SM clock)
+// the record pack took 17 us of 42 and the placement walk 20 us, and making the placement atomic non-returning changed
+// nothing: one 4-byte store per pair scattered over the whole bucket, and 16-byte record parts at a 48-byte stride,
+// cost about as much per store as full sectors would.  So with stage_cap > 0 both go through shared memory:
+//   - each warp writes the records of its 32 consecutive Gaussians as one contiguous 1536-byte span;
+//   - the CTA's pairs are placed tile by tile into a staging buffer of stage_cap (id, key, tile) entries, then written
+//     out in that order: the CTA's entries of one tile are consecutive slots of the bucket, written by neighbouring
+//     lanes.  A CTA with more pairs than the buffer holds writes each pair directly at the same slot instead.
+// Dynamic shared memory: s_cnt [T] int | s_off [T] int | s_id [stage_cap] int | s_key [stage_cap] | s_tile [stage_cap]
+// u16.  The record spans (kGaussBlock / 32 warps x 96 float4 = 48 KB) borrow s_id | s_key before the walks.
+constexpr int kStageCap = 12 * 1024;                   // staged pairs per CTA: 8.3k on average on the bench head
+constexpr int kStageMaxTiles = 10 * 1024;              // larger grids leave no room for the staging buffer
+constexpr size_t kStageEntryBytes = 4 + 4 + 2;
+static_assert(kStageCap * 8 >= (kGaussBlock / 32) * 96 * 16, "the record spans fit in s_id | s_key");
+
+// Gaussians per scatter CTA: the view spread over one wave of CTAs (one CTA per SM: 1024 threads and the staging
+// buffer).  A CTA runs its phases (loads, records, count walk, claims and scan, placement, write-out) one after the
+// other between barriers, so a second, nearly empty wave costs almost as much as the first: at 2048 Gaussians per CTA
+// the bench head's 300k took 147 CTAs on the 132 SMs of an H100 SXM, and one wave of 131 took the kernel from 31.9 to
+// 23.7 us.
+inline int scatter_per_cta(int G, int num_sms) {
+  const int per_sm = gb::cdiv(G, num_sms > 0 ? num_sms : 1);
+  return std::min(kScatItems * kGaussBlock, std::max(kGaussBlock, (per_sm + 31) & ~31));
+}
+
+inline int scatter_stage_cap(int smem_tiles) { return (smem_tiles > 0 && smem_tiles <= kStageMaxTiles) ? kStageCap : 0; }
+inline size_t scatter_smem_bytes(int smem_tiles) {
+  return (size_t)((smem_tiles + 3) & ~3) * 8 + (size_t)scatter_stage_cap(smem_tiles) * kStageEntryBytes;
+}
+
 __global__ void __launch_bounds__(kGaussBlock, 1) tile_scatter_kernel(
     int G, const int4* __restrict__ rects, const float2* __restrict__ xys, const float* __restrict__ conics,
     const float* __restrict__ colors3, const float* __restrict__ depths, const float* __restrict__ opacity,
-    const float* __restrict__ comp, int tbx, long long cap, int smem_tiles, int* __restrict__ cursor,
-    int* __restrict__ tile_ids, float4* __restrict__ rec_by_id) {
+    const float* __restrict__ comp, int tbx, long long cap, int per_cta, int smem_tiles, int stage_cap,
+    int* __restrict__ cursor, int* __restrict__ tile_ids, unsigned* __restrict__ keys, float4* __restrict__ rec_by_id) {
   extern __shared__ int s_cnt[];
-  int* s_base = s_cnt + smem_tiles;
+  __shared__ int s_warp[33];
+  const int tpad = (smem_tiles + 3) & ~3;  // keeps the record spans 16-byte aligned
+  int* s_off = s_cnt + tpad;
+  int* s_id = s_off + tpad;
+  unsigned* s_key = reinterpret_cast<unsigned*>(s_id + stage_cap);
+  unsigned short* s_tile = reinterpret_cast<unsigned short*>(s_key + stage_cap);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int t = threadIdx.x; t < smem_tiles; t += kGaussBlock) s_cnt[t] = 0;
-  const int base = blockIdx.x * (kGaussBlock * kScatItems);
+  const int base = blockIdx.x * per_cta, end = min(G, base + per_cta);
   int4 rc[kScatItems];
+  unsigned dk[kScatItems];
 #pragma unroll
   for (int j = 0; j < kScatItems; ++j) {  // all loads first: independent, in flight together
     const int i = base + j * kGaussBlock + threadIdx.x;
-    rc[j] = (i < G) ? rects[i] : make_int4(-1, 0, 0, 0);
+    rc[j] = (i < end) ? rects[i] : make_int4(-1, 0, 0, 0);
+    dk[j] = (i < end) ? __float_as_uint(depths[i]) : 0u;
   }
   __syncthreads();
   unsigned bx[kScatItems], by[kScatItems];  // x0 | x1 << 16, y0 | y1 << 16 (tile coordinates < 65536)
 #pragma unroll
   for (int j = 0; j < kScatItems; ++j) {
     const int i = base + j * kGaussBlock + threadIdx.x;
-    bx[j] = by[j] = 0u;
-    if (rc[j].x < 0) continue;  // culled
-    const int x0 = rc[j].x, y0 = rc[j].y, x1 = rc[j].z, y1 = rc[j].w;
-    bx[j] = (unsigned)x0 | ((unsigned)x1 << 16);
-    by[j] = (unsigned)y0 | ((unsigned)y1 << 16);
-    gb::pack_record_fused(i, xys, conics, colors3, depths, opacity, comp, rec_by_id + 3 * (size_t)i);
-    for (int ty = y0; ty < y1; ++ty)
-      for (int tx = x0; tx < x1; ++tx) {
-        if (smem_tiles) {
-          atomicAdd(&s_cnt[ty * tbx + tx], 1);
-        } else {
-          const int pos = atomicAdd(&cursor[ty * tbx + tx], 1);
-          if ((long long)pos < cap) tile_ids[pos] = i;
-        }
+    const bool vis = rc[j].x >= 0;  // false: culled or past the CTA's Gaussians
+    bx[j] = vis ? (unsigned)rc[j].x | ((unsigned)rc[j].z << 16) : 0u;
+    by[j] = vis ? (unsigned)rc[j].y | ((unsigned)rc[j].w << 16) : 0u;
+    if (stage_cap && j * kGaussBlock < per_cta) {  // the warp's 32 records through shared memory, then one span
+      float4* span = reinterpret_cast<float4*>(s_id) + warp * 96;
+      if (vis) gb::pack_record_fused(i, xys, conics, colors3, depths, opacity, comp, span + 3 * lane);
+      const unsigned vmask = __ballot_sync(0xffffffffu, vis);
+      __syncwarp();
+      float4* dst = rec_by_id + 3 * (size_t)(i - lane);
+#pragma unroll
+      for (int f = lane; f < 96; f += 32) {
+        const int r = f / 3, part = f - 3 * r;
+        if (((vmask >> r) & 1u) && (part < 2 || colors3)) dst[f] = span[f];
       }
+      __syncwarp();
+    } else if (vis) {
+      gb::pack_record_fused(i, xys, conics, colors3, depths, opacity, comp, rec_by_id + 3 * (size_t)i);
+    }
   }
-  if (!smem_tiles) return;
+  if (!smem_tiles) {
+#pragma unroll
+    for (int j = 0; j < kScatItems; ++j) {
+      const int i = base + j * kGaussBlock + threadIdx.x;
+      const int x0 = bx[j] & 0xffffu, x1 = bx[j] >> 16, y0 = by[j] & 0xffffu, y1 = by[j] >> 16;
+      for (int ty = y0; ty < y1; ++ty)
+        for (int tx = x0; tx < x1; ++tx) {
+          const int pos = atomicAdd(&cursor[ty * tbx + tx], 1);
+          if ((long long)pos < cap) {
+            tile_ids[pos] = i;
+            keys[pos] = dk[j];
+          }
+        }
+    }
+    return;
+  }
+#pragma unroll
+  for (int j = 0; j < kScatItems; ++j) {
+    const int x0 = bx[j] & 0xffffu, x1 = bx[j] >> 16, y0 = by[j] & 0xffffu, y1 = by[j] >> 16;
+    for (int ty = y0; ty < y1; ++ty)
+      for (int tx = x0; tx < x1; ++tx) atomicAdd(&s_cnt[ty * tbx + tx], 1);
+  }
   __syncthreads();
+  // the CTA's slots of every tile on the global cursor, claims issued back to back
+#pragma unroll 4
   for (int t = threadIdx.x; t < smem_tiles; t += kGaussBlock) {
     const int cnt = s_cnt[t];
-    s_base[t] = cnt ? atomicAdd(&cursor[t], cnt) : 0;
-    s_cnt[t] = 0;
+    s_off[t] = cnt ? atomicAdd(&cursor[t], cnt) : 0;
+  }
+  // local slots: the CTA's pairs tile by tile (exclusive scan of the counts); global slot = s_off[t] + local slot
+  int n_local = 0;
+  for (int t0 = 0; t0 < smem_tiles; t0 += kGaussBlock) {
+    const int t = t0 + threadIdx.x;
+    const int cnt = (t < smem_tiles) ? s_cnt[t] : 0;
+    int total;
+    const int loc = n_local + block_exclusive_scan(cnt, s_warp, total);
+    if (t < smem_tiles) {
+      s_off[t] -= loc;
+      s_cnt[t] = loc;  // from here: the next free local slot of the tile
+    }
+    n_local += total;
   }
   __syncthreads();
+  const bool staged = n_local <= stage_cap;  // uniform over the CTA
 #pragma unroll
   for (int j = 0; j < kScatItems; ++j) {
     const int i = base + j * kGaussBlock + threadIdx.x;
@@ -243,9 +329,28 @@ __global__ void __launch_bounds__(kGaussBlock, 1) tile_scatter_kernel(
     for (int ty = y0; ty < y1; ++ty)
       for (int tx = x0; tx < x1; ++tx) {
         const int t = ty * tbx + tx;
-        const int pos = s_base[t] + atomicAdd(&s_cnt[t], 1);
-        if ((long long)pos < cap) tile_ids[pos] = i;
+        const int e = atomicAdd(&s_cnt[t], 1);
+        if (staged) {
+          s_id[e] = i;
+          s_key[e] = dk[j];
+          s_tile[e] = (unsigned short)t;
+        } else {
+          const int pos = s_off[t] + e;
+          if ((long long)pos < cap) {
+            tile_ids[pos] = i;
+            keys[pos] = dk[j];
+          }
+        }
       }
+  }
+  if (!staged) return;
+  __syncthreads();
+  for (int e = threadIdx.x; e < n_local; e += kGaussBlock) {
+    const int pos = s_off[s_tile[e]] + e;
+    if ((long long)pos < cap) {
+      tile_ids[pos] = s_id[e];
+      keys[pos] = s_key[e];
+    }
   }
 }
 
@@ -359,8 +464,10 @@ __device__ __forceinline__ void minmax_to_smem(unsigned kmin, unsigned kmax, uns
 
 __device__ __forceinline__ int bits_of(unsigned span) { return span ? 32 - __clz((int)span) : 0; }
 
-// bucket: the tile's ids in arbitrary order (tile_scatter_kernel); out: the same ids sorted by (depth key, id).  Both
-// are [cap] arrays indexed by tile_bins; the chunked path for buckets longer than kSortCap uses both as scratch.
+// bucket: the tile's ids in arbitrary order and out: their depth keys at the same slots (tile_scatter_kernel); out
+// receives the same ids sorted by (depth key, id).  Both are [cap] arrays indexed by tile_bins.  The shared-memory path
+// reads every key and id of the tile before it writes out; the chunked path for buckets longer than kSortCap uses both
+// arrays as scratch, and so takes its keys from depth_keys[id].
 __global__ void __launch_bounds__(kSortThreads, 2) tile_sort_kernel(const int* __restrict__ order,
                                                                     const int2* __restrict__ tile_bins,
                                                                     const unsigned* __restrict__ depth_keys,
@@ -382,13 +489,15 @@ __global__ void __launch_bounds__(kSortThreads, 2) tile_sort_kernel(const int* _
     int id[kSortItems];
     unsigned dk[kSortItems];
 #pragma unroll
-    for (int j = 0; j < kSortItems; ++j) id[j] = holds(j, ipt, n) ? bucket[range.x + entry_of(j, ipt)] : -1;
+    for (int j = 0; j < kSortItems; ++j) {
+      const bool h = holds(j, ipt, n);
+      id[j] = h ? bucket[range.x + entry_of(j, ipt)] : -1;
+      dk[j] = h ? (unsigned)out[range.x + entry_of(j, ipt)] : 0u;
+    }
     unsigned kmin = 0xffffffffu, kmax = 0u, imin = 0xffffffffu, imax = 0u;
 #pragma unroll
     for (int j = 0; j < kSortItems; ++j) {
-      dk[j] = 0u;
       if (id[j] < 0) continue;
-      dk[j] = depth_keys[id[j]];
       kmin = min(kmin, dk[j]); kmax = max(kmax, dk[j]);
       imin = min(imin, (unsigned)id[j]); imax = max(imax, (unsigned)id[j]);
     }
@@ -543,6 +652,16 @@ inline Layout make_layout(int G, int T, int64_t cap) {
   return l;
 }
 
+// SMs of the current device, queried once per device
+int num_sms() {
+  static int s_sms[64] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+  if (dev < 0 || dev >= 64) return 0;
+  if (!s_sms[dev] && cudaDeviceGetAttribute(&s_sms[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 0;
+  return s_sms[dev];
+}
+
 // opt in to a dynamic shared-memory window above 48 KB, once per device and kernel
 template <typename K>
 int opt_in_smem(K kernel, size_t bytes, bool* done) {
@@ -642,13 +761,18 @@ static int bin_tiles_impl(int G, const float* xys, const float* depths, const in
   int* ids_sorted = ranked ? ext_ids : gids_sorted;
   const int items = count_items(G);
   const int smem_tiles = (T <= kMaxSmemTiles) ? T : 0;
+  const int stage_cap = scatter_stage_cap(smem_tiles);
+  const size_t scat_smem = scatter_smem_bytes(smem_tiles);
   static bool s_opt_c2[64] = {}, s_opt_c4[64] = {}, s_opt_scat[64] = {}, s_opt_sort[64] = {};
-  if ((size_t)smem_tiles * 8 > 40 * 1024) {
-    constexpr size_t kCountSmem = (size_t)kMaxSmemTiles * 4, kScatSmem = (size_t)kMaxSmemTiles * 8;
-    int e = (items == 2) ? opt_in_smem(tile_count_kernel<2>, kCountSmem, s_opt_c2)
-                         : opt_in_smem(tile_count_kernel<4>, kCountSmem, s_opt_c4);
+  if ((size_t)smem_tiles * 4 > 40 * 1024) {
+    constexpr size_t kCountSmem = (size_t)kMaxSmemTiles * 4;
+    const int e = (items == 2) ? opt_in_smem(tile_count_kernel<2>, kCountSmem, s_opt_c2)
+                               : opt_in_smem(tile_count_kernel<4>, kCountSmem, s_opt_c4);
     if (e) return e;
-    e = opt_in_smem(tile_scatter_kernel, kScatSmem, s_opt_scat);
+  }
+  {  // the largest window any grid asks for: the tile arrays of kMaxSmemTiles, or those of kStageMaxTiles + staging
+    const size_t a = scatter_smem_bytes(kMaxSmemTiles), b = scatter_smem_bytes(kStageMaxTiles);
+    const int e = opt_in_smem(tile_scatter_kernel, a > b ? a : b, s_opt_scat);
     if (e) return e;
   }
   const size_t sort_smem = (size_t)kSortCap * 8;
@@ -673,9 +797,10 @@ static int bin_tiles_impl(int G, const float* xys, const float* depths, const in
                            : gb_tile_order(T, tile_bins, tile_order, stream);
   if (e) return e;
   const bool late = colors_ready != nullptr;  // the colour quarter of the by-id records is filled after the tile sort
-  tile_scatter_kernel<<<gb::cdiv(G, kGaussBlock * kScatItems), kGaussBlock, (size_t)smem_tiles * 8, s>>>(
+  const int per_cta = scatter_per_cta(G, num_sms());
+  tile_scatter_kernel<<<gb::cdiv(G, per_cta), kGaussBlock, scat_smem, s>>>(
       G, rects, (const float2*)xys, conics, late ? nullptr : colors3, depths, opacity, compensation, tbx, (long long)cap,
-      smem_tiles, cursor, bucket, rec_by_id);
+      per_cta, smem_tiles, stage_cap, cursor, bucket, (unsigned*)ids_sorted, rec_by_id);
   tile_sort_kernel<<<T, kSortThreads, sort_smem, s>>>(tile_order, (const int2*)tile_bins, (const unsigned*)depths, bucket,
                                                       ids_sorted);
   gb::count_launches(2);
