@@ -13,12 +13,11 @@
 // into shared memory and runs the horizontal pass; kernel 2 runs the vertical pass on a column tile with its halos
 // and composites (render, alpha, mirror ball) in the same pass.  The environment map (<= a few hundred KB) stays in
 // L1/L2, so both kernels are bound by the blur arithmetic and one read + one write of the image per pass.
-#include "common.cuh"
+#include "envmap_common.cuh"
 
 namespace {
 
 constexpr float kPiGrid = 3.1415926f;                     // rotate_envmap_mat's texel grid uses this literal
-constexpr float kInvPi = (float)(1.0 / 3.14159265358979323846);  // (1 / np.pi) as torch rounds it for fp32
 constexpr float kA = -0.75f;                              // torch's bicubic convolution constant
 constexpr float kFocalScale = 0.2f;                       // envmap_to_image(focal_scale=0.2)
 constexpr int kBall = 200;                                // envmap_to_mirrorball(200, 200, ...)
@@ -27,13 +26,7 @@ constexpr int kR = 50, kTaps = 2 * kR + 1;                // 101-tap blur, paddi
 constexpr int kRowTile = 256;                             // kernel 1: outputs per block (one row segment)
 constexpr int kColTile = 32, kRowsPer = 8, kColRows = 8 * kRowsPer;  // kernel 2: 32 columns x 64 rows per block
 
-// u = atan2(x, z) / pi, v = 2 acos(y) / pi - 1 (ca_code/utils/envmap.py:213-215, 242-244, 158-160).  No clamp before
-// acos: |y| > 1 gives NaN, as torch.acos does.
-__device__ __forceinline__ float2 dir2uv(float x, float y, float z) {
-  const float u = __fmul_rn(kInvPi, atan2f(x, z));
-  const float v = __fmul_rn(kInvPi, acosf(y));
-  return make_float2(u, __fsub_rn(__fmul_rn(2.f, v), 1.f));
-}
+using gb::dir2uv;
 
 // grid_sample's border padding applied to one tap (clip_coordinates + the in-bounds cast).  fmaxf maps a NaN
 // coordinate to 0, so the fetch stays in bounds; the NaN weights still make the sample NaN, as in torch.

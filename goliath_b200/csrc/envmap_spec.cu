@@ -14,7 +14,7 @@
 // Backward: gradients to ref_dirs (through the rotation, dir2uv and the bilinear weights; zero where the border
 // clip is active, as grid_sample does) and to spec_vis.  The mip level is computed under no_grad upstream, so sigma
 // receives none; the environment map itself is a constant of the relighting loop (no gradient is produced for it).
-#include "common.cuh"
+#include "envmap_common.cuh"
 
 namespace {
 
@@ -32,40 +32,9 @@ struct EnvArgs {
   float *g_ref_dirs, *g_spec_vis;
 };
 
-struct Bilin {
-  int x0, y0, x1, y1;
-  float fx, fy;     // fractional weights of (x1, y1)
-  float mx, my;     // gradient multipliers of the border clip (0 where clipped)
-};
-
-// grid_sample coordinate handling: align_corners=False unnormalisation, padding_mode="border" clip
-__device__ __forceinline__ Bilin locate(float u, float v, int W, int H) {
-  Bilin b;
-  float ix = ((u + 1.f) * (float)W - 1.f) * 0.5f;
-  float iy = ((v + 1.f) * (float)H - 1.f) * 0.5f;
-  b.mx = (ix < 0.f || ix > (float)(W - 1)) ? 0.f : 1.f;
-  b.my = (iy < 0.f || iy > (float)(H - 1)) ? 0.f : 1.f;
-  ix = fminf(fmaxf(ix, 0.f), (float)(W - 1));
-  iy = fminf(fmaxf(iy, 0.f), (float)(H - 1));
-  const float x0f = floorf(ix), y0f = floorf(iy);
-  b.x0 = (int)x0f; b.y0 = (int)y0f;
-  b.x1 = b.x0 + 1; b.y1 = b.y0 + 1;
-  b.fx = ix - x0f; b.fy = iy - y0f;
-  return b;
-}
-
-// one channel plane: value and its derivatives w.r.t. the (unclipped-scale) pixel coordinates
-__device__ __forceinline__ float fetch(const float* __restrict__ p, const Bilin& b, int W, int H, float& ddx, float& ddy) {
-  const bool x1in = b.x1 < W, y1in = b.y1 < H;  // out-of-range neighbours contribute zero (their weight is zero too)
-  const float v00 = p[(size_t)b.y0 * W + b.x0];
-  const float v01 = x1in ? p[(size_t)b.y0 * W + b.x1] : 0.f;
-  const float v10 = y1in ? p[(size_t)b.y1 * W + b.x0] : 0.f;
-  const float v11 = (x1in && y1in) ? p[(size_t)b.y1 * W + b.x1] : 0.f;
-  const float wx0 = 1.f - b.fx, wy0 = 1.f - b.fy;
-  ddx = (v01 - v00) * wy0 + (v11 - v10) * b.fy;
-  ddy = (v10 - v00) * wx0 + (v11 - v01) * b.fx;
-  return v00 * wx0 * wy0 + v01 * b.fx * wy0 + v10 * wx0 * b.fy + v11 * b.fx * b.fy;
-}
+using gb::Bilin;
+using gb::fetch;
+using gb::locate;
 
 __device__ __forceinline__ float lerp_torch(float s, float e, float w) {  // th.lerp's two-sided formula
   return (w < 0.5f) ? s + w * (e - s) : e - (e - s) * (1.f - w);

@@ -7,8 +7,12 @@
   200x200 mirror ball in the bottom-right corner, two kernels (bicubic lookup + horizontal blur pass; vertical blur
   pass + composite).  K and Rt are read on the device, so the call never synchronises with the host.  The gradient
   goes to `render` only: alpha is detached in the reference (rgca.py:137,144) and envbg, K, Rt are data.
+* `prefilter_envmap_sg(sigma, v, env_tex, num_samples, xi=None, seed=None)` (envmap.py:305-323): the Monte-Carlo
+  spherical-Gaussian prefilter of the environment-spin mip chain, one warp per texel (csrc/envmap_prefilter.cu).
 
 Same signatures and results as the reference; no CPU fallback."""
+import ctypes
+
 import torch
 from torch.autograd import Function
 
@@ -87,3 +91,66 @@ def compose_envmap(render: torch.Tensor, alpha: torch.Tensor, envbg: torch.Tenso
     its [:3,:3] rotates the rays).  Returns render + (1 - alpha) * clamp(blurred environment, 0, 1) with the mirror
     ball blended into the bottom-right 200x200 corner.  Differentiable w.r.t. render only."""
     return _ComposeEnvmap.apply(render, alpha, envbg, K, Rt)
+
+
+def _prefilter_levels(levels, num_samples, seed=None):
+    """levels: list of (sigma, v [B,3,H,W], env_tex [B,3,He,We], xi [S,B,2,H,W] or None), all run in one launch.
+    Returns the prefiltered [B,3,H,W] of each level."""
+    q = len(levels)
+    if not 1 <= q <= 8:
+        raise RuntimeError("prefilter_envmap_sg: 1..8 levels per launch")
+    if int(num_samples) < 1:
+        raise RuntimeError("prefilter_envmap_sg: num_samples must be >= 1")
+    with_xi = levels[0][3] is not None
+    B = levels[0][1].shape[0]
+    hw, sig, vs, envs, xis, outs = [], [], [], [], [], []
+    for sigma, v, env_tex, xi in levels:
+        if not float(sigma) > 0.0:
+            raise RuntimeError("prefilter_envmap_sg: sigma must be > 0 (got %r)" % (sigma,))
+        if v.dim() != 4 or v.shape[0] != B or v.shape[1] != 3:
+            raise RuntimeError("prefilter_envmap_sg: v must be [B,3,H,W]")
+        if env_tex.dim() != 4 or env_tex.shape[:2] != v.shape[:2]:
+            raise RuntimeError("prefilter_envmap_sg: env_tex must be [B,3,He,We] with the B of v")
+        H, W = v.shape[2:]
+        if (xi is not None) != with_xi:
+            raise RuntimeError("prefilter_envmap_sg: xi must be given for every level or for none")
+        if xi is not None:
+            if xi.dim() == 4 and B == 1:
+                xi = xi[:, None]
+            if tuple(xi.shape) != (int(num_samples), B, 2, H, W):
+                raise RuntimeError("prefilter_envmap_sg: xi must be [num_samples,2,H,W] (B = 1) or [num_samples,B,2,H,W]"
+                                   " = %s (got %s)" % ((int(num_samples), B, 2, H, W), tuple(xi.shape)))
+        ts = [t.contiguous() for t in (v, env_tex) + ((xi,) if xi is not None else ())]
+        for t, n in zip(ts, ("v", "env_tex", "xi")):
+            _lib.check_input(t, n)
+        if len({t.device for t in ts + vs[:1]}) != 1:
+            raise RuntimeError("prefilter_envmap_sg: all tensors must be on one device")
+        vs.append(ts[0])
+        envs.append(ts[1])
+        xis.append(ts[2] if xi is not None else None)
+        outs.append(torch.empty_like(ts[0]))
+        hw += [H, W, env_tex.shape[2], env_tex.shape[3]]
+        sig.append(float(sigma))
+    if seed is None:
+        seed = int(torch.randint(0, 2 ** 63 - 1, (1,), dtype=torch.int64).item())  # torch's default CPU generator
+    ptrs = lambda ts: (ctypes.c_void_p * q)(*[t.data_ptr() for t in ts])
+    dev = vs[0].device
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().gb_envmap_prefilter_sg(
+            B, q, (ctypes.c_int32 * (4 * q))(*[int(x) for x in hw]), (ctypes.c_float * q)(*sig), ptrs(vs), ptrs(envs),
+            ptrs(xis) if with_xi else None, int(num_samples), int(seed) & (2 ** 64 - 1), ptrs(outs),
+            _lib.stream_ptr(dev)), "envmap_prefilter_sg")
+    return outs
+
+
+def prefilter_envmap_sg(sigma: float, v: torch.Tensor, env_tex: torch.Tensor, num_samples: int = 1,
+                        xi: torch.Tensor = None, seed: int = None) -> torch.Tensor:
+    """prefilterEnvmapSG: v [B,3,H,W] (unit directions), env_tex [B,3,He,We] -> [B,3,H,W], the mean of `num_samples`
+    bilinear lookups (border padding, align_corners=False) of env_tex along importance_sample_sg's directions around v
+    for a spherical Gaussian of width sigma (radians).
+
+    The draws come from a counter-based Philox stream keyed by `seed`; without one, the seed is drawn from torch's
+    default CPU generator, so torch.manual_seed reproduces a run.  `xi` [num_samples,B,2,H,W] (or [num_samples,2,H,W]
+    with B = 1) replaces the draws with the ones given: the tensors the reference's th.rand_like(v[:, :2]) returns, one
+    per sample, for checking the arithmetic sample for sample.  No gradient."""
+    return _prefilter_levels([(sigma, v, env_tex, xi)], num_samples, seed)[0]

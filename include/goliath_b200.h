@@ -419,6 +419,33 @@ int gb_envmap_compose_fwd(int B, int H, int W, int He, int We, const float* rend
                           float* out, void* stream);
 /* the only gradient of compose_envmap (alpha detached, envbg / K / Rt data): g_render = (1 - m) * g_out [B,3,H,W]. */
 int gb_envmap_compose_bwd(int B, int H, int W, const float* g_out, float* g_render, void* stream);
+/* replaces prefilterEnvmapSG (ca_code/utils/envmap.py:305-323) with importance_sample_sg (:251-281, the pdf not computed)
+ * and sample_uv (:295-302), for q (1..8) levels in one launch: out[l] [B,3,H,W] = mean over num_samples of the bilinear
+ * lookup (border padding, align_corners=False) of env_tex[l] [B,3,He,We] along normalize(t Hx + b Hy + n Hz), n = v[l]
+ * [B,3,H,W], up = (0,0,1) where n_z < 0.999 else (1,0,0), t = normalize(up x n), b = n x t, H = (cos phi sin theta,
+ * sin phi sin theta, cos theta), phi = 2 pi xi0, theta = sqrt(2) sigma erfinv(xi1 erf(pi / (sqrt(2) sigma))).
+ * dir2uv takes acos without a clamp, as the reference does: where rounding pushes the normalised y past +-1 the v
+ * coordinate is NaN, which grid_sample's border clip (and this kernel) turns into 0, so that sample reads the first
+ * texel row.  xi: NULL, or q device pointers to [num_samples,B,2,H,W] (the reference's th.rand_like(v[:, :2]) draws);
+ * with NULL, xi comes from a counter-based Philox4x32-10 stream keyed by seed at counter (sample pair, texel, item, l),
+ * and the per-texel sum runs in a fixed order, so a seed gives bit-identical output.
+ * level_hw: q x (H, W, He, We) and sigma [q] (> 0) in host memory; v / env_tex / xi / out: host arrays of device
+ * pointers. */
+int gb_envmap_prefilter_sg(int B, int q, const int32_t* level_hw, const float* sigma, const float* const* v,
+                           const float* const* env_tex, const float* const* xi, int num_samples, unsigned long long seed,
+                           float* const* out, void* stream);
+/* replaces the per-item loop of EnvSpinDecorator.forward (ca_code/utils/light_decorator.py:111-149), batched over B:
+ *   lightrot [B,3,3] = rvec_to_R((0, angles[b], 0)) (ca_code/utils/envmap.py:20-50, fp32; angle 0 gives I);
+ *   envbg [B,3,He,We] = rotate_envmap_mat(image, lightrot[b]) (gb_envmap_rotate) / perc90 * 255 / 255;
+ *   the 16x32 antialiased bilinear downsample of the rotated probe (torch's _upsample_bilinear2d_aa weights, horizontal
+ *   pass first into hpass [B,3,He,32] scratch);
+ *   envmap [B,3,16,32] = env_scale * down / sum(down * sin((row + 0.5) pi / 16)) over channels and texels;
+ *   light_intensity [B,512,3] = envmap[b].view(3, -1).t(); norm_scale [B] = env_scale / that sum.
+ * angles [B] in host memory (2 pi index / cycle); image [3,He,We] the static probe; perc90 > 0 its 90th percentile;
+ * He >= 16, 32 <= We <= 3072.  No host sync, no copy. */
+int gb_envmap_spin_table(int B, int He, int We, const float* angles, const float* image, float perc90, float env_scale,
+                         float* lightrot, float* envbg, float* hpass, float* envmap, float* light_intensity,
+                         float* norm_scale, void* stream);
 
 /* replaces the per-view post-processing of rgca.AutoEncoder.render (ca_code/models/rgca.py:136-151, with
  * render_gsplat.py:79-108): colour HWC -> CHW, alpha = 1 - final_T (detached), depth / alpha.clamp(0.05, 1).
