@@ -85,7 +85,12 @@ SIGNATURES = {
     "gb_mvp_slab_to_prims_bwd": (_i, [_i] * 6 + [_vp] * 3 + [_f, _f, _i] + [_vp] * 3 + [_vp]),
     "gb_mvp_prim_transform_fwd": (_i, [_i, _i] + [_vp] * 3 + [_f, _i] + [_vp] * 3 + [_vp]),
     "gb_mvp_prim_transform_bwd": (_i, [_i, _i] + [_vp] * 3 + [_f, _i] + [_vp] * 4 + [_vp]),
-    "gb_sg_shade_compose_fwd": (_i, [_vp] * 10 + [_i] * 4 + [_vp]),
+    "gb_mvp_prim_frames_fwd": (_i, [_i] * 4 + [_vp] * 10 + [_vp]),
+    "gb_lbs_max_joints": (_i, []),
+    "gb_lbs_skeleton_fwd": (_i, [_i] * 4 + [_vp, _vp, _i] + [_vp] * 7 + [_i] + [_vp] * 3 + [_vp]),
+    "gb_lbs_skin_fwd": (_i, [_i] * 4 + [_vp] * 7 + [_vp]),
+    "gb_lbs_skin_bwd": (_i, [_i] * 4 + [_vp] * 6 + [_vp]),
+    "gb_sg_shade_compose_fwd":(_i, [_vp] * 10 + [_i] * 4 + [_vp]),
     "gb_sg_shade_compose_bwd": (_i, [_vp] * 16 + [_i] * 4 + [_vp]),
     "gb_render_finish_fwd": (_i, [_i, _i] + [_vp] * 5 + [_vp]),
     "gb_render_finish_bwd": (_i, [_i, _i] + [_vp] * 4 + [_vp]),

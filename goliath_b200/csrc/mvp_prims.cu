@@ -156,6 +156,75 @@ __global__ void __launch_bounds__(128) prim_transform_kernel(int B, int K, const
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// primitive base frames on the posed mesh: make_postex + compute_tbn (geom.py:355-397,515-520) and the texel gather of
+// compute_view_cos (geom.py:349-352) through values_to_uv (geom.py:308-324)
+struct F3 {
+  float x, y, z;
+};
+__device__ __forceinline__ F3 ld3(const float* p) { return {p[0], p[1], p[2]}; }
+__device__ __forceinline__ F3 sub3(F3 a, F3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
+__device__ __forceinline__ F3 cross3(F3 a, F3 b) { return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x}; }
+// F.normalize(x, dim=-1): x / max(|x|, 1e-12); an infinite component gives NaN, as in torch
+__device__ __forceinline__ F3 normalize3(F3 a) {
+  const float d = fmaxf(sqrtf(a.x * a.x + a.y * a.y + a.z * a.z), 1e-12f);
+  return {a.x / d, a.y / d, a.z / d};
+}
+// torch's indexing of a negative index: -1 is the last row
+__device__ __forceinline__ int wrap(int i, int n) { return i < 0 ? i + n : i; }
+
+__global__ void __launch_bounds__(128) prim_frames_kernel(int B, int V, int NT, int T, const float* __restrict__ v,
+                                                          const int* __restrict__ vidx, const int* __restrict__ vtidx,
+                                                          const float* __restrict__ bary, const float* __restrict__ vt,
+                                                          const float* __restrict__ vn, const float* __restrict__ campos,
+                                                          float* posbase, float* rotbase, float* view_cos) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * T) return;
+  const int b = i / T, t = i % T;
+  const int r0 = vidx[3 * t], r1 = vidx[3 * t + 1], r2 = vidx[3 * t + 2];
+  const int i0 = wrap(r0, V), i1 = wrap(r1, V), i2 = wrap(r2, V);
+  const float* vb = v + (size_t)b * V * 3;
+  const F3 p0 = ld3(vb + 3 * i0), p1 = ld3(vb + 3 * i1), p2 = ld3(vb + 3 * i2);
+  const float w0 = bary[3 * t], w1 = bary[3 * t + 1], w2 = bary[3 * t + 2];
+  if (posbase) {
+    float* o = posbase + (size_t)i * 3;
+    o[0] = w0 * p0.x + w1 * p1.x + w2 * p2.x;
+    o[1] = w0 * p0.y + w1 * p1.y + w2 * p2.y;
+    o[2] = w0 * p0.z + w1 * p1.z + w2 * p2.z;
+  }
+  if (rotbase) {
+    const int j0 = wrap(vtidx[3 * t], NT), j1 = wrap(vtidx[3 * t + 1], NT), j2 = wrap(vtidx[3 * t + 2], NT);
+    const float u01 = vt[2 * j1] - vt[2 * j0], w01 = vt[2 * j1 + 1] - vt[2 * j0 + 1];
+    const float u02 = vt[2 * j2] - vt[2 * j0], w02 = vt[2 * j2 + 1] - vt[2 * j0 + 1];
+    const F3 e01 = sub3(p1, p0), e02 = sub3(p2, p0);
+    // no guard on the determinant: a degenerate UV triangle gives inf here and NaN below, as in the reference
+    const float f = 1.f / (u01 * w02 - w01 * u02);
+    const F3 tg = normalize3({f * (e01.x * w02 - e02.x * w01), f * (e01.y * w02 - e02.y * w01), f * (e01.z * w02 - e02.z * w01)});
+    const F3 nm = normalize3(cross3(e01, e02));
+    const F3 bt = normalize3(cross3(tg, nm));
+    float* R = rotbase + (size_t)i * 9;  // columns T, B, N
+    R[0] = tg.x; R[1] = bt.x; R[2] = nm.x;
+    R[3] = tg.y; R[4] = bt.y; R[5] = nm.y;
+    R[6] = tg.z; R[7] = bt.z; R[8] = nm.z;
+  }
+  if (view_cos) {
+    float c = 0.f;
+    if (r0 != -1 && r1 != -1 && r2 != -1) {
+      const float* nb = vn + (size_t)b * V * 3;
+      const F3 cp = ld3(campos + 3 * b);
+      const int id[3] = {i0, i1, i2};
+      const F3 p[3] = {p0, p1, p2};
+      const float w[3] = {w0, w1, w2};
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const F3 n = normalize3(ld3(nb + 3 * id[k])), d = normalize3(sub3(p[k], cp));
+        c += (n.x * d.x + n.y * d.y + n.z * d.z) * w[k];
+      }
+    }
+    view_cos[i] = c;
+  }
+}
+
 }  // namespace
 
 // hand_mvp.py:172-185 (+ the output activations :434,:472 and the valid-primitive gather render_raymarcher.py:44-46).
@@ -201,6 +270,20 @@ GB_API int gb_mvp_prim_transform_fwd(int B, int K, const float* dec, const float
   if (B <= 0 || K <= 0) return 0;
   prim_transform_kernel<false><<<gb::cdiv(B * K, 128), 128, 0, (cudaStream_t)stream>>>(
       B, K, dec, posbase, rotbase, prim_scale, zero_delta, primpos, primrot, primscale, nullptr);
+  gb::count_launches(1);
+  GB_CHECK_LAUNCH();
+  return 0;
+}
+
+// hand_mvp.py:386-408 (make_postex, compute_tbn) and :230-236 (compute_view_cos + values_to_uv) on the posed mesh.
+GB_API int gb_mvp_prim_frames_fwd(int B, int V, int NT, int T, const float* verts, const int32_t* vidx,
+                                  const int32_t* vtidx, const float* bary, const float* vt, const float* vn,
+                                  const float* campos, float* posbase, float* rotbase, float* view_cos, void* stream) {
+  if (B <= 0 || T <= 0) return 0;
+  if (V <= 0 || (rotbase && (NT <= 0 || !vtidx || !vt)) || (view_cos && (!vn || !campos)))
+    return (int)cudaErrorInvalidValue;
+  prim_frames_kernel<<<gb::cdiv(B * T, 128), 128, 0, (cudaStream_t)stream>>>(B, V, NT, T, verts, vidx, vtidx, bary, vt,
+                                                                             vn, campos, posbase, rotbase, view_cos);
   gb::count_launches(1);
   GB_CHECK_LAUNCH();
   return 0;

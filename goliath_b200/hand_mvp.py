@@ -7,15 +7,18 @@ checkpoints load, plus the two glue stages between those decoders and the raymar
   * `slabs_to_primrgba` — output activations + cat/permute/reshape + valid-primitive gather
                           (hand_mvp.py:434,472,172-185; render_raymarcher.py:44-46), csrc/mvp_prims.cu
 
-The mesh front end that produces `primposbase` / `primrotbase` / `view_cos_uv` (LBS, TBN, UV gather) is outside the
-path (SURVEY.md §8f-4) and is taken as input."""
+The mesh front end (DESIGN.md row R8') runs on kernels too: `GeomDecoder` poses the mesh with `lbs.LBSModule` and
+builds each primitive's base frame with `prim_base_frames`; `view_cos_uv` gives the RGB decoder's view conditioning
+(hand_mvp.py:230-236), both on csrc/mvp_prims.cu."""
 from typing import Optional, Tuple
 
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 from torch.autograd import Function
 
 from . import _lib
+from .geom import vert_normals
 from .nn import ConvBlock, ConvTranspose2dWNUB, Conv2dWNUB, FusedLeakyReLU, glorot, tile2d
 
 
@@ -197,3 +200,133 @@ def slabs_to_primrgba(primrgb, primalpha, primsize: Tuple[int, int, int] = (16, 
         slot, n_out = hit[0], hit[1]
     mul, add, relu = (25.0, 100.0, 1) if raw else (1.0, 0.0, 0)
     return _SlabsToPrims.apply(primrgb, primalpha, tuple(primsize), slot, n_out, mul, add, relu)
+
+
+# ------------------------------------------------------------------------------------------------ mesh front end
+def init_primitives(slab_size, n_prims, geo_fn):
+    """hand_mvp.py:50-68: sample the UV index images at the centre texel of each primitive's slab cell.  `geo_fn` is
+    the reference's GeometryModule or any holder with `vi`, `vti`, `vt` and `render_index_images(size, impaint=True)`.
+    As in the reference, the face image is the un-inpainted one, and torch's indexing of `vi[face]` makes a -1 face
+    index select the last face.  Returns (prim_vidx_img, prim_vtidx_img, prim_bary_img), each [S, S, 3]."""
+    stride = slab_size // int(n_prims ** 0.5)
+    _, face_index, bary_index = geo_fn.render_index_images(slab_size, impaint=True)
+    bary_index = torch.as_tensor(bary_index, device=geo_fn.vt.device)
+    cell = (slice(stride // 2, None, stride), slice(stride // 2, None, stride))
+    face = face_index[cell]
+    return geo_fn.vi[face], geo_fn.vti[face], bary_index[cell]
+
+
+def _frame_inputs(geom, name):
+    if torch.is_grad_enabled() and geom.requires_grad:
+        raise RuntimeError("%s: the base frames carry no gradient (the reference builds them under no_grad)" % name)
+    geom = geom.contiguous()
+    _lib.check_input(geom, "geom")
+    return geom
+
+
+def _i32(t):
+    return t.to(torch.int32).contiguous()
+
+
+def prim_base_frames(geom_lbs, vt, prim_vidx_img, prim_vtidx_img, prim_bary_img):
+    """make_postex + compute_tbn (geom.py:355-397,515-520) as GeomDecoder.forward uses them (hand_mvp.py:393-408), in
+    one kernel: geom_lbs [B,V,3] posed vertices -> (primposbase [B,K,3], primrotbase [B,K,3,3] with columns T, B, N),
+    K = S*S texels of the [S,S,3] index / barycentric images."""
+    geom = _frame_inputs(geom_lbs, "prim_base_frames")
+    vidx, vtidx = _i32(prim_vidx_img), _i32(prim_vtidx_img)
+    bary, vt = prim_bary_img.to(torch.float32).contiguous(), vt.to(torch.float32).contiguous()
+    for t, n in ((vidx, "prim_vidx_img"), (vtidx, "prim_vtidx_img")):
+        _lib.check_input(t, n, torch.int32)
+    _lib.check_input(bary, "prim_bary_img")
+    _lib.check_input(vt, "vt")
+    B, V = geom.shape[0], geom.shape[1]
+    T = vidx.numel() // 3
+    if vidx.shape[-1] != 3 or vtidx.shape != vidx.shape or bary.shape != vidx.shape or vt.shape[-1] != 2:
+        raise RuntimeError("index / barycentric images must be [S,S,3] and vt [NT,2]")
+    posbase = torch.empty(B, T, 3, device=geom.device)
+    rotbase = torch.empty(B, T, 3, 3, device=geom.device)
+    with torch.cuda.device(geom.device):
+        _lib.check(_lib.lib().gb_mvp_prim_frames_fwd(
+            B, V, vt.shape[0], T, _lib.ptr(geom), _lib.ptr(vidx), _lib.ptr(vtidx), _lib.ptr(bary), _lib.ptr(vt), None,
+            None, _lib.ptr(posbase), _lib.ptr(rotbase), None, _lib.stream_ptr(geom.device)), "mvp_prim_frames_fwd")
+    return posbase, rotbase
+
+
+def view_cos_uv(geom_lbs, vi, campos, prim_vidx_img, prim_bary_img):
+    """compute_view_cos + values_to_uv (geom.py:308-352) as hand_mvp.AutoEncoder.forward uses them (:230-236):
+    geom_lbs [B,V,3], vi [F,3] faces, campos [B,3] -> [B,1,S,S], zero at texels with a -1 index.  The vertex normals
+    come from `geom.vert_normals` (gb_vert_normals_fwd)."""
+    geom = _frame_inputs(geom_lbs, "view_cos_uv")
+    vidx = _i32(prim_vidx_img)
+    bary = prim_bary_img.to(torch.float32).contiguous()
+    campos = campos.to(torch.float32).contiguous()
+    _lib.check_input(vidx, "prim_vidx_img", torch.int32)
+    _lib.check_input(bary, "prim_bary_img")
+    _lib.check_input(campos, "campos")
+    B, V = geom.shape[0], geom.shape[1]
+    S0, S1 = vidx.shape[0], vidx.shape[1]
+    if vidx.shape != (S0, S1, 3) or bary.shape != vidx.shape or campos.shape != (B, 3):
+        raise RuntimeError("prim_vidx_img / prim_bary_img must be [S,S,3] and campos [B,3]")
+    vn = vert_normals(geom, vi)
+    out = torch.empty(B, 1, S0, S1, device=geom.device)
+    with torch.cuda.device(geom.device):
+        _lib.check(_lib.lib().gb_mvp_prim_frames_fwd(
+            B, V, 0, S0 * S1, _lib.ptr(geom), _lib.ptr(vidx), None, _lib.ptr(bary), None, _lib.ptr(vn),
+            _lib.ptr(campos), None, None, _lib.ptr(out), _lib.stream_ptr(geom.device)), "mvp_prim_frames_fwd")
+    return out
+
+
+class GeomDecoder(nn.Module):
+    """hand_mvp.py:351-444 with the reference's constructor, submodules (`lbs_fn`, `transdecoder`, `alphadecoder`)
+    and non-persistent `prim_*_img` buffers.  The front end (pose, base frames) runs under no_grad on the kernels;
+    `prim_transforms` composes it with TransDecoder's deltas, and the alpha slab's ReLU runs inside the last deconv."""
+
+    def __init__(self, inch, primsize_z, uv_size, n_prims, lbs_fn, geo_fn, primposstart, prim_scale=512):
+        super().__init__()
+        self.lbs_fn = lbs_fn
+        self.geo_fn = geo_fn
+        self.primposstart = primposstart
+        self.uv_size = uv_size
+        self.n_prims = n_prims
+        self.primsize_z = primsize_z
+        self.prim_scale = prim_scale
+        prim_vidx_img, prim_vtidx_img, prim_bary_img = init_primitives(uv_size, n_prims, geo_fn)
+        self.register_buffer("prim_vidx_img", prim_vidx_img, persistent=False)
+        self.register_buffer("prim_vtidx_img", prim_vtidx_img, persistent=False)
+        self.register_buffer("prim_bary_img", prim_bary_img, persistent=False)
+        self.transdecoder = TransDecoder(inch)
+        self.alphadecoder = DeconvContentDecoder(primsize_z, inch, 1)
+
+    def forward(self, pose, joint, iteration=-1):
+        B = pose.shape[0]
+        with torch.no_grad():
+            geom_lbs = self.lbs_fn.pose(torch.zeros_like(self.lbs_fn.lbs_template_verts), pose)
+            primposbase, primrotbase = prim_base_frames(geom_lbs, self.geo_fn.vt, self.prim_vidx_img,
+                                                        self.prim_vtidx_img, self.prim_bary_img)
+        zero_delta = bool(self.training and iteration < self.primposstart)
+        primpos, primrot, primscale = prim_transforms(self.transdecoder.raw(joint), primposbase, primrotbase,
+                                                      self.prim_scale, zero_delta)
+        tex = self.alphadecoder.texbranch
+        alpha = tex[-1](tex[:-1](joint), slope=0.0)  # LeakyReLU(0) = the reference's F.relu (:434)
+        alpha = alpha.view(B, self.primsize_z, 1, self.uv_size, self.uv_size)
+        return {"primalpha": alpha, "primpos": primpos, "primscale": primscale, "primrot": primrot,
+                "geom_lbs": geom_lbs}
+
+
+class RGBSlabDecoder(nn.Module):
+    """hand_mvp.py:447-474: the bilinear AO resize and the concatenation in torch, the deconv tower on the kernels,
+    then relu(25 x + 100)."""
+
+    def __init__(self, inch, primsize_z, uv_size, geo_fn):
+        super().__init__()
+        self.geo_fn = geo_fn
+        self.primsize_z = primsize_z
+        self.uv_size = uv_size
+        self.texdecoder = DeconvContentDecoder(primsize_z, inch, 3)
+
+    def forward(self, view_cos_uv, joint, ambient_occlusion):
+        B = joint.shape[0]
+        ao_ds = F.interpolate(ambient_occlusion, (64, 64), mode="bilinear")
+        rgb = self.texdecoder(torch.cat((joint, view_cos_uv, ao_ds), 1))
+        rgb = rgb.view(B, self.primsize_z, 3, self.uv_size, self.uv_size)
+        return F.relu(25.0 * rgb + 100.0)

@@ -553,6 +553,55 @@ int gb_mvp_prim_transform_bwd(int B, int K, const float* dec, const float* posba
                               float prim_scale, int zero_delta, const float* g_primpos, const float* g_primrot,
                               const float* g_primscale, float* g_dec, void* stream);
 
+/* replaces make_postex (ca_code/utils/geom.py:515-520) and compute_tbn (geom.py:355-397) as hand_mvp.GeomDecoder.forward
+ * calls them (hand_mvp.py:393-408), and compute_view_cos (geom.py:349-352) + values_to_uv (geom.py:308-324) as
+ * hand_mvp.AutoEncoder.forward calls them (hand_mvp.py:230-236).  One thread per (item, texel) on the posed vertices
+ * verts [B,V,3]; vidx / vtidx / bary [T,3] (int32, int32, fp32), vt [NT,2].  Outputs (each may be NULL):
+ *   posbase [B,T,3] = b0 v[i0] + b1 v[i1] + b2 v[i2];
+ *   rotbase [B,T,3,3] with the columns T, B, N of compute_tbn: f = 1/det of the UV edges, taken without a guard (a
+ *   degenerate UV triangle gives NaN, as in the reference), F.normalize with eps 1e-12, bitangent = normalize(T x N);
+ *   view_cos [B,T] = sum_k b_k <normalize(vn[i_k]), normalize(v[i_k] - campos[b])>, 0 where any index is -1;
+ *   vn [B,V,3] comes from gb_vert_normals_fwd, campos [B,3].
+ * A negative index in the frame outputs selects from the end, as torch's indexing does.  vtidx / vt are needed for
+ * rotbase, vn / campos for view_cos. */
+int gb_mvp_prim_frames_fwd(int B, int V, int NT, int T, const float* verts, const int32_t* vidx, const int32_t* vtidx,
+                           const float* bary, const float* vt, const float* vn, const float* campos, float* posbase,
+                           float* rotbase, float* view_cos, void* stream);
+
+/* ---------------------------------------------------------------- linear blend skinning (row R8') */
+
+/* Largest joint count gb_lbs_skeleton_fwd accepts: one CTA keeps every joint's state (8 floats) in shared memory. */
+int gb_lbs_max_joints(void);
+
+/* replaces ParameterTransform.forward + solve_skeleton_state + states_to_matrix (ca_code/utils/lbs.py:39-46,340-429)
+ * as LinearBlendSkinning.forward runs them (lbs.py:308-337), with the quaternion operations of
+ * ca_code/utils/quaternion.py:178-320.  One CTA per item b:
+ *   jp = transform [7J,P+S] . cat(motion[b] [P], scale[b] [S]) + transform_offsets [7J];
+ *   per joint: lt = jp[0:3] + joint_offset, lr = joint_rotation (x) fromXYZ(jp[3:6]), ls = 2^jp[6];
+ *   per joint with parent p, level by level: q = q_p (x) lr, t = rot(q_p, lt s_p) + t_p, s = s_p ls.
+ * scale rows are scale_stride floats apart (0 = one row for every item).  parents [J] int32 (-1 = root, parent < j);
+ * level_order [J] lists the joints level by level (roots first), level_start [n_levels+1] the level boundaries.
+ * bind_state [J,8] -> mats [B,J,3,4] (states_to_matrix); states [B,J,8] (t, q, s) is written when not NULL.
+ * J > gb_lbs_max_joints() returns cudaErrorInvalidValue. */
+int gb_lbs_skeleton_fwd(int B, int J, int P, int S, const float* motion, const float* scale, int scale_stride,
+                        const float* transform, const float* transform_offsets, const float* joint_offset,
+                        const float* joint_rotation, const int32_t* parents, const int32_t* level_order,
+                        const int32_t* level_start, int n_levels, const float* bind_state, float* mats, float* states,
+                        void* stream);
+
+/* replaces LinearBlendSkinning.skinning (lbs.py:226-254) and the template add / global scaling of LBSModule.pose
+ * (lbs.py:725-731): out [B,V,3] = gs * sum_{k<8} w_k mats[b, idx_k] [verts + templ; 1], slots summed in order.
+ * verts [vb,V,3] with vb = 1 or B; templ [V,3] or NULL (zero); skin_indices [V,8] int32, skin_weights [V,8];
+ * global_scaling [3] or NULL (one). */
+int gb_lbs_skin_fwd(int B, int V, int J, int vb, const float* mats, const float* verts, const float* templ,
+                    const int32_t* skin_indices, const float* skin_weights, const float* global_scaling, float* out,
+                    void* stream);
+/* gradient w.r.t. verts only: g_verts [vb,V,3] (written) = sum_k w_k mats[b, idx_k][:, :3]^T (gs * g_out[b]); a batch-1
+ * input sums b = 0..B-1 in order inside one thread, so the result is deterministic. */
+int gb_lbs_skin_bwd(int B, int V, int J, int vb, const float* mats, const int32_t* skin_indices,
+                    const float* skin_weights, const float* global_scaling, const float* g_out, float* g_verts,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif
