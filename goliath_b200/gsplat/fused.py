@@ -5,11 +5,13 @@ Equivalent, output for output, to the reference's call sequence in ca_code/utils
 arithmetic — but without the tensors that sequence materialises between the calls (`opacity * compensation[:, None]`,
 `depths[:, None].expand(-1, 3)`, the second binning) and without their autograd glue in the backward."""
 import os
+from typing import NamedTuple
 
 import torch
 from torch.autograd import Function
 
 from .. import _lib
+from .project import _project_bwd, _project_fwd
 from .utils import _tile_bounds, _workspace, bin_and_sort_gaussians, compute_cumulative_intersects, key_bits
 
 # sync-free mode: per-device overflow flag (int32 on the device, set by the bin-edges kernel when the intersection
@@ -53,6 +55,74 @@ def check_overflow(device=None) -> bool:
     return hit
 
 
+class _BlendPlan(NamedTuple):
+    sched: int  # 1: the tile order is an SM-affine schedule (gb_tile_schedule) the blend kernels draw their tiles from
+    order_len: int  # int32 entries of the tile order
+    fwd: object  # gb_rasterize_{sched,packed}_fwd
+    bwd: object  # gb_rasterize_{sched,packed}_bwd
+    ranked: bool  # the two-node path blends id-staged records (gb_rasterize_ranked_*, see RANKED)
+
+
+def _blend_plan(T, schedule=True):
+    """How the blend mode (gb_get_blend_mode) maps to a tile order and to the rasterize entry points of a render over T
+    tiles.  Blend modes 2 and 4 take an SM-affine schedule; `schedule=False` (the exact path, whose tile order is always
+    gb_tile_order) keeps the launch-order tiles in every mode."""
+    L = _lib.lib()
+    mode = L.gb_get_blend_mode()
+    sched = 1 if schedule and mode in (2, 4) else 0
+    return _BlendPlan(sched, L.gb_tile_schedule_ints(T) if sched else T,
+                      L.gb_rasterize_sched_fwd if sched else L.gb_rasterize_packed_fwd,
+                      L.gb_rasterize_sched_bwd if sched else L.gb_rasterize_packed_bwd,
+                      RANKED and not sched and mode == 3)
+
+
+def _bin_tiles(xys, depths, radii, conics, colors, opacity, comp, H, W, cap, plan, outs, ranked=False, n_out=None,
+               colors_ready=None):
+    """Bucket binning (csrc/splat_bin_tiles.cu) on the current stream, into the caller's `outs`: (gids [cap], records
+    [cap,12]) for gb_bin_tiles_pack_ev, or with `ranked` (ranks [cap], records [G,12], gids [G]) for
+    gb_bin_tiles_ranked.  `n_out` (device int32) receives the intersection count, `colors_ready` is the raw handle of
+    an event to wait for before the colours are read; either may be None.  Returns (bins [T,2], order)."""
+    G = xys.size(0)
+    dev = xys.device
+    L = _lib.lib()
+    tb = _tile_bounds(H, W, 16)
+    T = tb[0] * tb[1]
+    bins = torch.empty(T, 2, device=dev, dtype=torch.int32)
+    order = torch.empty(plan.order_len, device=dev, dtype=torch.int32)
+    ws = _workspace(dev, L.gb_bin_tiles_workspace_bytes(G, T, cap))
+    with torch.cuda.device(dev):
+        _lib.check((L.gb_bin_tiles_ranked if ranked else L.gb_bin_tiles_pack_ev)(
+            G, _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(colors), _lib.ptr(opacity),
+            _lib.ptr(comp), H, W, 16, cap, _lib.ptr(bins), _lib.ptr(order), plan.sched, *map(_lib.ptr, outs),
+            _lib.ptr(n_out), _lib.ptr(_overflow_flag(dev)), _lib.ptr(ws), colors_ready, _lib.stream_ptr(dev)),
+            "bin_tiles_ranked" if ranked else "bin_tiles_pack")
+    return bins, order
+
+
+def _blend_grads(H, W, v_out4, v_alpha, opacity, comp, blend, v_colors=None):
+    """Gradients through a blend.  `blend(st, v_out4, v_alpha, v_xy, v_conic, v_col4, v_opeff)` issues the rasterize
+    backward(s) on stream `st`; they accumulate atomically into the last four arrays, which are zeroed here with one
+    fill.  gb_splat_grad_unpack then turns v_col4 / v_opeff into the gradients of the colours (into `v_colors` when
+    given), opacity, compensation and depth.  Returns (v_xy, v_conic, v_colors, v_opacity, v_comp, v_depth)."""
+    G = comp.size(0)
+    dev = comp.device
+    f32 = dict(device=dev, dtype=torch.float32)
+    v_out4 = torch.zeros(H, W, 4, **f32) if v_out4 is None else v_out4.contiguous()
+    v_alpha = None if v_alpha is None else v_alpha.contiguous()  # NULL: no gradient through alpha (no zero fill)
+    acc = torch.zeros(G * 10, **f32)  # the four atomically-accumulated gradient arrays, one fill
+    v_xy, v_conic = acc[:2 * G].view(G, 2), acc[2 * G:5 * G].view(G, 3)
+    v_col4, v_opeff = acc[5 * G:9 * G].view(G, 4), acc[9 * G:]
+    v_colors = torch.empty(G, 3, **f32) if v_colors is None else v_colors
+    v_opacity, v_comp, v_depth = torch.empty(G, 1, **f32), torch.empty(G, **f32), torch.empty(G, **f32)
+    with torch.cuda.device(dev):
+        st = _lib.stream_ptr(dev)
+        blend(st, v_out4, v_alpha, v_xy, v_conic, v_col4, v_opeff)
+        _lib.check(_lib.lib().gb_splat_grad_unpack(G, _lib.ptr(v_col4), _lib.ptr(v_opeff), _lib.ptr(opacity),
+                                                   _lib.ptr(comp), _lib.ptr(v_colors), _lib.ptr(v_opacity),
+                                                   _lib.ptr(v_comp), _lib.ptr(v_depth), st), "splat_grad_unpack")
+    return v_xy, v_conic, v_colors, v_opacity, v_comp, v_depth
+
+
 class _RenderFused(Function):
     @staticmethod
     def forward(ctx, means3d, scales, quats, opacity, colors, viewmat, background, glob_scale, fx, fy, cx, cy, img_height,
@@ -68,42 +138,30 @@ class _RenderFused(Function):
         L = _lib.lib()
         f32 = dict(device=dev, dtype=torch.float32)
         i32 = dict(device=dev, dtype=torch.int32)
-        cov3d, xys, depths = torch.empty(G, 6, **f32), torch.empty(G, 2, **f32), torch.empty(G, **f32)
-        radii, conics, comp = torch.empty(G, **i32), torch.empty(G, 3, **f32), torch.empty(G, **f32)
-        num_tiles_hit = torch.empty(G, **i32)
         H, W, BW = int(img_height), int(img_width), 16
         out4 = torch.empty(H, W, 4, **f32)
         final_Ts = torch.empty(H, W, **f32)
         final_idx = torch.empty(H, W, **i32)
         bg4 = torch.cat([background, background[:1]])
+        xys, depths, radii, conics, comp, num_tiles_hit, cov3d = _project_fwd(
+            means3d, scales, quats, viewmat, glob_scale, fx, fy, cx, cy, H, W, BW, clip_thresh)
+        tb = _tile_bounds(H, W, BW)
+        T = tb[0] * tb[1]
+        plan = _blend_plan(T, schedule=capacity is not None)
         with torch.cuda.device(dev):
             st = _lib.stream_ptr(dev)
-            _lib.check(L.gb_project_gaussians_fwd(
-                G, _lib.ptr(means3d), _lib.ptr(scales), float(glob_scale), _lib.ptr(quats), _lib.ptr(viewmat), float(fx),
-                float(fy), float(cx), float(cy), H, W, BW, float(clip_thresh), _lib.ptr(cov3d), _lib.ptr(xys),
-                _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp), _lib.ptr(num_tiles_hit), st),
-                "project_gaussians_forward")
-            tb = _tile_bounds(H, W, BW)
-            T = tb[0] * tb[1]
-            # blend modes 2 and 4: the tile order is an SM-affine schedule and the blend kernels draw their tiles from it
-            sched = 1 if (capacity is not None and L.gb_get_blend_mode() in (2, 4)) else 0
             if capacity is not None:
                 # ---- sync-free path: the count never visits the host; buffers hold `capacity` intersections
-                cap = int(capacity)
+                cap = num_intersects = int(capacity)  # "some": the backward walks the bins, not the count
                 gids = torch.empty(cap, **i32)
-                order = torch.empty(L.gb_tile_schedule_ints(T) if sched else T, **i32)
                 records = torch.empty(cap, 12, **f32)
                 if BINNING == "buckets" and L.gb_bin_tiles_supported(G):
                     # per-tile buckets, each sorted by (depth, id) in shared memory (csrc/splat_bin_tiles.cu): same
                     # bins, ids and records as the key sort below, without sorting the intersection keys globally
-                    bins = torch.empty(T, 2, **i32)
-                    ws = _workspace(dev, L.gb_bin_tiles_workspace_bytes(G, T, cap))
-                    _lib.check(L.gb_bin_tiles_pack(G, _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii),
-                                                   _lib.ptr(conics), _lib.ptr(colors), _lib.ptr(opacity),
-                                                   _lib.ptr(comp), H, W, BW, cap, _lib.ptr(bins), _lib.ptr(order),
-                                                   sched, _lib.ptr(gids), _lib.ptr(records), None,
-                                                   _lib.ptr(_overflow_flag(dev)), _lib.ptr(ws), st), "bin_tiles_pack")
+                    bins, order = _bin_tiles(xys, depths, radii, conics, colors, opacity, comp, H, W, cap, plan,
+                                             (gids, records))
                 else:
+                    order = torch.empty(plan.order_len, **i32)
                     cum = torch.empty_like(num_tiles_hit)
                     ws = _workspace(dev, max(L.gb_cumsum_workspace_bytes(G), L.gb_sort_workspace_bytes(cap)))
                     _lib.check(L.gb_cumsum_i32(G, _lib.ptr(num_tiles_hit), _lib.ptr(cum), _lib.ptr(ws), st), "cumsum")
@@ -120,40 +178,35 @@ class _RenderFused(Function):
                                                        st), "sort_dn")
                     _lib.check(L.gb_get_tile_bin_edges_dn(cap, n_dev, _lib.ptr(isect_s), _lib.ptr(bins),
                                                           _lib.ptr(_overflow_flag(dev)), st), "edges_dn")
-                    _lib.check((L.gb_tile_schedule if sched else L.gb_tile_order)(T, _lib.ptr(bins), _lib.ptr(order), st),
-                               "tile_order")
+                    _lib.check((L.gb_tile_schedule if plan.sched else L.gb_tile_order)(
+                        T, _lib.ptr(bins), _lib.ptr(order), st), "tile_order")
                     _lib.check(L.gb_pack_records_fused_dn(cap, n_dev, _lib.ptr(gids), _lib.ptr(xys), _lib.ptr(conics),
                                                           _lib.ptr(colors), _lib.ptr(depths), _lib.ptr(opacity),
                                                           _lib.ptr(comp), _lib.ptr(records), st),
                                "pack_records_fused_dn")
-                _lib.check((L.gb_rasterize_sched_fwd if sched else L.gb_rasterize_packed_fwd)(
-                    H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(out4),
-                    _lib.ptr(final_Ts), _lib.ptr(final_idx), st), "rasterize_packed_forward")
-                num_intersects = cap  # "some": the backward walks the bins, not the count
             else:
                 num_intersects, cum = compute_cumulative_intersects(num_tiles_hit)
-            if capacity is not None:
-                pass
-            elif num_intersects < 1:
-                # reference behaviour with nothing to draw (gsplat 0.1.11 rasterize.py): background, final_Ts = 0
-                out4.copy_(bg4.expand(H, W, 4))
-                final_Ts.zero_()
-                final_idx.zero_()
-                gids = bins = order = records = torch.empty(0, **i32)
-            else:
-                _, _, _, gids, bins = bin_and_sort_gaussians(G, num_intersects, xys, depths, radii, cum, tb, BW)
-                order = torch.empty(T, **i32)
-                records = torch.empty(num_intersects, 12, **f32)
-                _lib.check(L.gb_tile_order(T, _lib.ptr(bins), _lib.ptr(order), st), "tile_order")
-                _lib.check(L.gb_pack_records_fused(num_intersects, _lib.ptr(gids), _lib.ptr(xys), _lib.ptr(conics),
-                                                   _lib.ptr(colors), _lib.ptr(depths), _lib.ptr(opacity), _lib.ptr(comp),
-                                                   _lib.ptr(records), st), "pack_records_fused")
-                _lib.check(L.gb_rasterize_packed_fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records),
-                                                     _lib.ptr(bg4), _lib.ptr(out4), _lib.ptr(final_Ts),
-                                                     _lib.ptr(final_idx), st), "rasterize_packed_forward")
+                if num_intersects < 1:
+                    # reference behaviour with nothing to draw (gsplat 0.1.11 rasterize.py): background, final_Ts = 0
+                    out4.copy_(bg4.expand(H, W, 4))
+                    final_Ts.zero_()
+                    final_idx.zero_()
+                    gids = bins = order = records = torch.empty(0, **i32)
+                else:
+                    _, _, _, gids, bins = bin_and_sort_gaussians(G, num_intersects, xys, depths, radii, cum, tb, BW)
+                    order = torch.empty(T, **i32)
+                    records = torch.empty(num_intersects, 12, **f32)
+                    _lib.check(L.gb_tile_order(T, _lib.ptr(bins), _lib.ptr(order), st), "tile_order")
+                    _lib.check(L.gb_pack_records_fused(num_intersects, _lib.ptr(gids), _lib.ptr(xys), _lib.ptr(conics),
+                                                       _lib.ptr(colors), _lib.ptr(depths), _lib.ptr(opacity),
+                                                       _lib.ptr(comp), _lib.ptr(records), st), "pack_records_fused")
+            if capacity is not None or num_intersects >= 1:
+                _lib.check(plan.fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4),
+                                    _lib.ptr(out4), _lib.ptr(final_Ts), _lib.ptr(final_idx), st),
+                           "rasterize_packed_forward")
         ctx.save_for_backward(means3d, scales, quats, opacity, viewmat, bg4, cov3d, radii, conics, comp, gids, bins, order,
                               records, final_Ts, final_idx)
-        ctx.meta = (G, H, W, num_intersects, float(glob_scale), float(fx), float(fy), sched)
+        ctx.meta = (H, W, num_intersects, float(glob_scale), float(fx), float(fy), plan)
         ctx.mark_non_differentiable(radii)
         ctx.set_materialize_grads(False)
         return out4, 1 - final_Ts, radii
@@ -162,34 +215,17 @@ class _RenderFused(Function):
     def backward(ctx, v_out4, v_alpha, _v_radii):
         (means3d, scales, quats, opacity, viewmat, bg4, cov3d, radii, conics, comp, gids, bins, order, records, final_Ts,
          final_idx) = ctx.saved_tensors
-        G, H, W, num_intersects, glob_scale, fx, fy, sched = ctx.meta
-        dev = means3d.device
-        L = _lib.lib()
-        f32 = dict(device=dev, dtype=torch.float32)
-        v_out4 = torch.zeros(H, W, 4, **f32) if v_out4 is None else v_out4.contiguous()
-        v_alpha = None if v_alpha is None else v_alpha.contiguous()  # NULL: no gradient through alpha (no zero fill)
-        acc = torch.zeros(G * 10, **f32)  # the four atomically-accumulated gradient arrays, one fill
-        v_xy, v_conic = acc[:2 * G].view(G, 2), acc[2 * G:5 * G].view(G, 3)
-        v_col4, v_opeff = acc[5 * G:9 * G].view(G, 4), acc[9 * G:]
-        v_colors, v_opacity = torch.empty(G, 3, **f32), torch.empty(G, 1, **f32)
-        v_comp, v_depth = torch.empty(G, **f32), torch.empty(G, **f32)
-        g_cov2d, g_cov3d = torch.empty(G, 3, **f32), torch.empty(G, 6, **f32)
-        g_mean, g_scale, g_quat = torch.empty(G, 3, **f32), torch.empty(G, 3, **f32), torch.empty(G, 4, **f32)
-        with torch.cuda.device(dev):
-            st = _lib.stream_ptr(dev)
+        H, W, num_intersects, glob_scale, fx, fy, plan = ctx.meta
+
+        def blend(st, *grads):
             if num_intersects >= 1:
-                _lib.check((L.gb_rasterize_sched_bwd if sched else L.gb_rasterize_packed_bwd)(
-                    H, W, 4, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4),
-                    _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(v_out4), _lib.ptr(v_alpha), _lib.ptr(v_xy),
-                    _lib.ptr(v_conic), _lib.ptr(v_col4), _lib.ptr(v_opeff), st), "rasterize_packed_backward")
-            _lib.check(L.gb_splat_grad_unpack(G, _lib.ptr(v_col4), _lib.ptr(v_opeff), _lib.ptr(opacity), _lib.ptr(comp),
-                                              _lib.ptr(v_colors), _lib.ptr(v_opacity), _lib.ptr(v_comp), _lib.ptr(v_depth),
-                                              st), "splat_grad_unpack")
-            _lib.check(L.gb_project_gaussians_bwd(
-                G, _lib.ptr(means3d), _lib.ptr(scales), glob_scale, _lib.ptr(quats), _lib.ptr(viewmat), fx, fy,
-                _lib.ptr(cov3d), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp), _lib.ptr(v_xy), _lib.ptr(v_depth),
-                _lib.ptr(v_conic), _lib.ptr(v_comp), _lib.ptr(g_cov2d), _lib.ptr(g_cov3d), _lib.ptr(g_mean),
-                _lib.ptr(g_scale), _lib.ptr(g_quat), st), "project_gaussians_backward")
+                _lib.check(plan.bwd(H, W, 4, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records),
+                                    _lib.ptr(bg4), _lib.ptr(final_Ts), _lib.ptr(final_idx), *map(_lib.ptr, grads), st),
+                           "rasterize_packed_backward")
+
+        v_xy, v_conic, v_colors, v_opacity, v_comp, v_depth = _blend_grads(H, W, v_out4, v_alpha, opacity, comp, blend)
+        g_mean, g_scale, g_quat = _project_bwd(means3d, scales, quats, viewmat, cov3d, radii, conics, comp, glob_scale,
+                                               fx, fy, v_xy, v_depth, v_conic, v_comp)
         return (g_mean, g_scale, g_quat, v_opacity, v_colors) + (None,) * 11
 
 
@@ -202,46 +238,17 @@ class _ProjectGeom(Function):
         for t, n in zip(ins, ("means3d", "scales", "quats", "viewmat")):
             _lib.check_input(t, n)
         means3d, scales, quats, viewmat = ins
-        G = means3d.size(0)
-        dev = means3d.device
-        f32 = dict(device=dev, dtype=torch.float32)
-        i32 = dict(device=dev, dtype=torch.int32)
-        cov3d, xys, depths = torch.empty(G, 6, **f32), torch.empty(G, 2, **f32), torch.empty(G, **f32)
-        radii, conics, comp = torch.empty(G, **i32), torch.empty(G, 3, **f32), torch.empty(G, **f32)
-        num_tiles_hit = torch.empty(G, **i32)
-        H, W = int(img_height), int(img_width)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_project_gaussians_fwd(
-                G, _lib.ptr(means3d), _lib.ptr(scales), float(glob_scale), _lib.ptr(quats), _lib.ptr(viewmat), float(fx),
-                float(fy), float(cx), float(cy), H, W, 16, float(clip_thresh), _lib.ptr(cov3d), _lib.ptr(xys),
-                _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp), _lib.ptr(num_tiles_hit),
-                _lib.stream_ptr(dev)), "project_gaussians_forward")
+        xys, depths, radii, conics, comp, _, cov3d = _project_fwd(means3d, scales, quats, viewmat, glob_scale, fx, fy,
+                                                                  cx, cy, img_height, img_width, 16, clip_thresh)
         ctx.save_for_backward(means3d, scales, quats, viewmat, cov3d, radii, conics, comp)
-        ctx.meta = (G, float(glob_scale), float(fx), float(fy))
+        ctx.meta = (float(glob_scale), float(fx), float(fy))
         ctx.mark_non_differentiable(radii)
         ctx.set_materialize_grads(False)
         return xys, depths, conics, comp, radii
 
     @staticmethod
     def backward(ctx, v_xy, v_depth, v_conic, v_comp, _v_radii):
-        means3d, scales, quats, viewmat, cov3d, radii, conics, comp = ctx.saved_tensors
-        G, glob_scale, fx, fy = ctx.meta
-        dev = means3d.device
-        f32 = dict(device=dev, dtype=torch.float32)
-
-        def z(t, shape):
-            return torch.zeros(shape, **f32) if t is None else t.contiguous()
-
-        v_xy, v_depth, v_conic, v_comp = z(v_xy, (G, 2)), z(v_depth, (G,)), z(v_conic, (G, 3)), z(v_comp, (G,))
-        g_cov2d, g_cov3d = torch.empty(G, 3, **f32), torch.empty(G, 6, **f32)
-        g_mean, g_scale, g_quat = torch.empty(G, 3, **f32), torch.empty(G, 3, **f32), torch.empty(G, 4, **f32)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_project_gaussians_bwd(
-                G, _lib.ptr(means3d), _lib.ptr(scales), glob_scale, _lib.ptr(quats), _lib.ptr(viewmat), fx, fy,
-                _lib.ptr(cov3d), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp), _lib.ptr(v_xy), _lib.ptr(v_depth),
-                _lib.ptr(v_conic), _lib.ptr(v_comp), _lib.ptr(g_cov2d), _lib.ptr(g_cov3d), _lib.ptr(g_mean),
-                _lib.ptr(g_scale), _lib.ptr(g_quat), _lib.stream_ptr(dev)), "project_gaussians_backward")
-        return (g_mean, g_scale, g_quat) + (None,) * 9
+        return _project_bwd(*ctx.saved_tensors, *ctx.meta, v_xy, v_depth, v_conic, v_comp) + (None,) * 9
 
 
 class _BinBlend(Function):
@@ -260,85 +267,64 @@ class _BinBlend(Function):
         L = _lib.lib()
         f32 = dict(device=dev, dtype=torch.float32)
         i32 = dict(device=dev, dtype=torch.int32)
-        H, W, BW = int(img_height), int(img_width), 16
+        H, W = int(img_height), int(img_width)
         out4 = torch.empty(H, W, 4, **f32)
         final_Ts = torch.empty(H, W, **f32)
         final_idx = torch.empty(H, W, **i32)
         bg4 = torch.cat([background, background[:1]])
-        tb = _tile_bounds(H, W, BW)
-        T = tb[0] * tb[1]
+        tb = _tile_bounds(H, W, 16)
         cap = int(capacity)
+        plan = _blend_plan(tb[0] * tb[1])
+        ev = None
+        if colors_event is not None:
+            ev = colors_event.cuda_event
+            colors.record_stream(torch.cuda.current_stream(dev))
+        # id-staged records (the default with the mom blend and launch-order tiles): the blend gathers each stage
+        # from the by-id table, the sorted 48-byte records are never materialised (csrc/splat_blend_mom.cu, RANKED)
+        if plan.ranked:
+            gids = torch.empty(G, **i32)            # identity (the C ABI's rank_to_gid)
+            ranks = torch.empty(cap, **i32)         # per tile: Gaussian ids in blend order
+            records = torch.empty(G, 12, **f32)     # one record per Gaussian, by id
+            outs = (ranks, records, gids)
+        else:
+            gids = torch.empty(cap, **i32)
+            ranks = gids  # unused
+            records = torch.empty(cap, 12, **f32)
+            outs = (gids, records)
+        bins, order = _bin_tiles(xys, depths, radii, conics, colors, opacity, comp, H, W, cap, plan, outs,
+                                 ranked=plan.ranked, colors_ready=ev)
         with torch.cuda.device(dev):
             st = _lib.stream_ptr(dev)
-            sched = 1 if L.gb_get_blend_mode() in (2, 4) else 0
-            order = torch.empty(L.gb_tile_schedule_ints(T) if sched else T, **i32)
-            bins = torch.empty(T, 2, **i32)
-            ws = _workspace(dev, L.gb_bin_tiles_workspace_bytes(G, T, cap))
-            ev = None
-            if colors_event is not None:
-                ev = colors_event.cuda_event
-                colors.record_stream(torch.cuda.current_stream(dev))
-            # id-staged records (the default with the mom blend and launch-order tiles): the blend gathers each stage
-            # from the by-id table, the sorted 48-byte records are never materialised (csrc/splat_blend_mom.cu, RANKED)
-            ranked = RANKED and not sched and L.gb_get_blend_mode() == 3
-            if ranked:
-                gids = torch.empty(G, **i32)            # identity (the C ABI's rank_to_gid)
-                ranks = torch.empty(cap, **i32)         # per tile: Gaussian ids in blend order
-                records = torch.empty(G, 12, **f32)     # one record per Gaussian, by id
-                _lib.check(L.gb_bin_tiles_ranked(G, _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics),
-                                                 _lib.ptr(colors), _lib.ptr(opacity), _lib.ptr(comp), H, W, BW, cap,
-                                                 _lib.ptr(bins), _lib.ptr(order), sched, _lib.ptr(ranks),
-                                                 _lib.ptr(records), _lib.ptr(gids), None, _lib.ptr(_overflow_flag(dev)),
-                                                 _lib.ptr(ws), ev, st), "bin_tiles_ranked")
+            if plan.ranked:
                 _lib.check(L.gb_rasterize_ranked_fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(ranks),
                                                      _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(out4), _lib.ptr(final_Ts),
                                                      _lib.ptr(final_idx), st), "rasterize_ranked_forward")
             else:
-                gids = torch.empty(cap, **i32)
-                ranks = gids  # unused
-                records = torch.empty(cap, 12, **f32)
-                _lib.check(L.gb_bin_tiles_pack_ev(G, _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics),
-                                                  _lib.ptr(colors), _lib.ptr(opacity), _lib.ptr(comp), H, W, BW, cap,
-                                                  _lib.ptr(bins), _lib.ptr(order), sched, _lib.ptr(gids),
-                                                  _lib.ptr(records), None, _lib.ptr(_overflow_flag(dev)), _lib.ptr(ws), ev,
-                                                  st), "bin_tiles_pack_ev")
-                _lib.check((L.gb_rasterize_sched_fwd if sched else L.gb_rasterize_packed_fwd)(
-                    H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(out4),
-                    _lib.ptr(final_Ts), _lib.ptr(final_idx), st), "rasterize_packed_forward")
+                _lib.check(plan.fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4),
+                                    _lib.ptr(out4), _lib.ptr(final_Ts), _lib.ptr(final_idx), st),
+                           "rasterize_packed_forward")
         ctx.save_for_backward(opacity, comp, bg4, gids, bins, order, records, final_Ts, final_idx, ranks)
-        ctx.meta = (G, H, W, sched, ranked)
+        ctx.meta = (H, W, plan)
         ctx.set_materialize_grads(False)
         return out4, 1 - final_Ts
 
     @staticmethod
     def backward(ctx, v_out4, v_alpha):
         opacity, comp, bg4, gids, bins, order, records, final_Ts, final_idx, ranks = ctx.saved_tensors
-        G, H, W, sched, ranked = ctx.meta
-        dev = opacity.device
-        L = _lib.lib()
-        f32 = dict(device=dev, dtype=torch.float32)
-        v_out4 = torch.zeros(H, W, 4, **f32) if v_out4 is None else v_out4.contiguous()
-        v_alpha = None if v_alpha is None else v_alpha.contiguous()
-        acc = torch.zeros(G * 10, **f32)  # the four atomically-accumulated gradient arrays, one fill
-        v_xy, v_conic = acc[:2 * G].view(G, 2), acc[2 * G:5 * G].view(G, 3)
-        v_col4, v_opeff = acc[5 * G:9 * G].view(G, 4), acc[9 * G:]
-        v_colors, v_opacity = torch.empty(G, 3, **f32), torch.empty(G, 1, **f32)
-        v_comp, v_depth = torch.empty(G, **f32), torch.empty(G, **f32)
-        with torch.cuda.device(dev):
-            st = _lib.stream_ptr(dev)
-            if ranked:
-                _lib.check(L.gb_rasterize_ranked_bwd(
+        H, W, plan = ctx.meta
+
+        def blend(st, *grads):
+            if plan.ranked:
+                _lib.check(_lib.lib().gb_rasterize_ranked_bwd(
                     H, W, 4, _lib.ptr(gids), _lib.ptr(ranks), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records),
-                    _lib.ptr(bg4), _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(v_out4), _lib.ptr(v_alpha),
-                    _lib.ptr(v_xy), _lib.ptr(v_conic), _lib.ptr(v_col4), _lib.ptr(v_opeff), st), "rasterize_ranked_backward")
+                    _lib.ptr(bg4), _lib.ptr(final_Ts), _lib.ptr(final_idx), *map(_lib.ptr, grads), st),
+                    "rasterize_ranked_backward")
             else:
-                _lib.check((L.gb_rasterize_sched_bwd if sched else L.gb_rasterize_packed_bwd)(
-                    H, W, 4, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4),
-                    _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(v_out4), _lib.ptr(v_alpha), _lib.ptr(v_xy),
-                    _lib.ptr(v_conic), _lib.ptr(v_col4), _lib.ptr(v_opeff), st), "rasterize_packed_backward")
-            _lib.check(L.gb_splat_grad_unpack(G, _lib.ptr(v_col4), _lib.ptr(v_opeff), _lib.ptr(opacity), _lib.ptr(comp),
-                                              _lib.ptr(v_colors), _lib.ptr(v_opacity), _lib.ptr(v_comp), _lib.ptr(v_depth),
-                                              st), "splat_grad_unpack")
+                _lib.check(plan.bwd(H, W, 4, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records),
+                                    _lib.ptr(bg4), _lib.ptr(final_Ts), _lib.ptr(final_idx), *map(_lib.ptr, grads), st),
+                           "rasterize_packed_backward")
+
+        v_xy, v_conic, v_colors, v_opacity, v_comp, v_depth = _blend_grads(H, W, v_out4, v_alpha, opacity, comp, blend)
         return (v_xy, v_depth, v_conic, v_comp, None, v_opacity, v_colors) + (None,) * 5
 
 

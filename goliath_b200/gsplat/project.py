@@ -41,35 +41,62 @@ def project_gaussians(
     return outs
 
 
+def _project_fwd(means3d, scales, quats, viewmat, glob_scale, fx, fy, cx, cy, img_height, img_width, block_width,
+                 clip_thresh):
+    """The projection kernel on the current stream.  Returns (xys [G,2], depths [G], radii [G] i32, conics [G,3],
+    compensation [G], num_tiles_hit [G] i32, cov3d [G,6])."""
+    G = means3d.size(0)
+    dev = means3d.device
+    f32 = dict(device=dev, dtype=torch.float32)
+    i32 = dict(device=dev, dtype=torch.int32)
+    cov3d, xys, depths = torch.empty(G, 6, **f32), torch.empty(G, 2, **f32), torch.empty(G, **f32)
+    radii, conics, comp = torch.empty(G, **i32), torch.empty(G, 3, **f32), torch.empty(G, **f32)
+    num_tiles_hit = torch.empty(G, **i32)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().gb_project_gaussians_fwd(
+            G, _lib.ptr(means3d), _lib.ptr(scales), float(glob_scale), _lib.ptr(quats), _lib.ptr(viewmat), float(fx),
+            float(fy), float(cx), float(cy), int(img_height), int(img_width), int(block_width), float(clip_thresh),
+            _lib.ptr(cov3d), _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp),
+            _lib.ptr(num_tiles_hit), _lib.stream_ptr(dev)), "project_gaussians_forward")
+    return xys, depths, radii, conics, comp, num_tiles_hit, cov3d
+
+
+def _project_bwd(means3d, scales, quats, viewmat, cov3d, radii, conics, comp, glob_scale, fx, fy, v_xy, v_depth, v_conic,
+                 v_comp):
+    """The projection backward on the current stream; a missing (None) gradient counts as zero.  Returns (v_means3d,
+    v_scales, v_quats)."""
+    G = means3d.size(0)
+    dev = means3d.device
+    f32 = dict(device=dev, dtype=torch.float32)
+
+    def z(t, shape):
+        return torch.zeros(shape, **f32) if t is None else t.contiguous()
+
+    v_xy, v_depth, v_conic, v_comp = z(v_xy, (G, 2)), z(v_depth, (G,)), z(v_conic, (G, 3)), z(v_comp, (G,))
+    g_cov2d, g_cov3d = torch.empty(G, 3, **f32), torch.empty(G, 6, **f32)
+    g_mean, g_scale, g_quat = torch.empty(G, 3, **f32), torch.empty(G, 3, **f32), torch.empty(G, 4, **f32)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().gb_project_gaussians_bwd(
+            G, _lib.ptr(means3d), _lib.ptr(scales), float(glob_scale), _lib.ptr(quats), _lib.ptr(viewmat), float(fx),
+            float(fy), _lib.ptr(cov3d), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp), _lib.ptr(v_xy),
+            _lib.ptr(v_depth), _lib.ptr(v_conic), _lib.ptr(v_comp), _lib.ptr(g_cov2d), _lib.ptr(g_cov3d),
+            _lib.ptr(g_mean), _lib.ptr(g_scale), _lib.ptr(g_quat), _lib.stream_ptr(dev)), "project_gaussians_backward")
+    return g_mean, g_scale, g_quat
+
+
 class _ProjectGaussians(Function):
     @staticmethod
     def forward(ctx, means3d, scales, glob_scale, quats, viewmat, fx, fy, cx, cy, img_height, img_width,
                 block_width, clip_thresh):
         for t, n in ((means3d, "means3d"), (scales, "scales"), (quats, "quats"), (viewmat, "viewmat")):
             _lib.check_input(t, n)
-        G = means3d.size(-2)
         if means3d.ndimension() != 2 or means3d.size(1) != 3:
             raise ValueError("means3d must have dimensions (N, 3)")
         if viewmat.numel() < 12:
             raise ValueError("viewmat must hold at least a 3x4 matrix")
-        dev = means3d.device
-        f32 = dict(device=dev, dtype=torch.float32)
-        cov3d = torch.empty(G, 6, **f32)
-        xys = torch.empty(G, 2, **f32)
-        depths = torch.empty(G, **f32)
-        radii = torch.empty(G, device=dev, dtype=torch.int32)
-        conics = torch.empty(G, 3, **f32)
-        compensation = torch.empty(G, **f32)
-        num_tiles_hit = torch.empty(G, device=dev, dtype=torch.int32)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_project_gaussians_fwd(
-                G, _lib.ptr(means3d), _lib.ptr(scales), float(glob_scale), _lib.ptr(quats), _lib.ptr(viewmat),
-                float(fx), float(fy), float(cx), float(cy), int(img_height), int(img_width), int(block_width),
-                float(clip_thresh), _lib.ptr(cov3d), _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii),
-                _lib.ptr(conics), _lib.ptr(compensation), _lib.ptr(num_tiles_hit), _lib.stream_ptr(dev)),
-                "project_gaussians_forward")
-        ctx.img_height, ctx.img_width, ctx.G = img_height, img_width, G
-        ctx.glob_scale, ctx.fx, ctx.fy, ctx.cx, ctx.cy = glob_scale, fx, fy, cx, cy
+        xys, depths, radii, conics, compensation, num_tiles_hit, cov3d = _project_fwd(
+            means3d, scales, quats, viewmat, glob_scale, fx, fy, cx, cy, img_height, img_width, block_width, clip_thresh)
+        ctx.glob_scale, ctx.fx, ctx.fy = glob_scale, fx, fy
         ctx.save_for_backward(means3d, scales, quats, viewmat, cov3d, radii, conics, compensation)
         ctx.mark_non_differentiable(radii, num_tiles_hit)
         ctx.set_materialize_grads(False)
@@ -78,27 +105,9 @@ class _ProjectGaussians(Function):
     @staticmethod
     def backward(ctx, v_xys, v_depths, v_radii, v_conics, v_compensation, v_num_tiles_hit, v_cov3d):
         means3d, scales, quats, viewmat, cov3d, radii, conics, compensation = ctx.saved_tensors
-        G = ctx.G
-        dev = means3d.device
-        f32 = dict(device=dev, dtype=torch.float32)
-
-        def _z(t, shape):
-            return torch.zeros(shape, **f32) if t is None else t.contiguous()
-
-        v_xys, v_depths = _z(v_xys, (G, 2)), _z(v_depths, (G,))
-        v_conics, v_compensation = _z(v_conics, (G, 3)), _z(v_compensation, (G,))
-        g_cov2d = torch.empty(G, 3, **f32)
-        g_cov3d = torch.empty(G, 6, **f32)
-        g_mean3d = torch.empty(G, 3, **f32)
-        g_scale = torch.empty(G, 3, **f32)
-        g_quat = torch.empty(G, 4, **f32)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_project_gaussians_bwd(
-                G, _lib.ptr(means3d), _lib.ptr(scales), float(ctx.glob_scale), _lib.ptr(quats), _lib.ptr(viewmat),
-                float(ctx.fx), float(ctx.fy), _lib.ptr(cov3d), _lib.ptr(radii), _lib.ptr(conics),
-                _lib.ptr(compensation), _lib.ptr(v_xys), _lib.ptr(v_depths), _lib.ptr(v_conics),
-                _lib.ptr(v_compensation), _lib.ptr(g_cov2d), _lib.ptr(g_cov3d), _lib.ptr(g_mean3d),
-                _lib.ptr(g_scale), _lib.ptr(g_quat), _lib.stream_ptr(dev)), "project_gaussians_backward")
+        g_mean3d, g_scale, g_quat = _project_bwd(means3d, scales, quats, viewmat, cov3d, radii, conics, compensation,
+                                                 ctx.glob_scale, ctx.fx, ctx.fy, v_xys, v_depths, v_conics,
+                                                 v_compensation)
         # v_cov3d (gradient of the returned cov3d) is ignored, as in gsplat 0.1.11
         v_viewmat = None
         if ctx.needs_input_grad[4]:

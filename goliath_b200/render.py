@@ -4,6 +4,7 @@
 `render(...)` keeps the reference signature and call sequence (project, rasterise rgb, rasterise depth as
 colour) so that its results are comparable call-for-call; the kernels underneath are the sm_90a ones.
 """
+from contextlib import nullcontext
 from typing import Optional
 
 import torch as th
@@ -84,9 +85,44 @@ _VIEW_STREAMS = {}
 MAX_VIEW_STREAMS = int(__import__("os").environ.get("GOLIATH_B200_VIEW_STREAMS", "4"))  # 0 / 1: views one after another
 
 
-class _nullctx:
-    def __enter__(self): return None
-    def __exit__(self, *a): return False
+def _intrinsics(K, intrinsics_host, n_views):
+    """(fx, fy, cx, cy) per view: `intrinsics_host` when the caller has them on the host, else read from K with four
+    `.item()` device syncs per view, as the reference does."""
+    if intrinsics_host is not None:
+        return intrinsics_host
+    return [(K[b, 0, 0].item(), K[b, 1, 1].item(), K[b, 0, 2].item(), K[b, 1, 2].item()) for b in range(n_views)]
+
+
+def _per_view(x, n_views, last):
+    """Per-view slices [-1, last] of a batched field as views whose backward is a plain view / stack: `x[b]` (select)
+    would make autograd zero-fill a full-batch tensor and copy into it for every field of every view (5 fills of up to
+    4.8 MB per view at B = 1)."""
+    return [x.reshape(-1, last)] if n_views == 1 else [t.reshape(-1, last) for t in th.unbind(x, 0)]
+
+
+def _issue_views(dev, n_views, capacity, render_view):
+    """[render_view(v) for v in range(n_views)], each a tuple of tensors.  With several views and the sync-free path
+    (`capacity` set) the views are issued on a small pool of side streams (view_streams): independent views overlap on
+    the device — one view's blend tail (SMs idle while the last tiles finish) runs under the next view's projection /
+    binning — and become parallel branches when the step is captured in a CUDA graph.  Each side stream waits for the
+    current stream before its first view, and the current stream waits for all of them at the end."""
+    pool = view_streams(dev, n_views) if (capacity is not None and n_views > 1) else None
+    main = th.cuda.current_stream(dev) if pool else None
+    outs = []
+    for v in range(n_views):
+        side = pool[v % len(pool)] if pool else None
+        if side is not None and v < len(pool):
+            side.wait_stream(main)
+        with (th.cuda.stream(side) if side is not None else nullcontext()):
+            out = render_view(v)
+        if side is not None:
+            for t in out:
+                t.record_stream(main)
+        outs.append(out)
+    if pool:
+        for side in pool[:min(n_views, len(pool))]:
+            main.wait_stream(side)
+    return outs
 
 
 def view_streams(dev, n_views):
@@ -180,43 +216,22 @@ def render_views(width: int, height: int, K: th.Tensor, Rt: th.Tensor, preds, in
     the sync-free fused path then waits for it only where the colours are first read (the record gather at the end of the
     binning), so projection, depth ranks, tile buckets and the per-tile sort run beside the shade."""
     B = Rt.shape[0]
+    intrinsics_host = _intrinsics(K, intrinsics_host, B)
     if fused:
-        # per view: one autograd node for project + bin/sort + pack + blend and one for the post-processing.  With several
-        # views and the sync-free path the views are issued on a small pool of side streams (view_streams): independent
-        # views overlap on the device — one view's blend tail (SMs idle while the last tiles finish) runs under the next
-        # view's projection / binning — and become parallel branches when the step is captured in a CUDA graph.
+        # per view: one autograd node for project + bin/sort + pack + blend and one for the post-processing
         from .gsplat.fused import render_fused
-        rgbs, alphas, depths = [], [], []
-        pool = view_streams(Rt.device, B) if (capacity is not None and B > 1) else None
-        main = th.cuda.current_stream(Rt.device) if pool else None
-        # per-view slices as views whose backward is a plain view / stack: `x[b]` (select) would make autograd zero-fill a
-        # full-batch tensor and copy into it for every field of every view (5 fills of up to 4.8 MB per view at B = 1)
-        def per_view(x, last):
-            return [x.reshape(-1, last)] if B == 1 else [t.reshape(-1, last) for t in th.unbind(x, 0)]
-        pv = dict(primpos=per_view(preds["primpos"], 3), primscale=per_view(preds["primscale"], 3),
-                  primqvec=per_view(preds["primqvec"], 4), opacity=per_view(preds["opacity"], 1),
-                  color=per_view(preds["color"], 3))
-        for b in range(B):
-            if intrinsics_host is not None:
-                fx, fy, cx, cy = intrinsics_host[b]
-            else:
-                fx, fy, cx, cy = K[b, 0, 0].item(), K[b, 1, 1].item(), K[b, 0, 2].item(), K[b, 1, 2].item()
-            side = pool[b % len(pool)] if pool else None
-            if side is not None and b < len(pool):
-                side.wait_stream(main)
-            with (th.cuda.stream(side) if side is not None else _nullctx()):
-                out4, alpha, _ = render_fused(
-                    pv["primpos"][b].contiguous(), pv["primscale"][b].contiguous(), 1.0, pv["primqvec"][b].contiguous(),
-                    Rt[b], fx, fy, cx, cy, height, width, pv["opacity"][b].contiguous(), pv["color"][b].contiguous(),
-                    _black(Rt.device), 0.1, capacity, colors_event=color_event)
-                r, a, d = _FinishView.apply(out4, alpha)
-            if side is not None:
-                for t_ in (r, a, d):
-                    t_.record_stream(main)
-            rgbs.append(r); alphas.append(a); depths.append(d)
-        if pool:
-            for side in pool[:min(B, len(pool))]:
-                main.wait_stream(side)
+        pv = {k: _per_view(preds[k], B, last)
+              for k, last in (("primpos", 3), ("primscale", 3), ("primqvec", 4), ("opacity", 1), ("color", 3))}
+
+        def render_view(b):
+            fx, fy, cx, cy = intrinsics_host[b]
+            out4, alpha, _ = render_fused(
+                pv["primpos"][b].contiguous(), pv["primscale"][b].contiguous(), 1.0, pv["primqvec"][b].contiguous(),
+                Rt[b], fx, fy, cx, cy, height, width, pv["opacity"][b].contiguous(), pv["color"][b].contiguous(),
+                _black(Rt.device), 0.1, capacity, colors_event=color_event)
+            return _FinishView.apply(out4, alpha)
+
+        rgbs, alphas, depths = zip(*_issue_views(Rt.device, B, capacity, render_view))
         if B == 1:
             return rgbs[0][None], alphas[0][None], depths[0][None]
         return th.stack(rgbs), th.stack(alphas), th.stack(depths)
@@ -224,10 +239,7 @@ def render_views(width: int, height: int, K: th.Tensor, Rt: th.Tensor, preds, in
         th.cuda.current_stream(Rt.device).wait_event(color_event)
     rgbs, Ts, depths = [], [], []
     for b in range(B):
-        if intrinsics_host is not None:
-            fx, fy, cx, cy = intrinsics_host[b]
-        else:
-            fx, fy, cx, cy = K[b, 0, 0].item(), K[b, 1, 1].item(), K[b, 0, 2].item(), K[b, 1, 2].item()
+        fx, fy, cx, cy = intrinsics_host[b]
         o = render(width, height, fx, fy, cx, cy, Rt[b], preds["primpos"][b], preds["primqvec"][b],
                    preds["primscale"][b], preds["opacity"][b], preds["color"][b], return_depth=True, fused=fused, capacity=capacity)
         rgbs.append(o["render"])
@@ -255,8 +267,7 @@ def render_views_envmap(width: int, height: int, K: th.Tensor, headrel_Rt: th.Te
     from .gsplat.olat import render_views_shared
 
     B = headrel_Rt.shape[0]
-    if intrinsics_host is None:
-        intrinsics_host = [(K[b, 0, 0].item(), K[b, 1, 1].item(), K[b, 0, 2].item(), K[b, 1, 2].item()) for b in range(B)]
+    intrinsics_host = _intrinsics(K, intrinsics_host, B)
     colors = th.stack([preds["color"].reshape(B, -1, 3), preds["diff_color"].reshape(B, -1, 3).clamp(min=0.0),
                        preds["spec_color"].reshape(B, -1, 3).clamp(min=0.0)], 1)
     geom = {k: preds[k] for k in ("primpos", "primqvec", "primscale", "opacity")}
