@@ -114,12 +114,19 @@ __device__ __forceinline__ Tile make_tile(int tile_id, int tbx) {
 //               per-warp list of hit indices, then blends the list four entries per round (one LDS.128 fetches the four
 //               indices): rounds are full except the last one of a stage, and the mask walk (brev / flo / lop per hit
 //               on the uniform path) is gone.  Same per-pixel operations in the same order -> identical pixels.
-template <int C, bool LIST, bool RANKED>
+// HITS (with LIST): each pixel warp also stores its hit lists for blend_bwd_lists_kernel.  Warp w of a tile with list
+//               range [x, y) appends the sorted indices of its hits, stage after stage, at hit_list[8x + w(y - x)] (a
+//               warp cannot hit more than y - x records, so the segments never overlap and need no device-side count),
+//               and writes hit_count[8 tile + w] = the number of leading entries the backward needs: up to and
+//               including the last hit any pixel of the warp blended (the backward's `idx <= final_idx` walk).  Block 0
+//               sets hit_count[8T], the backward's draw counter, to zero.  Only stores are added: pixels stay identical.
+template <int C, bool LIST, bool RANKED, bool HITS = false>
 __global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
     int img_w, int img_h, int tbx, const int* order, int sched, const int2* __restrict__ tile_bins,
     const float4* __restrict__ rec /* RANKED: the by-rank table */, const int* __restrict__ ranks /* RANKED only */,
     const float* __restrict__ background, float* __restrict__ final_Ts, int* __restrict__ final_idx,
-    float* __restrict__ out_img) {
+    float* __restrict__ out_img, int* __restrict__ hit_list = nullptr, int* __restrict__ hit_count = nullptr) {
+  static_assert(!HITS || LIST, "hit lists are the LIST variant's per-stage lists");
   __shared__ __align__(128) float4 s_rec[kFwdStages][kStageRecs * 3];
   __shared__ __align__(8) unsigned long long s_full[kFwdStages];
   __shared__ __align__(8) unsigned long long s_empty[kFwdStages];
@@ -217,6 +224,9 @@ __global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
   float T = 1.f;
   int cur_idx = 0;
   float acc[4] = {0.f, 0.f, 0.f, 0.f};
+  // HITS: this warp's list segment, entries stored so far, and the list position of the pixel's last blended hit
+  int* const seg = HITS ? hit_list + 8 * (size_t)range.x + (size_t)warp * (range.y - range.x) : nullptr;
+  int written = 0, last_pos = -1;
 
   bool counted = false;
   for (int b = 0; b < num_batches; ++b) {
@@ -262,6 +272,11 @@ __global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
         cnt += __popc(mask);
       }
       __syncwarp();
+      if (HITS) {
+        for (int i = lane; i < cnt; i += 32) seg[written + i] = batch_start + hl[i];
+        // a pixel that blends nothing keeps final_idx = 0, which the backward's walk still includes
+        if (b == 0 && range.x == 0 && cnt > 0 && hl[0] == 0 && inside) last_pos = 0;
+      }
       for (int i0 = 0; i0 < cnt; i0 += 16) {  // saturation is polled every four rounds
         const int i1 = min(i0 + 16, cnt);
         for (int i = i0; i < i1; i += 4) {
@@ -295,11 +310,13 @@ __global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
               if (C == 4) acc[3] += col[u].w * vis;
               T = next_T;
               cur_idx = batch_start + t[u];
+              if (HITS) last_pos = written + i + u;
             }
           }
         }
         if (__all_sync(0xffffffffu, done)) break;
       }
+      written += cnt;
     } else {
     for (int c0 = 0; c0 < batch_size; c0 += 32) {
         const int ti = c0 + lane;
@@ -349,6 +366,12 @@ __global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
   }
     __syncwarp();
     if (lane == 0) mbar_arrive(&s_empty[s]);
+  }
+  if (HITS) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) last_pos = max(last_pos, __shfl_xor_sync(0xffffffffu, last_pos, o));
+    if (lane == 0) hit_count[8 * tl.tile_id + warp] = last_pos + 1;
+    if (blockIdx.x == 0 && tr == 0) hit_count[8 * tbx * ((img_h + 15) >> 4)] = 0;
   }
   if (inside) {
     const size_t pix = (size_t)pyi * img_w + pxi;
@@ -688,6 +711,259 @@ __global__ void __launch_bounds__(kBwdThreads, 3) blend_bwd_mom_kernel(
   }
   if (cnt > 0) chunk(0, pad4(cnt));
   if (RANKED) cp_async_wait_all();
+}
+
+// ------------------------------------------------------------------ backward from the forward's hit lists
+// The ranked backward above has every pixel warp of a tile cull every record of the tile again, through a stage ring
+// that the slowest warp paces.  Here each (tile, pixel warp) is an independent work item: the warp walks the hit list
+// the forward stored for it (blend_fwd_ilp_kernel<.., HITS>) back to front, 16 entries per chunk, and gathers the
+// next chunk's records with cp.async straight from the by-id table into a double-buffered entry buffer while it runs
+// phase B of the current one (the list and id loads behind them are issued a chunk earlier).  Phases A / B and the REDs are those of blend_bwd_mom_kernel (entries in
+// record layout x y ex ey | A B C o | colour, index and id beside them), and the chunks hold the same hits in the same
+// order, so per warp the gradients are the same numbers; only the order of the atomic adds across warps changes.
+// Warps share nothing, so they draw items one at a time from a counter.  The kernel time is set by the warps with the
+// most hits, and those are not the warps of the longest tiles, so order_items_kernel first puts the items with hits in
+// descending order of their chunk count: the heaviest items start in the first wave, the light ones fill in behind.
+//
+// hit_count [16 T + 2]: per-item counts [8 T] (the forward) | draw counter (zeroed by the forward, reset by each
+// backward) | number of items with hits | those items, heaviest first [8 T] (order_items_kernel).
+constexpr int kListWarps = 4;
+constexpr int kListThreads = kListWarps * 32;
+constexpr int kOrderBuckets = 64;  // items are ordered by min(chunks, 63): bucket b holds items of 63 - b chunks
+
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+
+// one CTA: a counting sort of the n_items counts into descending chunk-count buckets (order inside a bucket is free)
+__global__ void __launch_bounds__(1024) order_items_kernel(int n_items, int* __restrict__ hit_count) {
+  __shared__ int s_off[kOrderBuckets];
+  const int tr = threadIdx.x, lane = tr & 31;
+  auto bucket = [](int n) { return kOrderBuckets - 1 - min((n + kChunk - 1) / kChunk, kOrderBuckets - 1); };
+  if (tr < kOrderBuckets) s_off[tr] = 0;
+  __syncthreads();
+  for (int i = tr; i < n_items; i += blockDim.x) {
+    const int n = hit_count[i];
+    if (n > 0) atomicAdd(&s_off[bucket(n)], 1);
+  }
+  __syncthreads();
+  if (tr < 32) {  // exclusive scan of the 64 bucket sizes, two per lane
+    const int a = s_off[2 * lane], b = s_off[2 * lane + 1];
+    int incl = a + b;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += t;
+    }
+    const int excl = incl - a - b;
+    s_off[2 * lane] = excl;
+    s_off[2 * lane + 1] = excl + a;
+    if (lane == 31) hit_count[n_items + 1] = incl;
+  }
+  __syncthreads();
+  int* items = hit_count + n_items + 2;
+  for (int i = tr; i < n_items; i += blockDim.x) {
+    const int n = hit_count[i];
+    if (n > 0) items[atomicAdd(&s_off[bucket(n)], 1)] = i;
+  }
+}
+
+template <int C>
+__global__ void __launch_bounds__(kListThreads, 6) blend_bwd_lists_kernel(
+    int img_w, int img_h, int tbx, int n_items, const int2* __restrict__ tile_bins, const int* __restrict__ hit_list,
+    const int* __restrict__ hit_count, int* draw /* hit_count + n_items */,
+    const int* __restrict__ ranks, const float4* __restrict__ rec, const float* __restrict__ background,
+    const float* __restrict__ final_Ts, const int* __restrict__ final_idx, const float* __restrict__ v_output,
+    const float* __restrict__ v_output_alpha, float* __restrict__ v_xy, float* __restrict__ v_conic,
+    float* __restrict__ v_colors, float* __restrict__ v_opacity) {
+  __shared__ __align__(16) float4 s_e[kListWarps][2][kChunk * 3];  // entries: the gathered records
+  __shared__ __align__(8) int2 s_ig[kListWarps][2][kChunk];        // (sorted index, Gaussian id) of each entry
+  __shared__ float2 s_m[kListWarps][kChunk * kMStride];            // (fac, v_sigma) of each (hit, pixel)
+  __shared__ float4 s_vo[kListWarps][32];
+
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  float2* M = s_m[wib];
+  float4* VO = s_vo[wib];
+  const int n_work = hit_count[n_items + 1];
+  const int* items = hit_count + n_items + 2;
+  const int n_draws = n_work + (int)gridDim.x * kListWarps;  // every warp's last draw finds the items exhausted
+  for (;;) {
+    int k = 0;
+    if (lane == 0) {
+      k = atomicAdd(draw, 1);
+      if (k == n_draws - 1) *draw = 0;  // the launch's last draw: the counter is ready for the next launch
+    }
+    k = __shfl_sync(0xffffffffu, k, 0);
+    if (k >= n_work) break;
+    const int item = items[k], tile = item >> 3, warp = item & 7;
+    const int n = hit_count[item];
+    const int2 range = tile_bins[tile];
+    const int* list = hit_list + 8 * (size_t)range.x + (size_t)warp * (range.y - range.x);
+    const Tile tl = make_tile(tile, tbx);
+    const int wx0 = tl.tx * 16 + ((warp & 1) << 3), wy0 = tl.ty * 16 + ((warp >> 1) << 2);
+    const int pxi = wx0 + (lane & 7), pyi = wy0 + (lane >> 3);
+    const bool inside = (pxi < img_w) && (pyi < img_h);
+    const float px = (float)pxi + 0.5f, py = (float)pyi + 0.5f;
+    const float fx0 = (float)wx0 + 0.5f, fy0 = (float)wy0 + 0.5f;
+    const size_t pix = inside ? ((size_t)pyi * img_w + pxi) : 0;
+
+    // chunk j holds list positions [top - cnt, top), top = n - 16 j, entry l = position top - 1 - l (back to front)
+    const int nchunks = (n + kChunk - 1) / kChunk;
+    int g_idx = 0, g_id = 0;  // this lane's entry of the next chunk to gather (lanes < 16)
+    auto load_next = [&](int j) {
+      const int top = n - kChunk * j;
+      if (lane < min(kChunk, top)) {
+        g_idx = list[top - 1 - lane];
+        g_id = ranks[g_idx];
+      }
+    };
+    // issue chunk j's gathers into buffer j & 1; pad its entry count up to a multiple of 4 with entries no pixel accepts
+    auto gather = [&](int j) {
+      const int cnt = min(kChunk, n - kChunk * j);
+      float4* E = s_e[wib][j & 1];
+      if (lane < cnt) {
+        const float4* src = rec + 3 * (size_t)g_id;
+        cp_async16(&E[lane * 3 + 0], src);
+        cp_async16(&E[lane * 3 + 1], src + 1);
+        cp_async16(&E[lane * 3 + 2], src + 2);
+        s_ig[wib][j & 1][lane] = make_int2(g_idx, g_id);
+      } else if (lane < ((cnt + 3) & ~3)) {
+        E[lane * 3 + 0] = make_float4(0.f, 0.f, 0.f, 0.f);
+        E[lane * 3 + 1] = make_float4(1.f, 0.f, 1.f, 0.f);
+        E[lane * 3 + 2] = make_float4(0.f, 0.f, 0.f, 0.f);
+        s_ig[wib][j & 1][lane] = make_int2(0x7fffffff, 0);
+      }
+      cp_async_commit();
+    };
+    load_next(0);
+    gather(0);
+
+    const float T_final = inside ? final_Ts[pix] : 1.f;
+    float T = T_final;
+    float bufv = 0.f;  // (colour accumulated behind the current Gaussian) . v_out
+    const int bin_final = inside ? final_idx[pix] : -1;
+    float vo[4] = {0.f, 0.f, 0.f, 0.f};
+    float voa = 0.f;
+    if (inside) {
+#pragma unroll
+      for (int c = 0; c < C; ++c) vo[c] = v_output[pix * C + c];
+      voa = v_output_alpha ? v_output_alpha[pix] : 0.f;  // NULL = no gradient through alpha
+    }
+    VO[lane] = make_float4(vo[0], vo[1], vo[2], vo[3]);
+    float bgdot = 0.f;
+#pragma unroll
+    for (int c = 0; c < C; ++c) bgdot += background[c] * vo[c];
+    const float tfc = T_final * (voa - bgdot);  // the two T_final * ra terms of v_alpha share it
+    if (nchunks > 1) load_next(1);
+
+    for (int j = 0; j < nchunks; ++j) {
+      const int cnt = min(kChunk, n - kChunk * j);
+      const int nn = j + 1 < nchunks ? kChunk : ((cnt + 3) & ~3);  // only the last chunk is short
+      const float4* E = s_e[wib][j & 1];
+      const int2* IG = s_ig[wib][j & 1];
+      cp_async_wait_all();  // chunk j has landed (chunk j + 1 is issued below)
+      __syncwarp();
+      // ---- phase A, lanes = pixels: the serial transmittance / colour-buffer recurrence over the chunk's hits
+#pragma unroll 1
+      for (int h0 = 0; h0 < nn; h0 += 4) {
+        float al[4], ov[4], ra[4];
+        float4 col[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const int h = h0 + u;
+          const float4 q0 = E[h * 3], q1 = E[h * 3 + 1];  // x y - - | A B C o
+          col[u] = E[h * 3 + 2];
+          const float dx = q0.x - px, dy = q0.y - py;
+          const float sigma = 0.5f * (q1.x * dx * dx + q1.z * dy * dy) + q1.y * dx * dy;
+          const float vis = exp_neg(sigma);
+          const float alpha = fminf(kAlphaMaxBwd, q1.w * vis);
+          // pixels outside the image have bin_final = -1, padding entries have idx = INT_MAX
+          const bool valid = (IG[h].x <= bin_final) && !(sigma < 0.f) && !(alpha < kAlphaMin);
+          al[u] = valid ? alpha : 0.f;
+          ov[u] = valid ? q1.w * vis : 0.f;
+          ra[u] = rcp_approx(1.f - al[u]);  // exactly 1 for the pairs that do not take part
+        }
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const float cc[4] = {col[u].x, col[u].y, col[u].z, col[u].w};
+          float cv = 0.f;
+#pragma unroll
+          for (int c = 0; c < C; ++c) cv += cc[c] * vo[c];
+          const float v_alpha = ((cv * T - bufv) + tfc) * ra[u];
+          T *= ra[u];
+          const float fac = al[u] * T;
+          bufv += cv * fac;
+          M[(h0 + u) * kMStride + lane] = make_float2(fac, -ov[u] * v_alpha);  // (fac, v_sigma); zeros when not valid
+        }
+      }
+      if (j + 1 < nchunks) {  // the next chunk's gathers run under phase B and the next phase A's start
+        gather(j + 1);
+        if (j + 2 < nchunks) load_next(j + 2);
+      }
+      __syncwarp();
+      // ---- phase B, lanes = (hit, half of the 8x4 footprint): colour sums and image moments of v_sigma, then RED
+      {
+        const int hh = lane & 15, half = lane >> 4;
+        const int he = min(hh, nn - 1);
+        const float4 q0 = E[he * 3], q1 = E[he * 3 + 1];
+        const int e_id = IG[he].y;
+        const float2* Mrow = M + hh * kMStride + half * 16;
+        const float4* V = VO + half * 16;
+        float g[4] = {0.f, 0.f, 0.f, 0.f};
+        float r00 = 0.f, r01 = 0.f, r10 = 0.f, r11 = 0.f, sii = 0.f;
+        float facmax = 0.f;  // fac = alpha * T > 0 exactly for the (hit, pixel) pairs that took a gradient
+#pragma unroll
+        for (int q = 0; q < 16; ++q) {
+          const float2 m = Mrow[q];
+          const float4 v = V[q];
+          const float fi = (float)(q & 7);
+          facmax = fmaxf(facmax, m.x);
+          g[0] += m.x * v.x;
+          g[1] += m.x * v.y;
+          g[2] += m.x * v.z;
+          if (C == 4) g[3] += m.x * v.w;
+          if (q < 8) {
+            r00 += m.y;
+            r10 += m.y * fi;
+          } else {
+            r01 += m.y;
+            r11 += m.y * fi;
+          }
+          sii += m.y * (fi * fi);
+        }
+        // pixel (i, j) of this half: dx = u - i, dy = v - j with j in {0, 1}
+        const float u_ = q0.x - fx0, v_ = q0.y - (fy0 + (float)(2 * half));
+        const float S0 = r00 + r01, Sj = r01, Si = r10 + r11, Sij = r11;
+        const float sx = u_ * S0 - Si, sy = v_ * S0 - Sj;       // sum v_sigma * dx, * dy
+        const float sxx = u_ * (u_ * S0 - 2.f * Si) + sii;      // sum v_sigma * dx^2
+        const float sxy = u_ * (v_ * S0 - Sj) - v_ * Si + Sij;  // sum v_sigma * dx * dy
+        const float syy = v_ * (v_ * S0 - 2.f * Sj) + Sj;       // sum v_sigma * dy^2  (j^2 == j)
+        float o[10];
+        o[0] = g[0]; o[1] = g[1]; o[2] = g[2]; o[3] = g[3];
+        o[4] = 0.5f * sxx; o[5] = sxy; o[6] = 0.5f * syy;
+        o[7] = q1.x * sx + q1.y * sy;  // v_xy.x = A sx + B sy
+        o[8] = q1.y * sx + q1.z * sy;  // v_xy.y = B sx + C sy
+        o[9] = S0;
+#pragma unroll
+        for (int i = 0; i < 10; ++i) o[i] += __shfl_xor_sync(0xffffffffu, o[i], 16);
+        facmax = fmaxf(facmax, __shfl_xor_sync(0xffffffffu, facmax, 16));
+        if (half == 0 && hh < nn && facmax > 0.f) {  // false hits (no valid pixel) add nothing
+          if (C == 4) {
+            gb::red_add_v4(v_colors + 4 * (size_t)e_id, o[0], o[1], o[2], o[3]);
+          } else {
+            gb::red_add(v_colors + 3 * (size_t)e_id + 0, o[0]);
+            gb::red_add(v_colors + 3 * (size_t)e_id + 1, o[1]);
+            gb::red_add(v_colors + 3 * (size_t)e_id + 2, o[2]);
+          }
+          gb::red_add(v_conic + 3 * (size_t)e_id + 0, o[4]);
+          gb::red_add(v_conic + 3 * (size_t)e_id + 1, o[5]);
+          gb::red_add(v_conic + 3 * (size_t)e_id + 2, o[6]);
+          gb::red_add_v2(v_xy + 2 * (size_t)e_id, o[7], o[8]);
+          // v_opacity = sum vis * v_alpha = -sum v_sigma / o   (o >= 1/255 wherever a pair was valid)
+          gb::red_add(v_opacity + e_id, -o[9] * rcp_approx(q1.w));
+        }
+      }
+      __syncwarp();  // phase B's reads of M / VO / this buffer are complete before they are overwritten
+    }
+  }
 }
 
 // ================================================================== four lighting conditions per pass (OLAT)
@@ -1171,18 +1447,22 @@ static bool fwd_list_variant() {
   return !(e && !strcmp(e, "rounds"));
 }
 
-// ranks == nullptr: `records` are the sorted 48-byte records; else `records` is the by-rank table and `ranks` the sorted ranks
+// ranks == nullptr: `records` are the sorted 48-byte records; else `records` is the by-rank table and `ranks` the sorted ranks.
+// hit_list != nullptr (ranked only): the forward also stores the hit lists for blend_bwd_lists_kernel.
 static int launch_fwd_any(int img_h, int img_w, int channels, const int32_t* tile_bins, const int32_t* tile_order, int sched,
                           const float* records, const int32_t* ranks, const float* background, float* out_img,
-                          float* final_Ts, int32_t* final_idx, cudaStream_t s) {
+                          float* final_Ts, int32_t* final_idx, cudaStream_t s, int32_t* hit_list = nullptr,
+                          int32_t* hit_count = nullptr) {
   const int tbx = gb::cdiv(img_w, 16), tby = gb::cdiv(img_h, 16);
   if (sched && !tile_order) return (int)cudaErrorInvalidValue;
   static const bool list = fwd_list_variant();
-#define GB_FWD_MOM(CC, LL, RR)                                                                                          \
-  blend_fwd_ilp_kernel<CC, LL, RR><<<tbx * tby, kFwdThreads, 0, s>>>(img_w, img_h, tbx, tile_order, sched,              \
-                                                                     (const int2*)tile_bins, (const float4*)records,    \
-                                                                     ranks, background, final_Ts, final_idx, out_img)
-  if (ranks) {
+#define GB_FWD_MOM(CC, LL, RR, ...)                                                                                     \
+  blend_fwd_ilp_kernel<CC, LL, RR, ##__VA_ARGS__><<<tbx * tby, kFwdThreads, 0, s>>>(                                   \
+      img_w, img_h, tbx, tile_order, sched, (const int2*)tile_bins, (const float4*)records, ranks, background, final_Ts, \
+      final_idx, out_img, hit_list, hit_count)
+  if (ranks && hit_list) {
+    if (channels == 3) GB_FWD_MOM(3, true, true, true); else GB_FWD_MOM(4, true, true, true);
+  } else if (ranks) {
     if (channels == 3) GB_FWD_MOM(3, true, true); else GB_FWD_MOM(4, true, true);
   } else if (channels == 3) {
     if (list) GB_FWD_MOM(3, true, false); else GB_FWD_MOM(3, false, false);
@@ -1226,6 +1506,42 @@ static int launch_bwd_any(int img_h, int img_w, int channels, const int32_t* gid
   return 0;
 }
 
+static int launch_bwd_lists(int img_h, int img_w, int channels, const int32_t* ranks, const int32_t* tile_bins,
+                            const int32_t* hit_list, int32_t* hit_count, const float* records,
+                            const float* background, const float* final_Ts, const int32_t* final_idx,
+                            const float* v_output, const float* v_output_alpha, float* v_xy, float* v_conic,
+                            float* v_colors, float* v_opacity, cudaStream_t s) {
+  const int tbx = gb::cdiv(img_w, 16), tby = gb::cdiv(img_h, 16);
+  const int n_items = 8 * tbx * tby;
+  int dev = 0;
+  GB_CUDA(cudaGetDevice(&dev));
+  // persistent grid: as many CTAs as fit on the device at once, each warp drawing items until they run out
+  static int resident[64][2] = {};
+  int uncached = 0;
+  int& per_sm = (dev >= 0 && dev < 64) ? resident[dev][channels == 4] : uncached;
+  if (per_sm == 0) {
+    int n = 0, sms = 0;
+    if (channels == 4)
+      GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, blend_bwd_lists_kernel<4>, kListThreads, 0));
+    else
+      GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, blend_bwd_lists_kernel<3>, kListThreads, 0));
+    GB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    per_sm = max(1, n) * sms;
+  }
+  const int grid = min(per_sm, gb::cdiv(n_items, kListWarps));
+  order_items_kernel<<<1, 1024, 0, s>>>(n_items, hit_count);
+#define GB_BWD_LISTS(CC)                                                                                                \
+  blend_bwd_lists_kernel<CC><<<grid, kListThreads, 0, s>>>(                                                             \
+      img_w, img_h, tbx, n_items, (const int2*)tile_bins, hit_list, hit_count, hit_count + n_items, ranks,              \
+      (const float4*)records, background, final_Ts, final_idx, v_output, v_output_alpha, v_xy, v_conic, v_colors,       \
+      v_opacity)
+  if (channels == 3) GB_BWD_LISTS(3); else GB_BWD_LISTS(4);
+#undef GB_BWD_LISTS
+  gb::count_launches(2);
+  GB_CHECK_LAUNCH();
+  return 0;
+}
+
 int launch_fwd_mom(int img_h, int img_w, int channels, const int32_t* tile_bins, const int32_t* tile_order, int sched,
                    const float* records, const float* background, float* out_img, float* final_Ts, int32_t* final_idx,
                    cudaStream_t s) {
@@ -1265,6 +1581,29 @@ GB_API int gb_rasterize_ranked_bwd(int img_h, int img_w, int channels, const int
   return gbblend::launch_bwd_any(img_h, img_w, channels, rank_to_gid, ranks_sorted, tile_bins, tile_order, 0, rec_by_rank,
                                  background, final_Ts, final_idx, v_output, v_output_alpha, v_xy, v_conic, v_colors,
                                  v_opacity, (cudaStream_t)stream);
+}
+// The same pair with the backward walking per-warp hit lists the forward stores (blend_bwd_lists_kernel): hit_list
+// [8 cap] and hit_count [16 T + 2] int32 (layout above order_items_kernel) are written by the forward and used by the
+// backward, which may be run more than once on them.
+GB_API int gb_rasterize_ranked_fwd_lists(int img_h, int img_w, int channels, const int32_t* tile_bins,
+                                         const int32_t* tile_order, const int32_t* ranks_sorted, const float* rec_by_rank,
+                                         const float* background, float* out_img, float* final_Ts, int32_t* final_idx,
+                                         int32_t* hit_list, int32_t* hit_count, void* stream) {
+  if (img_h <= 0 || img_w <= 0) return 0;
+  if ((channels != 3 && channels != 4) || !ranks_sorted || !hit_list || !hit_count) return (int)cudaErrorInvalidValue;
+  return gbblend::launch_fwd_any(img_h, img_w, channels, tile_bins, tile_order, 0, rec_by_rank, ranks_sorted, background,
+                                 out_img, final_Ts, final_idx, (cudaStream_t)stream, hit_list, hit_count);
+}
+GB_API int gb_rasterize_ranked_bwd_lists(int img_h, int img_w, int channels, const int32_t* ranks_sorted,
+                                         const int32_t* tile_bins, const int32_t* hit_list, int32_t* hit_count,
+                                         const float* rec_by_rank, const float* background, const float* final_Ts,
+                                         const int32_t* final_idx, const float* v_output, const float* v_output_alpha,
+                                         float* v_xy, float* v_conic, float* v_colors, float* v_opacity, void* stream) {
+  if (img_h <= 0 || img_w <= 0) return 0;
+  if ((channels != 3 && channels != 4) || !ranks_sorted || !hit_list || !hit_count) return (int)cudaErrorInvalidValue;
+  return gbblend::launch_bwd_lists(img_h, img_w, channels, ranks_sorted, tile_bins, hit_list, hit_count,
+                                   rec_by_rank, background, final_Ts, final_idx, v_output, v_output_alpha, v_xy, v_conic,
+                                   v_colors, v_opacity, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------- four lighting conditions per pass (OLAT), C ABI

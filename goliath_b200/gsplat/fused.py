@@ -293,32 +293,40 @@ class _BinBlend(Function):
             outs = (gids, records)
         bins, order = _bin_tiles(xys, depths, radii, conics, colors, opacity, comp, H, W, cap, plan, outs,
                                  ranked=plan.ranked, colors_ready=ev)
+        hit_list = hit_count = None
         with torch.cuda.device(dev):
             st = _lib.stream_ptr(dev)
             if plan.ranked:
-                _lib.check(L.gb_rasterize_ranked_fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(ranks),
-                                                     _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(out4), _lib.ptr(final_Ts),
-                                                     _lib.ptr(final_idx), st), "rasterize_ranked_forward")
+                # the forward stores each pixel warp's hits (sorted indices; 8 x cap int32 needs no device-side count)
+                # so that the backward walks them instead of culling every tile again
+                hit_list = torch.empty(8 * cap, **i32)
+                hit_count = torch.empty(16 * tb[0] * tb[1] + 2, **i32)
+                _lib.check(L.gb_rasterize_ranked_fwd_lists(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(ranks),
+                                                           _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(out4),
+                                                           _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(hit_list),
+                                                           _lib.ptr(hit_count), st), "rasterize_ranked_forward")
             else:
                 _lib.check(plan.fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4),
                                     _lib.ptr(out4), _lib.ptr(final_Ts), _lib.ptr(final_idx), st),
                            "rasterize_packed_forward")
-        ctx.save_for_backward(opacity, comp, bg4, gids, bins, order, records, final_Ts, final_idx, ranks)
+        ctx.save_for_backward(opacity, comp, bg4, gids, bins, order, records, final_Ts, final_idx, ranks, hit_list,
+                              hit_count)
         ctx.meta = (H, W, plan)
         ctx.set_materialize_grads(False)
         return out4, 1 - final_Ts
 
     @staticmethod
     def backward(ctx, v_out4, v_alpha):
-        opacity, comp, bg4, gids, bins, order, records, final_Ts, final_idx, ranks = ctx.saved_tensors
+        (opacity, comp, bg4, gids, bins, order, records, final_Ts, final_idx, ranks, hit_list,
+         hit_count) = ctx.saved_tensors
         H, W, plan = ctx.meta
 
         def blend(st, *grads):
             if plan.ranked:
-                _lib.check(_lib.lib().gb_rasterize_ranked_bwd(
-                    H, W, 4, _lib.ptr(gids), _lib.ptr(ranks), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records),
-                    _lib.ptr(bg4), _lib.ptr(final_Ts), _lib.ptr(final_idx), *map(_lib.ptr, grads), st),
-                    "rasterize_ranked_backward")
+                _lib.check(_lib.lib().gb_rasterize_ranked_bwd_lists(
+                    H, W, 4, _lib.ptr(ranks), _lib.ptr(bins), _lib.ptr(hit_list),
+                    _lib.ptr(hit_count), _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(final_Ts), _lib.ptr(final_idx),
+                    *map(_lib.ptr, grads), st), "rasterize_ranked_backward")
             else:
                 _lib.check(plan.bwd(H, W, 4, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records),
                                     _lib.ptr(bg4), _lib.ptr(final_Ts), _lib.ptr(final_idx), *map(_lib.ptr, grads), st),

@@ -215,6 +215,24 @@ int gb_rasterize_ranked_bwd(int img_h, int img_w, int channels, const int32_t* r
                             const float* background, const float* final_Ts, const int32_t* final_idx,
                             const float* v_output, const float* v_output_alpha, float* v_xy, float* v_conic,
                             float* v_colors, float* v_opacity, void* stream);
+/* The ranked pair with a backward that does not cull the tiles again: gb_rasterize_ranked_fwd_lists is
+ * gb_rasterize_ranked_fwd (identical out_img / final_Ts / final_idx) that also stores each pixel warp's footprint hits,
+ * as sorted indices into ranks_sorted, in hit_list [8 cap] int32 (warp w of a tile with range [x, y) at 8x + w(y - x))
+ * and in hit_count [16 T + 2] int32 the number of them the backward needs (hit_count[0 .. 8 T)); the rest of
+ * hit_count is the backward's work space (a draw counter the forward zeroes, and the (tile, warp) items ordered by hit
+ * count).  gb_rasterize_ranked_bwd_lists walks those lists back to front, one work item per (tile, pixel warp),
+ * heaviest items first, and gives gb_rasterize_ranked_bwd's gradients up to the order of the atomic adds; it may be run
+ * again on the same lists. */
+int gb_rasterize_ranked_fwd_lists(int img_h, int img_w, int channels, const int32_t* tile_bins, const int32_t* tile_order,
+                                  const int32_t* ranks_sorted, const float* rec_by_rank, const float* background,
+                                  float* out_img, float* final_Ts, int32_t* final_idx, int32_t* hit_list,
+                                  int32_t* hit_count, void* stream);
+int gb_rasterize_ranked_bwd_lists(int img_h, int img_w, int channels, const int32_t* ranks_sorted,
+                                  const int32_t* tile_bins, const int32_t* hit_list,
+                                  int32_t* hit_count, const float* rec_by_rank, const float* background,
+                                  const float* final_Ts, const int32_t* final_idx, const float* v_output,
+                                  const float* v_output_alpha, float* v_xy, float* v_conic, float* v_colors,
+                                  float* v_opacity, void* stream);
 
 /* launch order of the tiles, longest list first: order [T] int32 */
 int gb_tile_order(int num_tiles, const int32_t* tile_bins, int32_t* order, void* stream);
