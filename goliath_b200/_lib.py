@@ -117,6 +117,10 @@ SIGNATURES = {
     "gb_envmap_compose_bwd": (_i, [_i, _i, _i, _vp, _vp, _vp]),
     "gb_envmap_prefilter_sg": (_i, [_i, _i] + [_vp] * 5 + [_i, ctypes.c_ulonglong, _vp, _vp]),
     "gb_envmap_spin_table": (_i, [_i, _i, _i, _vp, _vp, _f, _f] + [_vp] * 6 + [_vp]),
+    "gb_mvp_shadow_march": (_i, [_i] * 5 + [_vp, _vp, _f] + [_vp] * 5 + [_i] * 4 + [_vp] * 3 + [_f, _f, _i, _i, _vp]),
+    "gb_olat_features": (_i, [_i] * 7 + [_f] + [_vp] * 9 + [_i, _vp, _vp]),
+    "gb_olat_compose_fwd": (_i, [_i] * 4 + [_vp] * 4 + [_i, _vp, _vp]),
+    "gb_olat_compose_bwd": (_i, [_i] * 4 + [_vp] * 6 + [_vp]),
     "gb_mvp_raymarch_bwd":(_i, [_i] * 4 + [_vp, _vp, _f] + [_vp] * 5 + [_i] * 3 + [_vp] + [_i] * 3 + [_vp] * 8
                             + [_i, _f, _f, _i, _i, _vp]),
 }

@@ -42,6 +42,8 @@ struct RMArgs {
   float4* rayrgba; float* raysat; float* shadow;                 // forward outputs (raysat/shadow nullable)
   const float4* grad_rayrgba;                                     // backward
   float* grad_primpos; float* grad_primrot; float* grad_primscale; float* grad_tplate; float* grad_warp;
+  int L;                                       // views per item (shadow march): transforms / bounds at n / L; 0 = 1
+  int U; const float* slab; const float* valid;  // shadow march: alpha slab [N/L,TD,U,U], valid mask [K] or null
 };
 
 __device__ __forceinline__ float3 ld3(const float* p) { return make_float3(p[0], p[1], p[2]); }
@@ -255,7 +257,7 @@ struct RaySetup {
   bool validthread;
   float3 raypos, raydir, pos;
   float t, rtmin, rtmax;
-  int nhit;
+  int nhit, item;
   int* hit;
   float2* ivl;
   const float *pp, *pr, *ps;
@@ -276,11 +278,12 @@ __device__ __forceinline__ RaySetup setup_ray(const RMArgs& a, int* s_hit, float
   r.raypos = ld3(a.raypos + 3 * o);
   r.raydir = ld3(a.raydir + 3 * o);
   const float2 tmm = a.tminmax[o];
-  r.pp = a.primpos + (size_t)r.n * a.K * 3;
-  r.pr = a.primrot + (size_t)r.n * a.K * 9;
-  r.ps = a.primscale + (size_t)r.n * a.K * 3;
+  r.item = a.L > 1 ? r.n / a.L : r.n;
+  r.pp = a.primpos + (size_t)r.item * a.K * 3;
+  r.pr = a.primrot + (size_t)r.item * a.K * 9;
+  r.ps = a.primscale + (size_t)r.item * a.K * 3;
   float rtmin = INFINITY, rtmax = -INFINITY;
-  r.nhit = build_hitlist(a.K, r.raypos, r.raydir, a.nodeaabb + (size_t)r.n * (2 * a.K - 1) * 6, r.pp, r.pr, r.ps, r.hit,
+  r.nhit = build_hitlist(a.K, r.raypos, r.raydir, a.nodeaabb + (size_t)r.item * (2 * a.K - 1) * 6, r.pp, r.pr, r.ps, r.hit,
                          r.ivl, rtmin, rtmax);
   r.rtmin = fmaxf(rtmin, tmm.x);
   r.rtmax = fminf(rtmax, tmm.y);
@@ -366,6 +369,77 @@ __global__ void raymarch_fwd_kernel(RMArgs a) {
   const size_t o = ((size_t)r.n * a.H + r.h) * a.W + r.w;
   a.rayrgba[o] = rgba;
   if (a.raysat) { a.raysat[3 * o] = raysat.x; a.raysat[3 * o + 1] = raysat.y; a.raysat[3 * o + 2] = raysat.z; }
+}
+
+// ------------------------------------------------------------------ deep shadow march over a shared alpha template
+// The relightable hand teacher (hand_teacher_mvp.py:274-358) marches, from each of L lights, a template whose rgb is the
+// constant 255 and whose alpha is the geometry decoder's slab, copied once per light, and keeps only the splat volume.
+// This kernel is raymarch_fwd_kernel<false, true> with the rgb and raysat work removed: the alpha accumulation,
+// saturation stop, fade and splat_shadow are the same expressions in the same order, so the splat volume depends on
+// the alpha channel alone, exactly as there.  View n reads the transforms and bounds of item n / L, and samples the
+// alpha slab [TD, U, U] of that item in place: primitive k = hy * (U / TW) + wx covers rows hy*TH.., columns wx*TW..
+// of the slab, so template voxel (z, y, x) of k is slab texel (z, hy*TH + y, wx*TW + x) (hand_teacher_mvp.py:289-311),
+// times valid[k].  Reading in place needs no per-item re-layout pass and no [B, K, TD, TH, TW] copy; the corners of a
+// trilinear lookup are U floats apart in y instead of TW, which costs cache lines, not extra passes.
+__device__ __forceinline__ float sample_alpha_slab(int D, int H, int W, int U, const float* base, float valid, float3 pos) {
+  const Tri t = tri_setup<true>(D, H, W, pos);
+  float w[8];
+  tri_weights(t, w);
+  float r = 0.f;
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    const int x = t.ix + (c & 1), y = t.iy + ((c >> 1) & 1), z = t.iz + ((c >> 2) & 1);
+    if (z >= 0 && z < D && y >= 0 && y < H && x >= 0 && x < W) r += (valid * base[((size_t)z * U + y) * U + x]) * w[c];
+  }
+  return r;
+}
+
+__global__ void shadow_march_kernel(RMArgs a) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int nwarps = (blockDim.x * blockDim.y + 31) >> 5;
+  int* s_hit = reinterpret_cast<int*>(smem);
+  float2* s_ivl = reinterpret_cast<float2*>(smem + (size_t)nwarps * kMaxHit * sizeof(int));
+  RaySetup r = setup_ray(a, s_hit, s_ivl);
+  const unsigned full = 0xffffffffu;
+  const size_t tsz = (size_t)a.TD * a.TH * a.TW;
+  const int nx = a.U / a.TW;
+  const float* slab = a.slab + (size_t)r.item * a.TD * a.U * a.U;
+  const float stepsize = a.stepsize;
+
+  float alpha = 0.f;
+  bool sat = false;
+  float t = r.t;
+  float3 pos = r.pos;
+  const bool live0 = !(t > r.rtmax + 1e-5f);
+  float tlo = warp_min(live0 ? t : INFINITY), thi = warp_max(live0 ? t : -INFINITY);
+  const float margin = 2.f * stepsize + 1e-3f;
+
+  while (!__all_sync(full, t > r.rtmax + 1e-5f || sat)) {
+    for (int ks = 0; ks < r.nhit; ++ks) {
+      const float2 iv = r.ivl[ks];
+      if (thi + margin < iv.x || tlo - margin > iv.y) continue;
+      const int k = r.hit[ks];
+      Local L = prim_local(r, k, pos);
+      if (inside_unit(L.y0) && !sat && t < r.rtmax + 1e-5f) {
+        const float3 y0 = L.y0;
+        const float fade = __expf(-a.fadescale * (__powf(fabsf(y0.x), a.fadeexp) + __powf(fabsf(y0.y), a.fadeexp) +
+                                                  __powf(fabsf(y0.z), a.fadeexp)));
+        const int hy = k / nx, wx = k - hy * nx;
+        float sw = sample_alpha_slab(a.TD, a.TH, a.TW, a.U, slab + (size_t)hy * a.TH * a.U + (size_t)wx * a.TW,
+                                     a.valid ? a.valid[k] : 1.f, y0);
+        sw *= fade;
+        splat_shadow(a.TD, a.TH, a.TW, 1.f - alpha, a.shadow + ((size_t)r.n * a.K + k) * 2 * tsz, y0);
+        const float newalpha = alpha + sw * stepsize;
+        const float contrib = fminf(newalpha, 1.f) - alpha;
+        alpha += 1.f * contrib;
+        if (newalpha >= 1.f) sat = true;
+      }
+    }
+    t += stepsize;
+    pos = pos + r.raydir * stepsize;
+    tlo += stepsize;
+    thi += stepsize;
+  }
 }
 
 // ------------------------------------------------------------------ forward, lane-compacted sampling (algo 0, no shadow)
@@ -969,6 +1043,39 @@ GB_API int gb_mvp_raymarch_bwd(int N, int H, int W, int K, const float* raypos, 
       GB_CUDA(cudaFuncSetAttribute(raymarch_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     raymarch_bwd_kernel<false><<<grid, block, smem, s>>>(a);
   }
+  gb::count_launches(1);
+  GB_CHECK_LAUNCH();
+  return 0;
+}
+
+// Deep shadow march of the relightable hand teacher (hand_teacher_mvp.py:274-358 with mvpraymarch(with_shadow=True)):
+// N = B * L light views, transforms [B,K,3] / [B,K,3,3] / [B,K,3] and bounds [B,2K-1,2,3] (gb_mvp_compute_aabb with
+// N = B) of item n / L, alpha slab [B,TD,U,U] sampled in place (U = n_prim_x * TW = n_prim_y * TH, K = n_prim_x *
+// n_prim_y), valid [K] or NULL.  Only output: the un-normalised splat volume shadow [N,K,TD,TH,TW,2], accumulated
+// into (the caller zero-fills it).  No rayrgba, no raysat.
+GB_API int gb_mvp_shadow_march(int N, int L, int H, int W, int K, const float* raypos, const float* raydir,
+                               float stepsize, const float* tminmax, const float* nodeaabb, const float* primpos,
+                               const float* primrot, const float* primscale, int TD, int TH, int TW, int U,
+                               const float* alpha_slab, const float* valid, float* shadow, float fadescale,
+                               float fadeexp, int blocksizex, int blocksizey, void* stream) {
+  RMArgs a = {};
+  a.N = N; a.H = H; a.W = W; a.K = K; a.raypos = raypos; a.raydir = raydir; a.stepsize = stepsize;
+  a.tminmax = (const float2*)tminmax; a.nodeaabb = nodeaabb; a.primpos = primpos; a.primrot = primrot;
+  a.primscale = primscale; a.TD = TD; a.TH = TH; a.TW = TW; a.fadescale = fadescale; a.fadeexp = fadeexp;
+  a.shadow = shadow; a.L = L; a.U = U; a.slab = alpha_slab; a.valid = valid;
+  const int chk = fill_and_launch_check(a, blocksizex, blocksizey);
+  if (chk > 0) return 0;
+  if (chk < 0 || L < 1 || N % L != 0 || TD < 1 || TH < 1 || TW < 1 || U % TW != 0 || U % TH != 0 ||
+      (U / TW) * (U / TH) != K || !alpha_slab || !shadow)
+    return (int)cudaErrorInvalidValue;
+  dim3 block(blocksizex, blocksizey);
+  dim3 grid(gb::cdiv(W, blocksizex), gb::cdiv(H, blocksizey), N);
+  const int nwarps = (blocksizex * blocksizey + 31) / 32;
+  const size_t smem = (size_t)nwarps * kMaxHit * (sizeof(int) + sizeof(float2));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (smem > 48 * 1024)
+    GB_CUDA(cudaFuncSetAttribute(shadow_march_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  shadow_march_kernel<<<grid, block, smem, s>>>(a);
   gb::count_launches(1);
   GB_CHECK_LAUNCH();
   return 0;

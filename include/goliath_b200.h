@@ -620,6 +620,40 @@ int gb_lbs_skin_bwd(int B, int V, int J, int vb, const float* mats, const int32_
                     const float* skin_weights, const float* global_scaling, const float* g_out, float* g_verts,
                     void* stream);
 
+/* ---------------------------------------------------------------- relightable hand teacher (row R8'') */
+
+/* replaces the deep shadow march of OLATRGBDecoder.forward_rgb (hand_teacher_mvp.py:274-358: the expanded [B*L, K,
+ * TD, TH, TW, 4] template through mvpraymarch(with_shadow=True)).  Forward only, arithmetic of the shadow-splatting
+ * forward march without its rgb.  N = B*L light views; view n reads the transforms [B,K,3] / [B,K,3,3] / [B,K,3] and
+ * bounds [B,2K-1,2,3] (gb_mvp_compute_aabb with N = B) of item n / L and samples the alpha slab [B,TD,U,U] in place
+ * (K = (U/TW)*(U/TH) primitives, row-major), times valid [K] (NULL = all valid).  shadow [N,K,TD,TH,TW,2] is
+ * accumulated into (the caller zero-fills it); nothing else is written. */
+int gb_mvp_shadow_march(int N, int L, int H, int W, int K, const float* raypos, const float* raydir, float stepsize,
+                        const float* tminmax, const float* nodeaabb, const float* primpos, const float* primrot,
+                        const float* primscale, int TD, int TH, int TW, int U, const float* alpha_slab,
+                        const float* valid, float* shadow, float fadescale, float fadeexp, int blocksizex,
+                        int blocksizey, void* stream);
+
+/* replaces the no_grad feature block of OLATRGBDecoder.forward_rgb (hand_teacher_mvp.py:359-439): U-Net input
+ * feat [B*L,7*TD,U,U] (light vector, view direction in the primitive frame, 1 - shadow), primshadow [B,TD,3,U,U]
+ * (the light mean of the normalised shadow, added when accumulate) and, when not NULL, the normalised shadow
+ * shadow_feat [B*L,TD,U,U].  Transforms in world units, light_pos [B,L,3], campos [B,3], shadow from
+ * gb_mvp_shadow_march. */
+int gb_olat_features(int B, int L, int K, int TD, int TH, int TW, int U, float volradius, const float* primpos,
+                     const float* primrot, const float* primscale, const float* valid, const float* light_pos,
+                     const float* campos, const float* shadow, float* feat, float* primshadow, int accumulate,
+                     float* shadow_feat, void* stream);
+
+/* replaces the OLAT compose of OLATRGBDecoder.forward_rgb (hand_teacher_mvp.py:468-479): rgb [B,Z,3,U,U] (added when
+ * accumulate) = sum_l s relu(25 t_c + 100) I[b,l,c] over tex [B*L,4Z,U,U] viewed [B,L,Z,4,U,U], s = sigmoid(t_0) or
+ * shadow_feat [B*L,Z,U,U] when not NULL; texolat [B,L,Z,3,U,U] = 25 t_c + 100 when not NULL. */
+int gb_olat_compose_fwd(int B, int L, int Z, int U, const float* tex, const float* intensity, const float* shadow_feat,
+                        float* rgb, int accumulate, float* texolat, void* stream);
+/* g_tex [B*L,4Z,U,U] (written) from g_rgb [B,Z,3,U,U] and g_texolat [B,L,Z,3,U,U] or NULL; t_0 gets zero when
+ * shadow_feat is given. */
+int gb_olat_compose_bwd(int B, int L, int Z, int U, const float* tex, const float* intensity, const float* shadow_feat,
+                        const float* g_rgb, const float* g_texolat, float* g_tex, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
