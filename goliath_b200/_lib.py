@@ -123,6 +123,11 @@ SIGNATURES = {
     "gb_olat_compose_bwd": (_i, [_i] * 4 + [_vp] * 6 + [_vp]),
     "gb_mvp_raymarch_bwd":(_i, [_i] * 4 + [_vp, _vp, _f] + [_vp] * 5 + [_i] * 3 + [_vp] + [_i] * 3 + [_vp] * 8
                             + [_i, _f, _f, _i, _i, _vp]),
+    "gb_upconv_block_fwd": (_i, [_i] * 6 + [_vp] * 10 + [_f] + [_vp] * 3 + [_vp]),
+    "gb_upconv_block_bwd": (_i, [_i] * 6 + [_vp] * 10 + [_f] + [_vp] * 10 + [_vp]),
+    "gb_sparse_rows_apply": (_i, [_i] * 3 + [_vp] * 4 + [_i64] * 3 + [_vp] + [_i64] * 3 + [_vp]),
+    "gb_conv3x3_ub_slice_fwd": (_i, [_i] * 5 + [_vp, _i64] + [_vp] * 4 + [_vp]),
+    "gb_conv3x3_ub_slice_bwd": (_i, [_i] * 5 + [_vp, _i64] + [_vp] * 6 + [_vp]),
 }
 
 

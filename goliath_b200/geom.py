@@ -84,15 +84,57 @@ def values_to_uv(values: torch.Tensor, index_img: torch.Tensor, bary_img: torch.
     return _ValuesToUV.apply(values, index_img, bary_img)
 
 
-class GeometryModule(torch.nn.Module):
-    """The part of the reference's GeometryModule (geom.py:186-278) the decoders use: `vn(verts)` and `to_uv(values)`.
-    vi [F,3]; index_image / bary_image [U,U,3] are the reference's precomputed assets."""
+def sample_uv_table(uv_coords: torch.Tensor, v2uv, H: int, W: int):
+    """the gather table of sample_uv (geom.py:281-304): bilinear at vt with align_corners=True and zeros padding, then
+    the mean over the v2uv columns (a padded row repeats its first entry, which the mean then weights more, as in the
+    reference).  One row per vertex (per UV coordinate without v2uv), 4 n_max entries."""
+    from .seams import GatherTable, _corners
 
-    def __init__(self, vi: torch.Tensor, index_image: torch.Tensor, bary_image: torch.Tensor):
+    vt = uv_coords.to(torch.float64).reshape(-1, 2)
+    cols, ws = _corners(vt[:, 0] * (W - 1), vt[:, 1] * (H - 1), H, W)
+    if v2uv is None:
+        return GatherTable(cols, ws, H * W)
+    idx = v2uv.to(torch.int64)
+    n_max = idx.shape[1]
+    return GatherTable(cols[idx].reshape(idx.shape[0], 4 * n_max), (ws[idx] / n_max).reshape(idx.shape[0], 4 * n_max),
+                       H * W)
+
+
+def sample_uv(values_uv: torch.Tensor, uv_coords: torch.Tensor, v2uv=None) -> torch.Tensor:
+    """geom.py:281-304 (mode bilinear, align_corners=True, flip_uvs=False): values_uv [B,C,H,W], uv_coords [N,2] ->
+    [B,N,C], or [B,V,C] averaged over the columns of v2uv [V,n_max].  Builds its table per call (no host sync); use
+    GeometryModule.from_uv to build it once."""
+    from .seams import gather
+
+    _lib.check_input(values_uv, "values_uv")
+    return gather(values_uv, sample_uv_table(uv_coords, v2uv, values_uv.shape[2], values_uv.shape[3]), rows_last=True)
+
+
+class GeometryModule(torch.nn.Module):
+    """The part of the reference's GeometryModule (geom.py:186-278) the decoders use: `vn(verts)`, `to_uv(values)` and,
+    given vt [N_uv,2] and v2uv [V,n_max], `from_uv(values_uv)`.  vi [F,3]; index_image / bary_image [U,U,3] are the
+    reference's precomputed assets."""
+
+    def __init__(self, vi: torch.Tensor, index_image: torch.Tensor, bary_image: torch.Tensor, vt=None, v2uv=None):
         super().__init__()
         self.register_buffer("vi", vi.to(torch.int32))
         self.register_buffer("index_image", index_image.to(torch.int32))
         self.register_buffer("bary_image", bary_image.to(torch.float32))
+        if vt is not None:
+            self.register_buffer("vt", torch.as_tensor(vt).to(torch.float32))
+            self.register_buffer("v2uv", torch.as_tensor(v2uv).to(torch.int32))
+        self._uv_table, self._uv_key = None, None
+
+    def from_uv(self, values_uv):
+        """geom.py:273-275: sample_uv(values_uv, vt, v2uv) with the gather table built once per (buffers, map size)"""
+        from .seams import gather
+
+        _lib.check_input(values_uv, "values_uv")
+        H, W = values_uv.shape[2], values_uv.shape[3]
+        key = (self.vt.device, self.vt.data_ptr(), self.vt._version, self.v2uv.data_ptr(), self.v2uv._version, H, W)
+        if self._uv_key != key:
+            self._uv_table, self._uv_key = sample_uv_table(self.vt, self.v2uv, H, W), key
+        return gather(values_uv, self._uv_table, rows_last=True)
 
     def vn(self, verts):
         return vert_normals(verts, self.vi)

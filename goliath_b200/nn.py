@@ -451,3 +451,117 @@ def glorot(m: nn.Module, alpha: float = 1.0) -> None:
         m.weight_g.fill_(float(m.weight_v.norm()))
         if m.bias is not None:
             m.bias.zero_()
+
+
+def _wn_chain(v, g, gw):
+    """weight-norm chain rule (g per output channel, norm over the whole tensor) from the effective-weight gradient"""
+    vnorm = v.norm()
+    w = g * v / vnorm
+    gg = (gw * v).sum(dim=tuple(range(1, v.dim())), keepdim=True) / vnorm
+    gv = g * gw / vnorm - (gw * w).sum() * v / (vnorm * vnorm)
+    return gv, gg.view_as(g)
+
+
+def _wn_scale(v, g):
+    return (g.reshape(-1) / v.norm()).contiguous()
+
+
+class _UpConvBlock(Function):
+    """UpConvBlockDeep forward / backward on csrc/upconv_wnub.cu (two kernels forward, eight backward)."""
+
+    @staticmethod
+    def forward(ctx, x, v1, g1, b1, v2, g2, b2, vr, gr, br, slope, groups):
+        x = x.contiguous()
+        _lib.check_input(x, "input")
+        for t, n in ((v1, "conv1.weight_v"), (v2, "conv2.weight_v"), (vr, "conv_resize.weight_v"),
+                     (b1, "conv1.bias"), (b2, "conv2.bias"), (br, "conv_resize.bias")):
+            _lib.check_input(t, n)
+        B, Cin, Hi, Wi = x.shape
+        Cout = v2.shape[0]
+        H, W = 2 * Hi, 2 * Wi
+        if (v1.shape != (Cin, Cin // groups, 3, 3) or v2.shape != (Cout, Cin // groups, 3, 3)
+                or vr.shape != (Cout, Cin // groups, 1, 1) or b1.shape != (Cin, H, W) or b2.shape != (Cout, H, W)):
+            raise RuntimeError("UpConvBlockDeep: parameter shapes do not match an input of %s" % (tuple(x.shape),))
+        s1, s2, sr = _wn_scale(v1, g1), _wn_scale(v2, g2), _wn_scale(vr, gr)
+        dev = x.device
+        h1 = torch.empty(B, Cin, H, W, device=dev)
+        out = torch.empty(B, Cout, H, W, device=dev)
+        train = any(ctx.needs_input_grad)
+        mask = torch.empty(B, Cout, H, W, device=dev, dtype=torch.uint8) if train else None
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().gb_upconv_block_fwd(
+                B, Cin, Cout, groups, Hi, Wi, _lib.ptr(x), _lib.ptr(v1), _lib.ptr(s1), _lib.ptr(b1), _lib.ptr(v2),
+                _lib.ptr(s2), _lib.ptr(b2), _lib.ptr(vr), _lib.ptr(sr), _lib.ptr(br), float(slope), _lib.ptr(h1),
+                _lib.ptr(out), _lib.ptr(mask), _lib.stream_ptr(dev)), "upconv_block_fwd")
+        if train:
+            ctx.save_for_backward(x, v1, g1, v2, g2, vr, gr, h1, mask)
+        ctx.slope, ctx.groups = float(slope), groups
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, v1, g1, v2, g2, vr, gr, h1, mask = ctx.saved_tensors
+        B, Cin, Hi, Wi = x.shape
+        Cout = v2.shape[0]
+        H, W = 2 * Hi, 2 * Wi
+        dev = x.device
+        gout = gout.contiguous()
+        s1, s2, sr = _wn_scale(v1, g1), _wn_scale(v2, g2), _wn_scale(vr, gr)
+        need_gx = ctx.needs_input_grad[0]
+        gz2 = torch.empty(B, Cout, H, W, device=dev)
+        gz1 = torch.empty(B, Cin, H, W, device=dev)
+        gu = torch.empty(B, Cin, H, W, device=dev) if need_gx else None
+        gx = torch.empty_like(x) if need_gx else None
+        gb1 = torch.empty(Cin, H, W, device=dev)
+        gb2 = torch.empty(Cout, H, W, device=dev)
+        gbr = torch.zeros(Cout, device=dev)
+        gw1, gw2, gwr = torch.zeros_like(v1), torch.zeros_like(v2), torch.zeros_like(vr)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().gb_upconv_block_bwd(
+                B, Cin, Cout, ctx.groups, Hi, Wi, _lib.ptr(x), _lib.ptr(v1), _lib.ptr(s1), _lib.ptr(v2), _lib.ptr(s2),
+                _lib.ptr(vr), _lib.ptr(sr), _lib.ptr(h1), _lib.ptr(mask), _lib.ptr(gout), ctx.slope, _lib.ptr(gz2),
+                _lib.ptr(gz1), _lib.ptr(gu), _lib.ptr(gb1), _lib.ptr(gb2), _lib.ptr(gbr), _lib.ptr(gw1), _lib.ptr(gw2),
+                _lib.ptr(gwr), _lib.ptr(gx), _lib.stream_ptr(dev)), "upconv_block_bwd")
+        gv1, gg1 = _wn_chain(v1, g1, gw1)
+        gv2, gg2 = _wn_chain(v2, g2, gw2)
+        gvr, ggr = _wn_chain(vr, gr, gwr)
+        return gx, gv1, gg1, gb1, gv2, gg2, gb2, gvr, ggr, gbr, None, None
+
+
+def _grouped(m, groups):
+    """give a weight-norm conv the reference's grouped weight_v [Cout, Cin/groups, k, k] (its kernel is the block's)"""
+    m.groups = groups
+    if groups != 1:
+        m.weight_v = nn.Parameter(torch.empty(m.out_channels, m.in_channels // groups, *m.kernel_size))
+        nn.init.kaiming_uniform_(m.weight_v, a=math.sqrt(5))
+        with torch.no_grad():
+            m.weight_g.fill_(float(m.weight_v.norm()))
+    return m
+
+
+class UpConvBlockDeep(nn.Module):
+    """blocks.py:382-434: bilinear x2 upsample (align_corners=True), grouped weight-normalised 1x1 skip with tied bias,
+    two grouped 3x3 Conv2dWNUB + LeakyReLU; the whole block runs on the two fused kernels of csrc/upconv_wnub.cu, and
+    `lrelu1` / `lrelu2` are parameter-free placeholders.  `size` is the OUTPUT size; the input is [B, Cin, size/2,
+    size/2].  Parameter names and shapes are the reference's."""
+
+    def __init__(self, in_channels, out_channels, size, lrelu_slope=0.2, wnorm_dim=0, groups=1):
+        super().__init__()
+        if wnorm_dim != 0:
+            raise NotImplementedError("only wnorm_dim = 0 (g per output channel) is supported")
+        if in_channels % groups or out_channels % groups or size % 2:
+            raise ValueError("channels must divide into groups and size must be even")
+        self.size, self.groups, self.lrelu_slope = size, groups, float(lrelu_slope)
+        self.conv_resize = _grouped(Conv2dWN(in_channels, out_channels, kernel_size=1), groups)
+        self.conv1 = _grouped(Conv2dWNUB(in_channels, in_channels, size, size, 3, 1, 1), groups)
+        self.lrelu1 = FusedLeakyReLU()
+        self.conv2 = _grouped(Conv2dWNUB(in_channels, out_channels, size, size, 3, 1, 1), groups)
+        self.lrelu2 = FusedLeakyReLU()
+
+    def forward(self, x):
+        if x.dim() != 4 or x.shape[2] * 2 != self.size or x.shape[3] * 2 != self.size:
+            raise RuntimeError("UpConvBlockDeep(size=%d) needs a [B, C, %d, %d] input (got %s)"
+                               % (self.size, self.size // 2, self.size // 2, tuple(x.shape)))
+        c1, c2, cr = self.conv1, self.conv2, self.conv_resize
+        return _UpConvBlock.apply(x, c1.weight_v, c1.weight_g, c1.bias, c2.weight_v, c2.weight_g, c2.bias,
+                                  cr.weight_v, cr.weight_g, cr.bias, self.lrelu_slope, self.groups)

@@ -654,6 +654,49 @@ int gb_olat_compose_fwd(int B, int L, int Z, int U, const float* tex, const floa
 int gb_olat_compose_bwd(int B, int L, int Z, int U, const float* tex, const float* intensity, const float* shadow_feat,
                         const float* g_rgb, const float* g_texolat, float* g_tex, void* stream);
 
+/* ---------------------------------------------------------------- body decoder (row R9, csrc/upconv_wnub.cu) */
+
+/* replaces blocks.UpConvBlockDeep.forward (ca_code/nn/blocks.py:382-434): UpsamplingBilinear2d (align_corners=True,
+ * x2), the weight-normalised grouped conv_resize 1x1 (tied bias), conv1 / conv2 3x3 "same" (la.Conv2dUB, untied bias
+ * [C,2Hi,2Wi], layers.py:276-327) and both LeakyReLUs, in two kernels; u and the skip are never written.
+ * x [B,Cin,Hi,Wi]; v1 [Cin,Cin/G,3,3], v2 [Cout,Cin/G,3,3], vr [Cout,Cin/G]; s1 / s2 / sr = weight_g / ||weight_v||_F
+ * per output channel; b1 [Cin,H,W], b2 [Cout,H,W], br [Cout].  h1 [B,Cin,H,W] (conv1's activation, kept for the
+ * backward), out [B,Cout,H,W]; mask [B,Cout,H,W] uint8 = conv2's pre-activation > 0, or NULL when no backward follows. */
+int gb_upconv_block_fwd(int B, int Cin, int Cout, int groups, int Hi, int Wi, const float* x, const float* v1,
+                        const float* s1, const float* b1, const float* v2, const float* s2, const float* b2,
+                        const float* vr, const float* sr, const float* br, float slope, float* h1, float* out,
+                        unsigned char* mask, void* stream);
+/* backward of the above (replaces the autograd graph of the same lines).  Scratch gz2 [B,Cout,H,W], gz1 and gu
+ * [B,Cin,H,W]; gb1 [Cin,H,W] and gb2 [Cout,H,W] written (batch sums); gbr [Cout], gw1, gw2 and gwr ACCUMULATED (caller
+ * zeroes them): gradients of the effective weights at unit scale.  gx [B,Cin,Hi,Wi] or NULL is a gather over the
+ * upsample's footprint (no atomics). */
+int gb_upconv_block_bwd(int B, int Cin, int Cout, int groups, int Hi, int Wi, const float* x, const float* v1,
+                        const float* s1, const float* v2, const float* s2, const float* vr, const float* sr,
+                        const float* h1, const unsigned char* mask, const float* gout, float slope, float* gz2,
+                        float* gz1, float* gu, float* gb1, float* gb2, float* gbr, float* gw1, float* gw2, float* gwr,
+                        float* gx, void* stream);
+
+/* replaces impaint_batch / resample_tex (ca_code/utils/seams.py:14-41: index_put of src texels into dst texels,
+ * (1-w) tex + w grid_sample(tex, 2(uv-0.5)) with align_corners=False and border padding) and sample_uv
+ * (ca_code/utils/geom.py:273-304: grid_sample at vt with align_corners=True, zeros padding, then the mean over the
+ * v2uv columns), forward and backward, as one fixed-order gather per output row:
+ *   out[b, c, r] = sum_{e in [row_ptr[r], row_ptr[r+1])} coef[e] in[b, c, col[e]]
+ * with element strides per tensor (in_bs / in_cs / in_rs per item / channel / row).  The backward is the same call on
+ * the transposed table, built once per set of seam buffers, so both directions are deterministic. */
+int gb_sparse_rows_apply(int B, int C, int n_rows, const int* row_ptr, const int* col, const float* coef,
+                         const float* in, long long in_bs, long long in_cs, long long in_rs, float* out,
+                         long long out_bs, long long out_cs, long long out_rs, void* stream);
+
+/* replaces th.split + la.Conv2dWNUB of mesh_vae.py:615-621 (verts_conv / tex_conv, 3x3 "same", untied bias, no
+ * activation, on channels [0,4) / [4,8) of the seam-sampled map) without a copy of the slice: item b of x (and of gx)
+ * starts at b * x_bs floats.  v [Cout,Cin,3,3], scale [Cout], bias [Cout,H,W], out [B,Cout,H,W]. */
+int gb_conv3x3_ub_slice_fwd(int B, int Cin, int Cout, int H, int W, const float* x, long long x_bs, const float* v,
+                            const float* scale, const float* bias, float* out, void* stream);
+/* g_bias [Cout,H,W] written; gw [Cout,Cin,3,3] ACCUMULATED (unit scale); gx written on channels [0,Cin) of each item,
+ * or NULL. */
+int gb_conv3x3_ub_slice_bwd(int B, int Cin, int Cout, int H, int W, const float* x, long long x_bs, const float* v,
+                            const float* scale, const float* gout, float* g_bias, float* gx, float* gw, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
