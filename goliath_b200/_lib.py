@@ -128,6 +128,9 @@ SIGNATURES = {
     "gb_sparse_rows_apply": (_i, [_i] * 3 + [_vp] * 4 + [_i64] * 3 + [_vp] + [_i64] * 3 + [_vp]),
     "gb_conv3x3_ub_slice_fwd": (_i, [_i] * 5 + [_vp, _i64] + [_vp] * 4 + [_vp]),
     "gb_conv3x3_ub_slice_bwd": (_i, [_i] * 5 + [_vp, _i64] + [_vp] * 6 + [_vp]),
+    "gb_body_tex_compose_workspace_bytes": (_sz, [_i, _i]),
+    "gb_body_tex_compose_fwd": (_i, [_i] * 3 + [_vp] * 5 + [_f] + [_vp] * 3 + [_vp]),
+    "gb_body_tex_compose_bwd": (_i, [_i] * 3 + [_vp] * 5 + [_f] + [_vp] * 9 + [_vp]),
 }
 
 

@@ -15,7 +15,10 @@ import torch.nn as tnn
 from torch.autograd import Function
 
 from . import _lib
-from .nn import ConvBlock, Conv2dWNUB, LinearWN, UpConvBlockDeep, _wn_chain, _wn_scale, glorot, tile2d
+from .nn import (ConvBlock, Conv2dWNUB, FusedLeakyReLU, LinearWN, UpConvBlockDeep, _wn_chain, _wn_scale, glorot,
+                 tile2d)
+from .seams import SeamSampler
+from .unet import UNetWB
 
 
 class _ConvSlices(Function):
@@ -138,3 +141,150 @@ class ConvDecoder(tnn.Module):
         verts_uv_delta_rec = verts_uv * self.verts_scale
         return {"geom_delta_rec": self.geo_fn.from_uv(verts_uv_delta_rec), "geom_uv_delta_rec": verts_uv_delta_rec,
                 "tex_mean_rec": tex * self.tex_scale, "embs_conv": embs_conv, "pose_conv": pose_conv}
+
+
+class UNetViewDecoder(tnn.Module):
+    """mesh_vae.py:633-649.  `geo_fn` carries `vi` [F,3], `index_image` [S,S,3] and `bary_image` [S,S,3] (a
+    `goliath_b200.geom.GeometryModule`); the view cosine (compute_view_cos + values_to_uv, geom.py:308-352, zero at
+    uncovered texels) runs under no_grad on `hand_mvp.view_cos_uv`, the U-Net on `goliath_b200.unet.UNetWB`."""
+
+    def __init__(self, geo_fn, net_uv_size, seam_sampler, n_init_ftrs=8):
+        super().__init__()
+        self.geo_fn = geo_fn
+        self.net_uv_size = net_uv_size
+        self.unet = UNetWB(4, 3, n_init_ftrs=n_init_ftrs, size=net_uv_size)
+        self.register_buffer("faces", geo_fn.vi.to(torch.int64), persistent=False)
+
+    def forward(self, geom_rec, tex_mean_rec, camera_pos):
+        from .hand_mvp import view_cos_uv
+
+        with torch.no_grad():
+            vc = view_cos_uv(geom_rec, self.geo_fn.vi, camera_pos, self.geo_fn.index_image, self.geo_fn.bary_image)
+        cond_view = torch.cat([vc, tex_mean_rec], dim=1)
+        return {"tex_view_rec": self.unet(cond_view), "cond_view": cond_view}
+
+
+class UpscaleNet(tnn.Module):
+    """mesh_vae.py:652-678: conv_block (3x3 Conv2dWNUB + LeakyReLU, fused) and the 1x1 untied-bias out_block on the
+    stride-1 kernels, then torch's pixel_shuffle.  Inside `TextureComposer` the out_block and the pixel shuffle run in
+    the composite kernel instead."""
+
+    def __init__(self, in_channels, out_channels, n_ftrs, size=1024, upscale_factor=2):
+        super().__init__()
+        conv = Conv2dWNUB(in_channels, n_ftrs, size, size, kernel_size=3, padding=1)
+        conv.fused_slope = 0.2
+        self.conv_block = tnn.Sequential(conv, FusedLeakyReLU())
+        self.out_block = Conv2dWNUB(n_ftrs, out_channels * upscale_factor ** 2, size, size, kernel_size=1, padding=0)
+        self.pixel_shuffle = tnn.PixelShuffle(upscale_factor=upscale_factor)
+        self.apply(lambda m: glorot(m, 0.2))
+        glorot(self.out_block, 1.0)
+
+    def forward(self, x):
+        if not x.is_cuda:
+            raise RuntimeError("UpscaleNet runs on CUDA only (no CPU fallback): the input is on %s" % x.device)
+        return self.pixel_shuffle(self.out_block(self.conv_block(x)))
+
+
+class _TexCompose(Function):
+    """P = ((U(T1) + PS(out_block(h))) * tex_std + tex_mean) * S3 on csrc/body_tex.cu (mesh_vae.py:211-222 with
+    mesh_vae.py:670-678); the backward recomputes the pre-shadow texture."""
+
+    @staticmethod
+    def forward(ctx, t1, h, v, g, bias, tex_mean, s3, tex_std):
+        t1, h, s3 = t1.contiguous(), h.contiguous(), s3.contiguous()
+        v2, bias = v.reshape(v.shape[0], -1).contiguous(), bias.contiguous()
+        tex_mean = tex_mean.contiguous()
+        for t, n in ((t1, "T1"), (h, "h"), (v2, "out_block.weight_v"), (bias, "out_block.bias"),
+                     (tex_mean, "tex_mean"), (s3, "shadow map")):
+            _lib.check_input(t, n)
+        B, C, H, W = t1.shape
+        if (C != 3 or h.shape != (B, 4, H, W) or v2.shape != (12, 4) or bias.shape != (12, H, W)
+                or tex_mean.shape != (1, 3, 2 * H, 2 * W) or s3.shape != (B, 1, 2 * H, 2 * W)):
+            raise RuntimeError("texture composite: shapes do not match T1 %s" % (tuple(t1.shape),))
+        scale = _wn_scale(v, g)
+        out = torch.empty(B, 3, 2 * H, 2 * W, device=t1.device)
+        with torch.cuda.device(t1.device):
+            _lib.check(_lib.lib().gb_body_tex_compose_fwd(
+                B, H, W, _lib.ptr(t1), _lib.ptr(h), _lib.ptr(v2), _lib.ptr(scale), _lib.ptr(bias), float(tex_std),
+                _lib.ptr(tex_mean), _lib.ptr(s3), _lib.ptr(out), _lib.stream_ptr(t1.device)), "body_tex_compose_fwd")
+        ctx.save_for_backward(t1, h, v, g, bias, tex_mean, s3)
+        ctx.tex_std = float(tex_std)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_out):
+        t1, h, v, g, bias, tex_mean, s3 = ctx.saved_tensors
+        B, _, H, W = t1.shape
+        dev = t1.device
+        g_out = g_out.contiguous()
+        scale = _wn_scale(v, g)
+        g_t1, g_h, g_s3 = torch.empty_like(t1), torch.empty_like(h), torch.empty_like(s3)
+        g_bias = torch.empty_like(bias)
+        g_w = torch.zeros_like(v)
+        L = _lib.lib()
+        ws = torch.empty(L.gb_body_tex_compose_workspace_bytes(H, W) // 4, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(L.gb_body_tex_compose_bwd(
+                B, H, W, _lib.ptr(t1), _lib.ptr(h), _lib.ptr(v.reshape(v.shape[0], -1).contiguous()),
+                _lib.ptr(scale), _lib.ptr(bias), ctx.tex_std, _lib.ptr(tex_mean), _lib.ptr(s3), _lib.ptr(g_out),
+                _lib.ptr(g_t1), _lib.ptr(g_h), _lib.ptr(g_bias), _lib.ptr(g_w), _lib.ptr(g_s3), _lib.ptr(ws),
+                _lib.stream_ptr(dev)), "body_tex_compose_bwd")
+        gv, gg = _wn_chain(v, g, g_w)
+        return g_t1, g_h, gv, gg, g_bias, None, g_s3, None
+
+
+class TextureComposer(tnn.Module):
+    """mesh_vae.AutoEncoder.forward_tex (mesh_vae.py:204-228) with the `upscale_net`, `seam_sampler`,
+    `seam_sampler_2k` and `tex_mean` [1,3,2S,2S] of the reference's AutoEncoder under the same key names, so that
+    subset of an AutoEncoder checkpoint loads strictly.  `tex_mean` is passed in prepared (the blur and resize of the
+    asset's colour mean is one-off asset preparation); `tex_std` is a float as in the reference.
+
+    forward(tex_mean_rec [B,3,S,S], tex_view_rec [B,3,S,S], shadow_map [B,1,2S,2S]) -> tex_rec [B,3,2S,2S]:
+      T1 = seam_sampler(tex_mean_rec + tex_view_rec)                 (impaint + resample, one gather)
+      h  = upscale_net.conv_block(cat(tex_mean_rec, tex_view_rec))
+      S3 = seam_sampler_2k.resample(seam_sampler_2k(shadow_map))
+      P  = ((U(T1) + PS(out_block(h))) * tex_std + tex_mean) * S3     (csrc/body_tex.cu, one kernel)
+      tex_rec = seam_sampler_2k.resample(seam_sampler_2k(P))
+    Unlike the reference, whose impaint writes into the caller's shadow_map through a view, the inputs are left as they
+    are; the gradients are the same."""
+
+    def __init__(self, seam_sampler, seam_sampler_2k, tex_mean, tex_std=64.0, n_ftrs=4):
+        super().__init__()
+        for sampler in (seam_sampler, seam_sampler_2k):
+            if not isinstance(sampler, SeamSampler):
+                raise TypeError("TextureComposer needs goliath_b200.seams.SeamSampler instances")
+        self.upscale_net = UpscaleNet(in_channels=6, out_channels=3, n_ftrs=n_ftrs, size=1024, upscale_factor=2)
+        self.seam_sampler = seam_sampler
+        self.seam_sampler_2k = seam_sampler_2k
+        self.register_buffer("tex_mean", torch.as_tensor(tex_mean, dtype=torch.float32))
+        self.tex_std = tex_std
+        if self.tex_mean.dim() != 4 or tuple(self.tex_mean.shape[:2]) != (1, 3):
+            raise ValueError("tex_mean must be [1, 3, 2S, 2S] (got %s)" % (tuple(self.tex_mean.shape),))
+
+    def _check(self, tex_mean_rec, tex_view_rec, shadow_map):
+        """tex_mean must be twice the size of tex_mean_rec, and each sampler built for the maps it receives"""
+        S = tex_mean_rec.shape[-1]
+        size2 = tuple(self.tex_mean.shape[2:])
+        if (tex_mean_rec.shape[-2:] != (S, S) or tex_view_rec.shape != tex_mean_rec.shape
+                or size2 != (2 * S, 2 * S) or shadow_map.shape[-2:] != size2):
+            raise RuntimeError("TextureComposer: tex_mean %s must be twice the size of tex_mean_rec %s, and the "
+                               "shadow map %s of tex_mean's size" % (tuple(self.tex_mean.shape),
+                                                                     tuple(tex_mean_rec.shape),
+                                                                     tuple(shadow_map.shape)))
+        for sampler, size, n in ((self.seam_sampler, (S, S), "seam_sampler"),
+                                 (self.seam_sampler_2k, size2, "seam_sampler_2k")):
+            got = tuple(sampler.uvs.shape[:2])
+            if got != size:
+                raise RuntimeError("%s was built for %s maps, it receives %s" % (n, got, size))
+
+    def forward(self, tex_mean_rec, tex_view_rec, shadow_map):
+        for t, n in ((tex_mean_rec, "tex_mean_rec"), (tex_view_rec, "tex_view_rec"), (shadow_map, "shadow_map")):
+            if not t.is_cuda:
+                raise RuntimeError("TextureComposer runs on CUDA only (no CPU fallback): %s is on %s" % (n, t.device))
+        self._check(tex_mean_rec, tex_view_rec, shadow_map)
+        t1 = self.seam_sampler(tex_mean_rec + tex_view_rec)
+        h = self.upscale_net.conv_block(torch.cat([tex_mean_rec, tex_view_rec], dim=1))
+        s3 = self.seam_sampler_2k.resample(self.seam_sampler_2k(shadow_map))
+        ob = self.upscale_net.out_block
+        p = _TexCompose.apply(t1, h, ob.weight_v, ob.weight_g, ob.bias, self.tex_mean, s3, self.tex_std)
+        return self.seam_sampler_2k.resample(self.seam_sampler_2k(p))

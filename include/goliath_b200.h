@@ -697,6 +697,27 @@ int gb_conv3x3_ub_slice_fwd(int B, int Cin, int Cout, int H, int W, const float*
 int gb_conv3x3_ub_slice_bwd(int B, int Cin, int Cout, int H, int W, const float* x, long long x_bs, const float* v,
                             const float* scale, const float* gout, float* g_bias, float* gx, float* gw, void* stream);
 
+/* replaces the 2048^2 part of mesh_vae.AutoEncoder.forward_tex (ca_code/models/mesh_vae.py:211-222: bilinear x2
+ * upsample with align_corners=False, `+ upscale_net(x)`, `* tex_std + tex_mean`, `* shadow_map`) together with the
+ * end of UpscaleNet.forward (mesh_vae.py:670-678: the 4 -> 12 1x1 out_block with untied bias, then PixelShuffle(2)):
+ *   out[b,c,y,x] = ((U(t1)[b,c,y,x] + z[b, 4c + 2(y%2) + x%2, y/2, x/2]) * tex_std + tex_mean[c,y,x]) * s3[b,y,x],
+ *   z[b,o,i,j] = scale[o] * sum_k v[o,k] h[b,k,i,j] + bias[o,i,j]
+ * t1 [B,3,H,W], h [B,4,H,W], v [12,4] (out_block.weight_v), scale [12] = weight_g / ||weight_v||_F, bias [12,H,W],
+ * tex_mean [1,3,2H,2W], s3 [B,1,2H,2W], out [B,3,2H,2W].  Neither z, the upsampled map nor the pre-shadow texture is
+ * written. */
+int gb_body_tex_compose_fwd(int B, int H, int W, const float* t1, const float* h, const float* v, const float* scale,
+                            const float* bias, float tex_std, const float* tex_mean, const float* s3, float* out,
+                            void* stream);
+/* backward of the above; recomputes the pre-shadow texture from t1, h and the weights.  g_t1 [B,3,H,W] (a gather over
+ * the upsample's footprint, no atomics), g_h [B,4,H,W], g_bias [12,H,W] (batch sum) and g_s3 [B,1,2H,2W] written;
+ * g_w [12,4] ACCUMULATED (caller zeroes it) = gradient of the effective weight at unit scale, summed in a fixed order
+ * through `workspace` (gb_body_tex_compose_workspace_bytes(H, W) bytes), so repeated calls are bitwise equal. */
+size_t gb_body_tex_compose_workspace_bytes(int H, int W);
+int gb_body_tex_compose_bwd(int B, int H, int W, const float* t1, const float* h, const float* v, const float* scale,
+                            const float* bias, float tex_std, const float* tex_mean, const float* s3,
+                            const float* g_out, float* g_t1, float* g_h, float* g_bias, float* g_w, float* g_s3,
+                            float* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
