@@ -131,6 +131,11 @@ SIGNATURES = {
     "gb_body_tex_compose_workspace_bytes": (_sz, [_i, _i]),
     "gb_body_tex_compose_fwd": (_i, [_i] * 3 + [_vp] * 5 + [_f] + [_vp] * 3 + [_vp]),
     "gb_body_tex_compose_bwd": (_i, [_i] * 3 + [_vp] * 5 + [_f] + [_vp] * 9 + [_vp]),
+    "gb_mesh_raster_workspace_bytes": (_sz, [_i] * 4),
+    "gb_mesh_raster": (_i, [_i] * 5 + [_vp] * 4 + [_vp]),
+    "gb_mesh_render_fwd": (_i, [_i] * 8 + [_vp] * 11 + [_vp]),
+    "gb_mesh_render_bwd_workspace_bytes": (_sz, [_i] * 6),
+    "gb_mesh_render_bwd": (_i, [_i] * 8 + [_vp] * 9 + [_i] + [_vp] * 5 + [_vp]),
 }
 
 

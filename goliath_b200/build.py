@@ -15,9 +15,10 @@ LIB = os.path.join(HERE, "libgoliath_b200.so")
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
-# per-file extra flags.  splat_project.cu carries the bit-exact binning contract: no FMA contraction.
+# per-file extra flags.  splat_project.cu carries the bit-exact binning contract, mesh_raster.cu the bit-exact index
+# image: no FMA contraction.
 # sg_shade.cu mirrors the reference extension's own flag (extensions/sgutils/setup.py:31) for last-bit parity.
-EXTRA = {"splat_project.cu": ["-fmad=false"], "sg_shade.cu": ["-use_fast_math"],
+EXTRA = {"splat_project.cu": ["-fmad=false"], "mesh_raster.cu": ["-fmad=false"], "sg_shade.cu": ["-use_fast_math"],
          "mvp_raymarch.cu": ["-use_fast_math"]}  # extensions/mvpraymarch/setup.py:31
 
 

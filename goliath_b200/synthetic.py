@@ -113,3 +113,53 @@ def mvp_scene(N: int = 2, side: int = 8, T=(4, 8, 8), img_h: int = 64, img_w: in
                focal=torch.full((N, 2), f), princpt=torch.tensor([[img_w / 2.0, img_h / 2.0]] * N),
                img_h=img_h, img_w=img_w, volradius=1.0)
     return out
+
+
+def body_mesh(n_faces: int, img_h: int = 2048, img_w: int = 1334, batch: int = 4, seed: int = SEED) -> Dict:
+    """A closed multi-part stand-in for the body template (its face count is not known here): 8 lat-long
+    ellipsoids over a 1.8 m tall box, about n_faces faces in all, UVs per vertex; and `batch` cameras 2.3-2.7 m in
+    front of it with the configuration's image size (fx = fy = 2000 * H / 2048).  Returns float32 verts [V,3],
+    int32 vi / vti [F,3], vt [V,2], K [B,3,3] and Rt [B,3,4]."""
+    g = torch.Generator().manual_seed(seed)
+    parts = 8
+    per = max(n_faces // parts, 8)
+    nlon = max(int(math.sqrt(per)), 4)
+    nlat = max(per // (2 * nlon) + 1, 3)
+    verts, vi, vt = [], [], []
+    for k in range(parts):
+        lat = torch.linspace(0, math.pi, nlat + 1, dtype=torch.float64)[1:-1]
+        lon = torch.arange(nlon, dtype=torch.float64) * (2 * math.pi / nlon)
+        ring = torch.stack([torch.sin(lat)[:, None] * torch.cos(lon), torch.cos(lat)[:, None].expand(-1, nlon),
+                            torch.sin(lat)[:, None] * torch.sin(lon)], -1).reshape(-1, 3)
+        pts = torch.cat([torch.tensor([[0.0, 1.0, 0.0]], dtype=torch.float64), ring,
+                         torch.tensor([[0.0, -1.0, 0.0]], dtype=torch.float64)])
+        radii = torch.tensor([0.10, 0.22, 0.10], dtype=torch.float64) * (0.7 + 0.6 * torch.rand(3, generator=g))
+        centre = torch.tensor([0.5 * (torch.rand(1, generator=g).item() - 0.5), 1.6 * (k + 0.5) / parts - 0.8,
+                               0.2 * (torch.rand(1, generator=g).item() - 0.5)], dtype=torch.float64)
+        uv = torch.cat([torch.tensor([[0.5, 0.0]], dtype=torch.float64),
+                        torch.stack([(lon / (2 * math.pi))[None].expand(nlat - 1, -1),
+                                     (lat / math.pi)[:, None].expand(-1, nlon)], -1).reshape(-1, 2),
+                        torch.tensor([[0.5, 1.0]], dtype=torch.float64)])
+        base = sum(v.shape[0] for v in verts)
+        f = []
+        for j in range(nlon):
+            j1 = (j + 1) % nlon
+            f.append((0, 1 + j1, 1 + j))
+            for r in range(nlat - 2):
+                a, b = 1 + r * nlon + j, 1 + r * nlon + j1
+                f += [(a, b, a + nlon), (b, b + nlon, a + nlon)]
+            last = 1 + (nlat - 2) * nlon
+            f.append((last + j, last + j1, last + nlon))
+        verts.append(pts * radii + centre)
+        vt.append(uv)
+        vi.append(torch.tensor(f, dtype=torch.int64) + base)
+    verts, vt, vi = torch.cat(verts).float(), torch.cat(vt).float(), torch.cat(vi).to(torch.int32)
+    f = 2000.0 * img_h / 2048.0
+    K = torch.tensor([[f, 0.0, img_w / 2.0], [0.0, f, img_h / 2.0], [0.0, 0.0, 1.0]]).expand(batch, 3, 3).clone()
+    Rt = torch.zeros(batch, 3, 4)
+    for b in range(batch):
+        yaw = 0.6 * (torch.rand(1, generator=g).item() - 0.5)
+        c, s = math.cos(yaw), math.sin(yaw)
+        Rt[b, :, :3] = torch.tensor([[c, 0.0, s], [0.0, 1.0, 0.0], [-s, 0.0, c]])
+        Rt[b, :, 3] = torch.tensor([0.0, 0.0, 2.3 + 0.4 * torch.rand(1, generator=g).item()])
+    return dict(verts=verts, vi=vi, vti=vi.clone(), vt=vt, K=K, Rt=Rt)

@@ -718,6 +718,41 @@ int gb_body_tex_compose_bwd(int B, int H, int W, const float* t1, const float* h
                             const float* g_out, float* g_t1, float* g_h, float* g_bias, float* g_w, float* g_s3,
                             float* workspace, void* stream);
 
+/* ---------------------------------------------------------------- body render (csrc/mesh_raster.cu)
+ * Conventions (DESIGN.md R9'', PARITY UNPINNED: drtk is outside the reference tree): pixel (x, y) samples the screen
+ * point (x + 0.5, y + 0.5); a face is drawn only if its three vertices have z > 0 (no near clipping, no backface
+ * culling) and its screen area is non-zero; the inside test is inclusive (every screen-space barycentric
+ * lambda_k >= 0) for either winding; perspective-correct barycentrics b_k = (lambda_k / z_k) / sum_j lambda_j / z_j
+ * and depth = 1 / sum_j lambda_j / z_j. */
+
+/* replaces drtk.rasterize(v_pix, vi, h, w) (ca_code/utils/render_drtk.py:47).  v_pix [B,V,3] (x, y in pixels, z =
+ * camera depth), vi [F,3] int32, index_img [B,H,W] int32 out (-1 = background).  Each pixel keeps the face with the
+ * smallest key (float_bits(depth) << 32) | face_id: the smaller depth, then the smaller face id, in any launch order.
+ * Faces with a pixel box over 256 samples are rasterised one CTA per face.  Bit-exact with oracle/mesh_oracle.c.
+ * `workspace`: gb_mesh_raster_workspace_bytes(B, F, H, W) bytes. */
+size_t gb_mesh_raster_workspace_bytes(int B, int F, int H, int W);
+int gb_mesh_raster(int B, int V, int F, int H, int W, const float* v_pix, const int32_t* vi, int32_t* index_img,
+                   void* workspace, void* stream);
+/* replaces drtk.render + drtk.interpolate of (2 vt - 1) + F.grid_sample(tex, vt_img, bilinear, align_corners=False,
+ * zero padding) * mask (render_drtk.py:48-63), one thread per pixel.  vti [F,3] int32, vt [Vt,2], tex [B,C,Ht,Wt];
+ * outputs depth_img [B,H,W] (0 on the background), bary_img [B,3,H,W], vt_img [B,2,H,W], mask [B,1,H,W] and render
+ * [B,C,H,W], each written once. */
+int gb_mesh_render_fwd(int B, int V, int F, int H, int W, int C, int Ht, int Wt, const float* v_pix, const int32_t* vi,
+                       const int32_t* vti, const float* vt, const float* tex, const int32_t* index_img,
+                       float* depth_img, float* bary_img, float* vt_img, float* mask, float* render, void* stream);
+/* replaces the autograd graph of render_drtk.py:45-73 from `render` to v_pix and tex, including
+ * drtk.edge_grad_estimator when edge_grad != 0 (the project's estimator, DESIGN.md R9'').  g_v_pix [B,V,3] and g_tex
+ * [B,C,Ht,Wt] are written, bitwise repeatable (no float atomics): per-pixel records stably sorted by face and by
+ * texel, fixed-order sums per face and per texel, and a vertex gather over the CSR list inc_ptr [V+1] / inc [3F]
+ * (entries 3 f + corner, grouped by vertex, ascending within a vertex) that the caller builds once per vi.
+ * `workspace`: gb_mesh_render_bwd_workspace_bytes(B, F, H, W, Ht, Wt) bytes. */
+size_t gb_mesh_render_bwd_workspace_bytes(int B, int F, int H, int W, int Ht, int Wt);
+int gb_mesh_render_bwd(int B, int V, int F, int H, int W, int C, int Ht, int Wt, const float* v_pix, const int32_t* vi,
+                       const int32_t* vti, const float* vt, const float* tex, const int32_t* index_img,
+                       const float* vt_img, const float* render, const float* g_render, int edge_grad,
+                       const int32_t* inc_ptr, const int32_t* inc, float* g_v_pix, float* g_tex, void* workspace,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif
