@@ -92,6 +92,7 @@ SIGNATURES = {
     "gb_lbs_skeleton_fwd": (_i, [_i] * 4 + [_vp, _vp, _i] + [_vp] * 7 + [_i] + [_vp] * 3 + [_vp]),
     "gb_lbs_skin_fwd": (_i, [_i] * 4 + [_vp] * 7 + [_vp]),
     "gb_lbs_skin_bwd": (_i, [_i] * 4 + [_vp] * 6 + [_vp]),
+    "gb_lbs_unskin_fwd": (_i, [_i] * 4 + [_vp] * 7 + [_vp]),
     "gb_sg_shade_compose_fwd":(_i, [_vp] * 10 + [_i] * 4 + [_vp]),
     "gb_sg_shade_compose_bwd": (_i, [_vp] * 16 + [_i] * 4 + [_vp]),
     "gb_render_finish_fwd": (_i, [_i, _i] + [_vp] * 5 + [_vp]),
@@ -136,6 +137,10 @@ SIGNATURES = {
     "gb_mesh_render_fwd": (_i, [_i] * 8 + [_vp] * 11 + [_vp]),
     "gb_mesh_render_bwd_workspace_bytes": (_sz, [_i] * 6),
     "gb_mesh_render_bwd": (_i, [_i] * 8 + [_vp] * 9 + [_i] + [_vp] * 5 + [_vp]),
+    "gb_downconv_block_fwd": (_i, [_i] * 6 + [_vp, _i64, _i64, _i, _i, _i, _vp, _f] + [_vp] * 9 + [_f] + [_vp] * 3 + [_vp]),
+    "gb_downconv_block_bwd_workspace_bytes": (_sz, [_i] * 6),
+    "gb_downconv_block_bwd": (_i, [_i] * 6 + [_vp, _i64, _i64, _i, _i, _i, _vp, _f] + [_vp] * 9 + [_f] + [_vp] * 10
+                              + [_vp]),
 }
 
 

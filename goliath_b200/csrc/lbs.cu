@@ -11,6 +11,8 @@
 //   2. skin: one thread per (item, vertex): out = gs * sum_k w_k M[idx_k] [v + template; 1], slots in order.
 //      Its backward sends the gradient to the vertices only and sums a batch-1 input over B inside the thread, in
 //      order, so the result is deterministic.
+//   3. unskin (LBSModule.unpose, lbs.py:273-306,733-739): one thread per (item, vertex) blends the same matrices,
+//      inverts the blended affine map in registers and applies it; no [B,V,4,4] temporary and no host loop.
 // Quaternions are (x, y, z, w), as ca_code/utils/quaternion.py:178-320 (batchMul, batchRot, batchInvert,
 // batchFromXYZ) stores them.
 #include "common.cuh"
@@ -190,6 +192,46 @@ __global__ void __launch_bounds__(kThreads) skin_bwd_kernel(SkinArgs a, const fl
   o[0] = s0; o[1] = s1; o[2] = s2;
 }
 
+// out = (sum_k w_k M[idx_k])^-1 [verts / gs; 1] - template.  The reference appends the row (0,0,0,1) to the blended
+// [3,4] matrix [A | t] and calls inverse() on the 4x4 (lbs.py:293-301); the inverse of such a matrix is
+// [A^-1 | -A^-1 t] over the same bottom row, so A^-1 (x - t) is the same result.  A^-1 = adj(A) / det(A).  A blend of
+// unrelated joint rotations can be close to singular and x - t cancels, so everything after the loads runs in double
+// (a few hundred operations per vertex).  det(A) == 0 gives NaN for that vertex (the reference's inverse() raises).
+__global__ void __launch_bounds__(kThreads) unskin_fwd_kernel(SkinArgs a, float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (i >= (long long)a.B * a.V) return;
+  const int v = (int)(i % a.V), b = (int)(i / a.V);
+  const float* x = a.verts + ((size_t)(a.vb == 1 ? 0 : b) * a.V + v) * 3;
+  double x0 = x[0], x1 = x[1], x2 = x[2];
+  if (a.gs) { x0 /= (double)a.gs[0]; x1 /= (double)a.gs[1]; x2 /= (double)a.gs[2]; }
+  double m[12];
+#pragma unroll
+  for (int c = 0; c < 12; ++c) m[c] = 0.0;
+#pragma unroll
+  for (int k = 0; k < kSlots; ++k) {
+    const double wk = a.w[(size_t)v * kSlots + k];
+    const float* mk = a.mats + ((size_t)b * a.J + a.idx[(size_t)v * kSlots + k]) * 12;
+#pragma unroll
+    for (int c = 0; c < 12; ++c) m[c] += wk * (double)mk[c];
+  }
+  const double c00 = m[5] * m[10] - m[6] * m[9], c01 = m[6] * m[8] - m[4] * m[10], c02 = m[4] * m[9] - m[5] * m[8];
+  const double det = m[0] * c00 + m[1] * c01 + m[2] * c02;
+  const double d0 = x0 - m[3], d1 = x1 - m[7], d2 = x2 - m[11];
+  float o0, o1, o2;
+  if (det == 0.0) {
+    o0 = o1 = o2 = __int_as_float(0x7fc00000);
+  } else {
+    const double r = 1.0 / det;
+    double u0 = r * (c00 * d0 + (m[2] * m[9] - m[1] * m[10]) * d1 + (m[1] * m[6] - m[2] * m[5]) * d2);
+    double u1 = r * (c01 * d0 + (m[0] * m[10] - m[2] * m[8]) * d1 + (m[2] * m[4] - m[0] * m[6]) * d2);
+    double u2 = r * (c02 * d0 + (m[1] * m[8] - m[0] * m[9]) * d1 + (m[0] * m[5] - m[1] * m[4]) * d2);
+    if (a.templ) { u0 -= (double)a.templ[3 * v]; u1 -= (double)a.templ[3 * v + 1]; u2 -= (double)a.templ[3 * v + 2]; }
+    o0 = (float)u0; o1 = (float)u1; o2 = (float)u2;
+  }
+  float* o = out + (size_t)i * 3;
+  o[0] = o0; o[1] = o1; o[2] = o2;
+}
+
 }  // namespace
 
 GB_API int gb_lbs_max_joints(void) { return kMaxJoints; }
@@ -229,6 +271,18 @@ GB_API int gb_lbs_skin_bwd(int B, int V, int J, int vb, const float* mats, const
   SkinArgs a{B, V, J, vb, mats, nullptr, nullptr, skin_weights, global_scaling, skin_indices};
   skin_bwd_kernel<<<(unsigned)gb::cdiv64((long long)vb * V, kThreads), kThreads, 0, (cudaStream_t)stream>>>(a, g_out,
                                                                                                            g_verts);
+  gb::count_launches(1);
+  GB_CHECK_LAUNCH();
+  return 0;
+}
+
+GB_API int gb_lbs_unskin_fwd(int B, int V, int J, int vb, const float* mats, const float* verts, const float* templ,
+                             const int32_t* skin_indices, const float* skin_weights, const float* global_scaling,
+                             float* out, void* stream) {
+  if (B <= 0 || V <= 0) return 0;
+  if (J <= 0 || (vb != 1 && vb != B)) return (int)cudaErrorInvalidValue;
+  SkinArgs a{B, V, J, vb, mats, verts, templ, skin_weights, global_scaling, skin_indices};
+  unskin_fwd_kernel<<<(unsigned)gb::cdiv64((long long)B * V, kThreads), kThreads, 0, (cudaStream_t)stream>>>(a, out);
   gb::count_launches(1);
   GB_CHECK_LAUNCH();
   return 0;

@@ -3,7 +3,8 @@
 dtypes), so a checkpoint holding the reference's `lbs_fn.*` buffers loads with strict=True.
 
 The posing runs on csrc/lbs.cu: one launch computes the parameter transform, the joint chain (level by level of the
-skeleton tree) and the skinning matrices, a second one skins the vertices.  Gradients flow to the vertices only;
+skeleton tree) and the skinning matrices, a second one skins the vertices, or, for `unpose`, applies the inverse of
+each vertex's blended matrix (forward only).  Gradients flow to the vertices only;
 pose and scale gradients are not implemented, so a `motion` / `scales` that requires grad is refused.  The bind state
 is computed once on the host at construction, as the reference does."""
 from typing import Any, Dict, Optional
@@ -266,6 +267,31 @@ class LinearBlendSkinning(nn.Module):
         tabs = self._kernel_tables()
         return _Skin.apply(verts, mats, template, tabs["skin_idx"], tabs["skin_w"], global_scaling)
 
+    def unskin(self, mats, verts, template=None, global_scaling=None):
+        """The inverse of `skin`: (blended matrix)^-1 [verts / global_scaling; 1] - template, one launch (lbs.py:273-306
+        with the scaling and template of lbs.py:733-739).  verts [1 or B, V, 3]; a vertex whose blended matrix is
+        singular comes back NaN.  Forward only: a `verts` that requires grad is refused."""
+        if torch.is_grad_enabled() and verts.requires_grad:
+            raise RuntimeError("verts requires grad, but the unskinning kernel has no backward (call it under no_grad)")
+        tabs = self._kernel_tables()
+        verts = verts.contiguous()
+        _lib.check_input(verts, "verts")
+        B, J = mats.shape[0], mats.shape[1]
+        vb, V = tuple(verts.shape[:2]) if verts.dim() == 3 else (0, 0)
+        if verts.shape[2:] != (3,) or vb not in (1, B) or tabs["skin_idx"].shape != (V, N_SLOTS):
+            raise RuntimeError("verts must be [1 or B, V, 3] with V = the skinned mesh's vertex count")
+        out = torch.empty(B, V, 3, device=verts.device)
+        with torch.cuda.device(verts.device):
+            _lib.check(_lib.lib().gb_lbs_unskin_fwd(
+                B, V, J, vb, _lib.ptr(mats), _lib.ptr(verts), _lib.ptr(template), _lib.ptr(tabs["skin_idx"]),
+                _lib.ptr(tabs["skin_w"]), _lib.ptr(global_scaling), _lib.ptr(out), _lib.stream_ptr(verts.device)),
+                "lbs_unskin_fwd")
+        return out
+
+    def unpose(self, poses: torch.Tensor, scales: torch.Tensor, verts: torch.Tensor):
+        """lbs.py:256-271: poses [B,P], scales [B,S], posed verts [B,V,3] -> unposed verts [B,V,3]."""
+        return self.unskin(self.skeleton(poses, scales), verts)
+
     def forward(self, poses: torch.Tensor, scales: torch.Tensor, verts_unposed: Optional[torch.Tensor] = None):
         """lbs.py:308-337: poses [B,P], scales [B,S], verts_unposed [1 or B, V, 3] (default: the rest mesh) -> [B,V,3]."""
         if verts_unposed is None:
@@ -305,6 +331,13 @@ class LBSModule(nn.Module):
         if tpl is None:
             verts_unposed, tpl = verts_unposed + template, None
         return self.lbs_fn.skin(mats, verts_unposed, tpl, self._gscale())
+
+    def unpose(self, verts: torch.Tensor, motion: torch.Tensor):
+        """lbs_fn.unpose(motion, lbs_scale, verts / global_scaling) - lbs_template_verts  (lbs.py:733-739)."""
+        mats = self.lbs_fn.skeleton(motion, self.lbs_scale.reshape(1, -1).expand(motion.shape[0], -1))
+        tpl = self._template(self.lbs_template_verts, verts.shape[-2])
+        out = self.lbs_fn.unskin(mats, verts, tpl, self._gscale())
+        return out if tpl is not None else out - self.lbs_template_verts
 
     def template_pose(self, motion: torch.Tensor):
         """global_scaling * lbs_fn(motion, lbs_scale, lbs_template_verts)  (lbs.py:741-745)."""

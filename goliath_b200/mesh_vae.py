@@ -8,15 +8,20 @@ convolutions read their halves of the 8-channel map in place), the seam sampler 
 Constructor, parameter names and shapes, buffers and the Glorot initialisation are the reference's, so a checkpoint of
 the reference class loads with strict=True.  `geo_fn` and `seam_sampler` are duck-typed as in the reference: any object
 with `from_uv`, and `impaint` / `resample`.  The small pieces stay in torch: the LinearWN layers, tile2d x mask, the
-face / body merge and the concatenations.  Forward and backward are free of host synchronisation; CPU tensors raise."""
+face / body merge and the concatenations.  Forward and backward are free of host synchronisation; CPU tensors raise.
+
+The encoders `mesh_vae.Encoder` / `FaceEncoder` (mesh_vae.py:344-436) run on the fused `ConvDownBlock` kernels of
+csrc/downconv_wnub.cu, the first block building its resized, masked input inside its kernels; `encode` is
+`AutoEncoder.encode` (mesh_vae.py:230-239) as a function over the LBS module, the geometry module and the encoders."""
 import numpy as np
 import torch
 import torch.nn as tnn
+import torch.nn.functional as F
 from torch.autograd import Function
 
 from . import _lib
-from .nn import (ConvBlock, Conv2dWNUB, FusedLeakyReLU, LinearWN, UpConvBlockDeep, _wn_chain, _wn_scale, glorot,
-                 tile2d)
+from .nn import (ConvBlock, ConvDownBlock, Conv2dWNUB, FusedLeakyReLU, LinearWN, UpConvBlockDeep, _wn_chain,
+                 _wn_scale, glorot, tile2d)
 from .seams import SeamSampler
 from .unet import UNetWB
 
@@ -288,3 +293,74 @@ class TextureComposer(tnn.Module):
         ob = self.upscale_net.out_block
         p = _TexCompose.apply(t1, h, ob.weight_v, ob.weight_g, ob.bias, self.tex_mean, s3, self.tex_std)
         return self.seam_sampler_2k.resample(self.seam_sampler_2k(p))
+
+
+class Encoder(tnn.Module):
+    """mesh_vae.py:344-421: seven ConvDownBlocks (3 -> 8 @ 512 ... 128 -> 128 @ 8) and two LinearWN heads.  The input
+    conditioning `verts_scale * bilinear(verts_unposed_uv -> 512^2) * mask` (align_corners=False) is evaluated inside
+    the first block's kernels, for any input size and for a strided window of a larger map, so neither the resized map
+    nor a crop is written.  `encode` computes verts_unposed_uv under no_grad, so no gradient flows to it: an input
+    that requires grad is refused.  The reparameterisation noise is torch's randn_like, drawn as the reference
+    draws it."""
+
+    def __init__(self, n_embs: int, mask, noise_std: float = 1.0, mean_scale: float = 0.1, logvar_scale: float = 0.1,
+                 verts_scale: float = 1.0):
+        super().__init__()
+        self.noise_std, self.n_embs = noise_std, n_embs
+        self.mean_scale, self.logvar_scale, self.verts_scale = mean_scale, logvar_scale, verts_scale
+        self.verts_conv = ConvDownBlock(3, 8, 512)
+        if len(mask.shape) != 2:
+            raise ValueError("mask must be [H, W] (got %s)" % (tuple(mask.shape),))
+        mask = torch.as_tensor(mask[np.newaxis, np.newaxis], dtype=torch.float32)
+        self.register_buffer("mask", F.interpolate(mask, size=(512, 512), mode="bilinear").to(torch.bool))
+        self.joint_conv_blocks = tnn.Sequential(ConvDownBlock(8, 16, 256), ConvDownBlock(16, 32, 128),
+                                                ConvDownBlock(32, 32, 64), ConvDownBlock(32, 64, 32),
+                                                ConvDownBlock(64, 128, 16), ConvDownBlock(128, 128, 8))
+        self.mu = LinearWN(4 * 4 * 128, n_embs)
+        self.logvar = LinearWN(4 * 4 * 128, n_embs)
+        self.apply(lambda m: glorot(m, 0.2))
+        glorot(self.mu, 1.0)
+        glorot(self.logvar, 1.0)
+
+    def forward(self, verts_unposed_uv):
+        if not verts_unposed_uv.is_cuda:
+            raise RuntimeError("Encoder runs on CUDA only (no CPU fallback): verts_unposed_uv is on %s"
+                               % verts_unposed_uv.device)
+        if verts_unposed_uv.dim() != 4 or verts_unposed_uv.shape[1] != 3:
+            raise RuntimeError("verts_unposed_uv must be [B, 3, H, W] (got %s)" % (tuple(verts_unposed_uv.shape),))
+        B = verts_unposed_uv.shape[0]
+        x = self.verts_conv(verts_unposed_uv, resize_mask=self.mask, scale=self.verts_scale)
+        x = self.joint_conv_blocks(x).reshape(B, -1)
+        embs_mu = self.mean_scale * self.mu(x)
+        embs_logvar = self.logvar_scale * self.logvar(x)
+        if self.training:
+            embs = embs_mu + torch.exp(embs_logvar) * torch.randn_like(embs_mu) * self.noise_std
+        else:
+            embs = embs_mu.clone()
+        return {"embs": embs, "embs_mu": embs_mu, "embs_logvar": embs_logvar}
+
+
+class FaceEncoder(tnn.Module):
+    """mesh_vae.py:424-436: an `Encoder` on the [512:, :512] window of the UV position map, read in place."""
+
+    def __init__(self, mask, **kwargs):
+        super().__init__()
+        if len(mask.shape) != 2 or mask.shape[0] <= 512:
+            raise ValueError("mask must be [H, W] with H > 512 (got %s)" % (tuple(mask.shape),))
+        self.encoder = Encoder(**kwargs, mask=mask[512:, :512])
+
+    def forward(self, verts_unposed_uv):
+        if verts_unposed_uv.dim() != 4 or verts_unposed_uv.shape[2] <= 512:
+            raise RuntimeError("verts_unposed_uv must be [B, 3, H, W] with H > 512 (got %s)"
+                               % (tuple(verts_unposed_uv.shape),))
+        preds = self.encoder(verts_unposed_uv[:, :, 512:, :512])
+        return {"face_" + k: v for k, v in preds.items()}
+
+
+def encode(lbs_fn, geo_fn, encoder, encoder_face, registration_vertices, pose):
+    """mesh_vae.AutoEncoder.encode (mesh_vae.py:230-239): unpose the registered vertices and lay them out in UV under
+    no_grad, then both encoders; returns the merged dict (embs*, face_embs*).  One stream, no host synchronisation."""
+    with torch.no_grad():
+        verts_unposed = lbs_fn.unpose(registration_vertices, pose)
+        verts_unposed_uv = geo_fn.to_uv(verts_unposed)
+    return {**encoder(verts_unposed_uv), **encoder_face(verts_unposed_uv)}

@@ -7,7 +7,10 @@ The stride-2 4x4 transposed convolution + untied bias + LeakyReLU runs as ONE ha
 forward, and its backward as three more (activation/bias gradient, data gradient, weight gradient) — no cuDNN
 (csrc/deconv_wnub.cu).  The stride-2 4x4 convolution of the RGCA encoder (`Conv2dWNUB(.., 4, 2, 1)`) runs on the same
 kernels with the two sides of the layer exchanged.  Round-1 status: fp32 SIMT kernels; LinearWN is a plain library
-GEMM (cuBLAS via F.linear)."""
+GEMM (cuBLAS via F.linear).
+
+The body model's residual blocks run as fused blocks instead of layer by layer: `UpConvBlockDeep` (decoder,
+csrc/upconv_wnub.cu) and `ConvDownBlock` (encoders, csrc/downconv_wnub.cu)."""
 import math
 from typing import Optional
 
@@ -565,3 +568,131 @@ class UpConvBlockDeep(nn.Module):
         c1, c2, cr = self.conv1, self.conv2, self.conv_resize
         return _UpConvBlock.apply(x, c1.weight_v, c1.weight_g, c1.bias, c2.weight_v, c2.weight_g, c2.bias,
                                   cr.weight_v, cr.weight_g, cr.bias, self.lrelu_slope, self.groups)
+
+
+class _DownConvBlock(Function):
+    """ConvDownBlock forward / backward on csrc/downconv_wnub.cu (two kernels forward, ten or eleven backward).  With
+    `cond_mask` the block's input is cond_scale * bilinear(x -> mask's size) * cond_mask, built inside the kernels."""
+
+    @staticmethod
+    def forward(ctx, x, v1, g1, b1, v2, g2, b2, vr, gr, br, slope, groups, cond_mask, cond_scale):
+        if x.dim() != 4 or not x.is_cuda or x.dtype != torch.float32:
+            raise RuntimeError("input must be a float32 CUDA tensor [B, C, H, W]")
+        if cond_mask is None or x.stride(3) != 1 or min(x.stride()) < 1:
+            x = x.contiguous()  # a window of a larger map is read in place only by the fused resize
+        for t, n in ((v1, "conv1.weight_v"), (v2, "conv2.weight_v"), (vr, "conv_resize.weight_v"),
+                     (b1, "conv1.bias"), (b2, "conv2.bias"), (br, "conv_resize.bias")):
+            _lib.check_input(t, n)
+        B, Cin, Hs, Ws = x.shape
+        Cout = v2.shape[0]
+        if cond_mask is None:
+            H, W = Hs, Ws
+        else:
+            _lib.check_input(cond_mask, "mask", torch.bool)
+            H, W = cond_mask.shape[-2:]
+            if cond_mask.numel() != H * W:
+                raise RuntimeError("mask must hold one [H, W] plane")
+        if (H % 2 or W % 2 or v1.shape != (Cin, Cin // groups, 3, 3) or v2.shape != (Cout, Cin // groups, 3, 3)
+                or vr.shape != (Cout, Cin // groups, 1, 1) or b1.shape != (Cin, H, W)
+                or b2.shape != (Cout, H // 2, W // 2) or br.shape != (Cout,)):
+            raise RuntimeError("ConvDownBlock: parameter shapes do not match an input of %s" % (tuple(x.shape),))
+        s1, s2, sr = _wn_scale(v1, g1), _wn_scale(v2, g2), _wn_scale(vr, gr)
+        dev = x.device
+        h1 = torch.empty(B, Cin, H, W, device=dev)
+        out = torch.empty(B, Cout, H // 2, W // 2, device=dev)
+        train = any(ctx.needs_input_grad)
+        mask = torch.empty(B, Cout, H // 2, W // 2, device=dev, dtype=torch.uint8) if train else None
+        ctx.xargs = (B, Cin, Cout, groups, H, W)
+        ctx.cond = (x.stride(0), x.stride(1), x.stride(2), Hs, Ws)
+        ctx.cond_scale = float(cond_scale)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().gb_downconv_block_fwd(
+                *ctx.xargs, _lib.ptr(x), *ctx.cond, _lib.ptr(cond_mask), ctx.cond_scale, _lib.ptr(v1), _lib.ptr(s1),
+                _lib.ptr(b1), _lib.ptr(v2), _lib.ptr(s2), _lib.ptr(b2), _lib.ptr(vr), _lib.ptr(sr), _lib.ptr(br),
+                float(slope), _lib.ptr(h1), _lib.ptr(out), _lib.ptr(mask), _lib.stream_ptr(dev)), "downconv_block_fwd")
+        if train:
+            ctx.save_for_backward(x, v1, g1, v2, g2, vr, gr, h1, mask, cond_mask)
+        ctx.slope = float(slope)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, v1, g1, v2, g2, vr, gr, h1, mask, cond_mask = ctx.saved_tensors
+        B, Cin, Cout, groups, H, W = ctx.xargs
+        dev = x.device
+        gout = gout.contiguous()
+        s1, s2, sr = _wn_scale(v1, g1), _wn_scale(v2, g2), _wn_scale(vr, gr)
+        need_gx = ctx.needs_input_grad[0]
+        if need_gx and cond_mask is not None:
+            raise RuntimeError("ConvDownBlock: the fused resize + mask of the input has no backward")
+        L = _lib.lib()
+        gz2 = torch.empty(B, Cout, H // 2, W // 2, device=dev)
+        gz1 = torch.empty(B, Cin, H, W, device=dev)
+        gx = torch.empty(B, Cin, H, W, device=dev) if need_gx else None
+        gb1 = torch.empty(Cin, H, W, device=dev)
+        gb2 = torch.empty(Cout, H // 2, W // 2, device=dev)
+        gbr = torch.empty(Cout, device=dev)
+        gw1, gw2, gwr = torch.empty_like(v1), torch.empty_like(v2), torch.empty_like(vr)
+        ws = torch.empty(L.gb_downconv_block_bwd_workspace_bytes(*ctx.xargs) // 4, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(L.gb_downconv_block_bwd(
+                *ctx.xargs, _lib.ptr(x), *ctx.cond, _lib.ptr(cond_mask), ctx.cond_scale, _lib.ptr(v1), _lib.ptr(s1),
+                _lib.ptr(v2), _lib.ptr(s2), _lib.ptr(vr), _lib.ptr(sr), _lib.ptr(h1), _lib.ptr(mask), _lib.ptr(gout),
+                ctx.slope, _lib.ptr(gz2), _lib.ptr(gz1), _lib.ptr(gb1), _lib.ptr(gb2), _lib.ptr(gbr), _lib.ptr(gw1),
+                _lib.ptr(gw2), _lib.ptr(gwr), _lib.ptr(gx), _lib.ptr(ws), _lib.stream_ptr(dev)), "downconv_block_bwd")
+        gv1, gg1 = _wn_chain(v1, g1, gw1)
+        gv2, gg2 = _wn_chain(v2, g2, gw2)
+        gvr, ggr = _wn_chain(vr, gr, gwr)
+        return gx, gv1, gg1, gb1, gv2, gg2, gb2, gvr, ggr, gbr, None, None, None, None
+
+
+def _block_only(*args, **kwargs):
+    raise NotImplementedError("a stride-2 layer of ConvDownBlock runs inside the block's kernels only")
+
+
+def _strided(m):
+    """mark a weight-norm conv as a stride-2 layer of ConvDownBlock: a holder of the reference's parameters"""
+    m.stride = (2, 2)
+    m.forward = _block_only
+    return m
+
+
+class ConvDownBlock(nn.Module):
+    """blocks.py:327-379: grouped weight-normalised 1x1 stride-2 skip with tied bias, 3x3 Conv2dWNUB + LeakyReLU at the
+    input size, 3x3 stride-2 Conv2dWNUB + LeakyReLU; the whole block runs on the two fused kernels of
+    csrc/downconv_wnub.cu, and `lrelu1` / `lrelu2` are parameter-free placeholders.  `size` is the INPUT size; the
+    output is [B, Cout, size/2, size/2].  Parameter names and shapes are the reference's.
+
+    forward(x, resize_mask=None, scale=1.0): with a bool `resize_mask` [.., size, size] the block's input is
+    scale * bilinear(x -> size x size, align_corners=False) * resize_mask, computed inside the kernels from x
+    [B, Cin, Hs, Ws], which may be a strided window of a larger map (unit stride along a row); that input is never
+    written, and no gradient reaches x through it (asking for one raises)."""
+
+    def __init__(self, in_channels, out_channels, size, lrelu_slope=0.2, groups=1, wnorm_dim=0):
+        super().__init__()
+        if wnorm_dim != 0:
+            raise NotImplementedError("only wnorm_dim = 0 (g per output channel) is supported")
+        if in_channels % groups or out_channels % groups or size % 2:
+            raise ValueError("channels must divide into groups and size must be even")
+        self.size, self.groups, self.lrelu_slope = size, groups, float(lrelu_slope)
+        self.conv_resize = _strided(_grouped(Conv2dWN(in_channels, out_channels, kernel_size=1), groups))
+        self.conv1 = _grouped(Conv2dWNUB(in_channels, in_channels, size, size, 3, 1, 1), groups)
+        self.lrelu1 = FusedLeakyReLU()
+        self.conv2 = _strided(_grouped(Conv2dWNUB(in_channels, out_channels, size // 2, size // 2, 3, 1, 1), groups))
+        self.lrelu2 = FusedLeakyReLU()
+
+    def forward(self, x, resize_mask=None, scale: float = 1.0):
+        if resize_mask is None:
+            if x.dim() != 4 or tuple(x.shape[2:]) != (self.size, self.size):
+                raise RuntimeError("ConvDownBlock(size=%d) needs a [B, C, %d, %d] input (got %s)"
+                                   % (self.size, self.size, self.size, tuple(x.shape)))
+        else:
+            if resize_mask.dtype != torch.bool or tuple(resize_mask.shape[-2:]) != (self.size, self.size):
+                raise RuntimeError("resize_mask must be a bool [.., %d, %d] tensor" % (self.size, self.size))
+            if torch.is_grad_enabled() and x.requires_grad:
+                raise RuntimeError("ConvDownBlock: the fused resize + mask of the input has no backward, and the input "
+                                   "requires grad")
+        c1, c2, cr = self.conv1, self.conv2, self.conv_resize
+        return _DownConvBlock.apply(x, c1.weight_v, c1.weight_g, c1.bias, c2.weight_v, c2.weight_g, c2.bias,
+                                    cr.weight_v, cr.weight_g, cr.bias, self.lrelu_slope, self.groups, resize_mask,
+                                    scale)

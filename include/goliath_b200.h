@@ -620,6 +620,16 @@ int gb_lbs_skin_bwd(int B, int V, int J, int vb, const float* mats, const int32_
                     const float* skin_weights, const float* global_scaling, const float* g_out, float* g_verts,
                     void* stream);
 
+/* replaces LinearBlendSkinning.unskinning (lbs.py:273-306: a [B,V,4,4] blended matrix and inverse() in a Python loop
+ * over the batch) and the scaling / template of LBSModule.unpose (lbs.py:733-739):
+ *   out [B,V,3] = (sum_{k<8} w_k mats[b, idx_k])^-1 [verts / gs; 1] - templ.
+ * The blended [3,4] matrix [A | t] is inverted as an affine map in registers (adjugate / determinant in double, then
+ * A^-1 (x - t)); the reference's fourth row is (0,0,0,1), so this is its 4x4 inverse.  det(A) == 0 writes NaN for that
+ * vertex.  Arguments as gb_lbs_skin_fwd; forward only. */
+int gb_lbs_unskin_fwd(int B, int V, int J, int vb, const float* mats, const float* verts, const float* templ,
+                      const int32_t* skin_indices, const float* skin_weights, const float* global_scaling, float* out,
+                      void* stream);
+
 /* ---------------------------------------------------------------- relightable hand teacher (row R8'') */
 
 /* replaces the deep shadow march of OLATRGBDecoder.forward_rgb (hand_teacher_mvp.py:274-358: the expanded [B*L, K,
@@ -752,6 +762,36 @@ int gb_mesh_render_bwd(int B, int V, int F, int H, int W, int C, int Ht, int Wt,
                        const float* vt_img, const float* render, const float* g_render, int edge_grad,
                        const int32_t* inc_ptr, const int32_t* inc, float* g_v_pix, float* g_tex, void* workspace,
                        void* stream);
+
+/* ---------------------------------------------------------------- body encoders (row R9''', csrc/downconv_wnub.cu) */
+
+/* replaces blocks.ConvDownBlock.forward (ca_code/nn/blocks.py:327-379): conv1 3x3 stride 1 and conv2 3x3 stride 2
+ * pad 1 (la.Conv2dUB, untied biases [Cin,H,W] and [Cout,H/2,W/2]), both LeakyReLUs and the weight-normalised grouped
+ * conv_resize 1x1 stride 2 (tied bias), in two kernels; the skip is never written.  H and W (the input size) are even.
+ * x is read through element strides x_bs (item), x_cs (channel), x_rs (row), unit along a row.  With cond_mask == NULL
+ * x is [B,Cin,H,W] (Hs = H, Ws = W).  With cond_mask [H,W] uint8 the block's input is
+ *   cond_scale * bilinear(x [B,Cin,Hs,Ws] -> H x W, align_corners = False) * cond_mask
+ * evaluated while tiles are staged (replaces mesh_vae.py:394-399, and the crop of mesh_vae.py:434 through the strides).
+ * v1 [Cin,Cin/G,3,3], v2 [Cout,Cin/G,3,3], vr [Cout,Cin/G]; s1 / s2 / sr = weight_g / ||weight_v||_F per output
+ * channel; b1 [Cin,H,W], b2 [Cout,H/2,W/2], br [Cout].  h1 [B,Cin,H,W] (conv1's activation, kept for the backward),
+ * out [B,Cout,H/2,W/2]; mask [B,Cout,H/2,W/2] uint8 = conv2's pre-activation > 0, or NULL when no backward follows. */
+int gb_downconv_block_fwd(int B, int Cin, int Cout, int groups, int H, int W, const float* x, long long x_bs,
+                          long long x_cs, int x_rs, int Hs, int Ws, const unsigned char* cond_mask, float cond_scale,
+                          const float* v1, const float* s1, const float* b1, const float* v2, const float* s2,
+                          const float* b2, const float* vr, const float* sr, const float* br, float slope, float* h1,
+                          float* out, unsigned char* mask, void* stream);
+/* backward of the above (replaces the autograd graph of the same lines).  Scratch gz2 [B,Cout,H/2,W/2] and gz1
+ * [B,Cin,H,W]; gb1 [Cin,H,W], gb2 [Cout,H/2,W/2], gbr [Cout] and the effective-weight gradients at unit scale gw1, gw2,
+ * gwr are all WRITTEN.  gx [B,Cin,H,W] or NULL (it must be NULL with cond_mask: the resize has no backward).  Every sum
+ * runs in a fixed order (no float atomics), so the gradients are bitwise repeatable.
+ * `workspace`: gb_downconv_block_bwd_workspace_bytes(B, Cin, Cout, groups, H, W) bytes. */
+size_t gb_downconv_block_bwd_workspace_bytes(int B, int Cin, int Cout, int groups, int H, int W);
+int gb_downconv_block_bwd(int B, int Cin, int Cout, int groups, int H, int W, const float* x, long long x_bs,
+                          long long x_cs, int x_rs, int Hs, int Ws, const unsigned char* cond_mask, float cond_scale,
+                          const float* v1, const float* s1, const float* v2, const float* s2, const float* vr,
+                          const float* sr, const float* h1, const unsigned char* mask, const float* gout, float slope,
+                          float* gz2, float* gz1, float* gb1, float* gb2, float* gbr, float* gw1, float* gw2,
+                          float* gwr, float* gx, void* workspace, void* stream);
 
 #ifdef __cplusplus
 }
