@@ -141,6 +141,9 @@ SIGNATURES = {
     "gb_downconv_block_bwd_workspace_bytes": (_sz, [_i] * 6),
     "gb_downconv_block_bwd": (_i, [_i] * 6 + [_vp, _i64, _i64, _i, _i, _i, _vp, _f] + [_vp] * 9 + [_f] + [_vp] * 10
                               + [_vp]),
+    "gb_depth_disc_mask": (_i, [_i] * 3 + [_vp, _f, _vp, _vp]),
+    "gb_pixel_bias_fwd": (_i, [_i] * 7 + [_vp] * 4 + [_vp]),
+    "gb_pixel_bias_bwd": (_i, [_i] * 7 + [_vp] * 3 + [_vp]),
 }
 
 

@@ -113,16 +113,25 @@ def sample_uv(values_uv: torch.Tensor, uv_coords: torch.Tensor, v2uv=None) -> to
 class GeometryModule(torch.nn.Module):
     """The part of the reference's GeometryModule (geom.py:186-278) the decoders use: `vn(verts)`, `to_uv(values)` and,
     given vt [N_uv,2] and v2uv [V,n_max], `from_uv(values_uv)`.  vi [F,3]; index_image / bary_image [U,U,3] are the
-    reference's precomputed assets."""
+    reference's precomputed assets.  vti [F,3], face_index_image [U,U] and valid_mask [U,U,1] are registered only when
+    given, so a full module holds the reference's eight buffers (a checkpoint's `geo_fn.*` keys load strictly) and
+    the smaller holders keep their keys."""
 
-    def __init__(self, vi: torch.Tensor, index_image: torch.Tensor, bary_image: torch.Tensor, vt=None, v2uv=None):
+    def __init__(self, vi: torch.Tensor, index_image: torch.Tensor, bary_image: torch.Tensor, vt=None, v2uv=None,
+                 vti=None, face_index_image=None, valid_mask=None):
         super().__init__()
-        self.register_buffer("vi", vi.to(torch.int32))
-        self.register_buffer("index_image", index_image.to(torch.int32))
-        self.register_buffer("bary_image", bary_image.to(torch.float32))
+        self.register_buffer("vi", torch.as_tensor(vi).to(torch.int32))
+        self.register_buffer("index_image", torch.as_tensor(index_image).to(torch.int32))
+        self.register_buffer("bary_image", torch.as_tensor(bary_image).to(torch.float32))
         if vt is not None:
             self.register_buffer("vt", torch.as_tensor(vt).to(torch.float32))
             self.register_buffer("v2uv", torch.as_tensor(v2uv).to(torch.int32))
+        if vti is not None:
+            self.register_buffer("vti", torch.as_tensor(vti).to(torch.int32))
+        if face_index_image is not None:
+            self.register_buffer("face_index_image", torch.as_tensor(face_index_image).to(torch.int32))
+        if valid_mask is not None:
+            self.register_buffer("valid_mask", torch.as_tensor(valid_mask).to(torch.bool))
         self._uv_table, self._uv_key = None, None
 
     def from_uv(self, values_uv):
@@ -141,3 +150,23 @@ class GeometryModule(torch.nn.Module):
 
     def to_uv(self, values):
         return values_to_uv(values, self.index_image, self.bary_image)
+
+
+def depth_discontuity_mask(depth: torch.Tensor, threshold: float = 40.0, kscale: float = 4.0,
+                           pool_ksize: int = 3) -> torch.Tensor:
+    """geom.py:768-794 (the reference's name) on one kernel (csrc/body_frame.cu): depth [B,1,H,W] -> torch.bool
+    [B,1,H,W], true where a pixel within the 3x3 neighbourhood inside the image has a Sobel gradient norm (zero
+    padding) above `threshold`.  `kscale` is unused, as in the reference; only pool_ksize 3 is implemented.  No
+    gradient (the reference runs it under no_grad)."""
+    if pool_ksize != 3:
+        raise ValueError("depth_discontuity_mask: only pool_ksize = 3 is implemented (got %d)" % pool_ksize)
+    depth = depth.detach().contiguous()
+    _lib.check_input(depth, "depth")
+    if depth.dim() != 4 or depth.shape[1] != 1:
+        raise RuntimeError("depth_discontuity_mask: depth must be [B,1,H,W] (got %s)" % (tuple(depth.shape),))
+    B, _, H, W = depth.shape
+    mask = torch.empty(B, 1, H, W, device=depth.device, dtype=torch.bool)
+    with torch.cuda.device(depth.device):
+        _lib.check(_lib.lib().gb_depth_disc_mask(B, H, W, _lib.ptr(depth), float(threshold), _lib.ptr(mask),
+                                                 _lib.stream_ptr(depth.device)), "depth_disc_mask")
+    return mask

@@ -12,7 +12,10 @@ face / body merge and the concatenations.  Forward and backward are free of host
 
 The encoders `mesh_vae.Encoder` / `FaceEncoder` (mesh_vae.py:344-436) run on the fused `ConvDownBlock` kernels of
 csrc/downconv_wnub.cu, the first block building its resized, masked input inside its kernels; `encode` is
-`AutoEncoder.encode` (mesh_vae.py:230-239) as a function over the LBS module, the geometry module and the encoders."""
+`AutoEncoder.encode` (mesh_vae.py:230-239) as a function over the LBS module, the geometry module and the encoders.
+
+`AutoEncoder` (mesh_vae.py:72-341) runs the whole frame on these stages with the reference's constructor and keys, and
+finishes the render with the depth-discontinuity mask and `CameraPixelBias` on csrc/body_frame.cu."""
 import numpy as np
 import torch
 import torch.nn as tnn
@@ -20,6 +23,7 @@ import torch.nn.functional as F
 from torch.autograd import Function
 
 from . import _lib
+from .geom import depth_discontuity_mask
 from .nn import (ConvBlock, ConvDownBlock, Conv2dWNUB, FusedLeakyReLU, LinearWN, UpConvBlockDeep, _wn_chain,
                  _wn_scale, glorot, tile2d)
 from .seams import SeamSampler
@@ -364,3 +368,217 @@ def encode(lbs_fn, geo_fn, encoder, encoder_face, registration_vertices, pose):
         verts_unposed = lbs_fn.unpose(registration_vertices, pose)
         verts_unposed_uv = geo_fn.to_uv(verts_unposed)
     return {**encoder(verts_unposed_uv), **encoder_face(verts_unposed_uv)}
+
+
+class _PixelBias(Function):
+    """rgb + bilinear(bias[idx]) on csrc/body_frame.cu; the bias gradient is a fixed-order gather per texel"""
+
+    @staticmethod
+    def forward(ctx, rgb, bias, idx):
+        rgb, bias, idx = rgb.contiguous(), bias.contiguous(), idx.contiguous()
+        _lib.check_input(rgb, "rgb")
+        _lib.check_input(bias, "bias")
+        _lib.check_input(idx, "camera indices", torch.int64)
+        B, C, H, W = rgb.shape
+        if bias.dim() != 4 or bias.shape[1] != 1 or idx.shape != (B,):
+            raise RuntimeError("pixel bias: bias must be [n_cams,1,h,w] and the indices [B] (got %s, %s)"
+                               % (tuple(bias.shape), tuple(idx.shape)))
+        out = torch.empty_like(rgb)
+        n, _, Hb, Wb = bias.shape
+        with torch.cuda.device(rgb.device):
+            _lib.check(_lib.lib().gb_pixel_bias_fwd(B, C, H, W, n, Hb, Wb, _lib.ptr(rgb), _lib.ptr(bias), _lib.ptr(idx),
+                                                    _lib.ptr(out), _lib.stream_ptr(rgb.device)), "pixel_bias_fwd")
+        ctx.save_for_backward(idx)
+        ctx.shapes = (tuple(rgb.shape), tuple(bias.shape))
+        return out
+
+    @staticmethod
+    def backward(ctx, g_out):
+        (idx,) = ctx.saved_tensors
+        (B, C, H, W), (n, _, Hb, Wb) = ctx.shapes
+        g_bias = None
+        if ctx.needs_input_grad[1]:
+            g_out = g_out.contiguous()
+            g_bias = torch.empty(n, 1, Hb, Wb, device=g_out.device)
+            with torch.cuda.device(g_out.device):
+                _lib.check(_lib.lib().gb_pixel_bias_bwd(B, C, H, W, n, Hb, Wb, _lib.ptr(idx), _lib.ptr(g_out),
+                                                        _lib.ptr(g_bias), _lib.stream_ptr(g_out.device)),
+                           "pixel_bias_bwd")
+        return g_out if ctx.needs_input_grad[0] else None, g_bias, None
+
+
+class CameraPixelBias(tnn.Module):
+    """mesh_vae.py:51-69 with its parameter `bias` [n_cams, 1, image_width // ds_rate, image_height // ds_rate] (width
+    and height swapped, as in the reference) stretched to (image_height, image_width) with torch's half-pixel bilinear
+    index.  forward(idxs [B] int64, rgb [B,C,H,W]) -> rgb + bias_up in one kernel (mesh_vae.py:335-339); without rgb it
+    returns bias_up [B,1,H,W] as the reference's forward does.  Two backward calls give the same bits."""
+
+    def __init__(self, image_height, image_width, cameras, ds_rate) -> None:
+        super().__init__()
+        self.image_height, self.image_width = image_height, image_width
+        self.cameras = cameras
+        self.n_cameras = len(cameras)
+        self.register_parameter("bias", tnn.Parameter(
+            torch.zeros(self.n_cameras, 1, image_width // ds_rate, image_height // ds_rate)))
+
+    def forward(self, idxs: torch.Tensor, rgb: torch.Tensor = None) -> torch.Tensor:
+        if rgb is None:
+            rgb = torch.zeros(idxs.shape[0], 1, self.image_height, self.image_width, device=self.bias.device)
+        if tuple(rgb.shape[2:]) != (self.image_height, self.image_width):
+            raise RuntimeError("CameraPixelBias: the image must be %d x %d (got %s)"
+                               % (self.image_height, self.image_width, tuple(rgb.shape)))
+        return _PixelBias.apply(rgb, self.bias, idxs)
+
+
+def _gaussian_blur(img, kernel_size):
+    """torchvision.transforms.functional.gaussian_blur(img, kernel_size) with its default sigma
+    0.3 ((k - 1) 0.5 - 1) + 0.8 and reflect padding, restated in torch (one-off asset preparation on the CPU)"""
+    sigma = 0.3 * ((kernel_size - 1) * 0.5 - 1) + 0.8
+    half = (kernel_size - 1) * 0.5
+    x = torch.linspace(-half, half, steps=kernel_size, dtype=img.dtype)
+    k1 = torch.exp(-0.5 * (x / sigma).pow(2))
+    k1 = k1 / k1.sum()
+    k2 = torch.mm(k1[:, None], k1[None, :]).expand(img.shape[-3], 1, kernel_size, kernel_size)
+    p = kernel_size // 2
+    return F.conv2d(F.pad(img, [p, p, p, p], mode="reflect"), k2, groups=img.shape[-3])
+
+
+def _values_to_uv_cpu(values, index_img, bary_img):
+    """geom.values_to_uv (geom.py:308-324) in torch, for the constructor's one-off `meye_mask`"""
+    index_mask = torch.all(index_img != -1, dim=-1)
+    flat = torch.sum(values[:, index_img[index_mask].to(torch.int64)].permute(0, 3, 1, 2)
+                     * bary_img[index_mask].to(torch.float32), dim=-1)
+    out = torch.zeros(values.shape[0], values.shape[-1], *index_img.shape[:2], dtype=values.dtype)
+    out[:, :, index_mask] = flat
+    return out
+
+
+UV_IMAGES = ("index_image", "bary_image", "face_index_image", "valid_mask")
+
+
+def _get(obj, name, default=None):
+    if isinstance(obj, dict):
+        return obj.get(name, default)
+    return getattr(obj, name, default)
+
+
+class AutoEncoder(tnn.Module):
+    """mesh_vae.AutoEncoder (mesh_vae.py:72-341): the body avatar's frame on this project's stages, with the
+    reference's constructor and state-dict keys (the shared geometry module and seam sampler repeat under
+    `decoder.*` / `decoder_view.*`), so `AutoEncoder(**config.model, assets=assets)` builds from mesh_vae_example.yml
+    and a reference checkpoint loads with strict=True.
+
+    `assets` (attributes or dict keys) carries the reference's assets and, because this project does not rasterise
+    the UV layout, the four `geo_fn` images a checkpoint stores: index_image / bary_image [1024,1024,3],
+    face_index_image [1024,1024] and valid_mask [1024,1024,1].  `tex_mean` (blur + resize of color_mean) and
+    `meye_mask` are prepared in torch on the CPU at construction, as the reference's constructor does.
+
+    forward() runs on CUDA only and issues no host synchronisation after the first call (which builds the cached
+    gather and render tables).  Unlike the reference, `preds["shadow_map"]` is the shadow net's map, not the copy
+    forward_tex impaints in place; `pose_to_shadow`, `encode=False` and `pixel_cal` without `cal` raise."""
+
+    forward_tex = TextureComposer.forward
+    _check = TextureComposer._check
+
+    def __init__(self, encoder, encoder_face, decoder, decoder_view, shadow_net, upscale_net, assets,
+                 pose_to_shadow=None, renderer=None, cal=None, pixel_cal=None, learn_blur: bool = True):
+        super().__init__()
+        from .geom import GeometryModule
+        from .lbs import LBSModule
+        from .mesh_render import RenderLayer
+        from .photo_loss import CalV5, LearnableBlur
+        from .shadow import ShadowUNet
+
+        if pose_to_shadow is not None:
+            raise NotImplementedError("AutoEncoder: pose_to_shadow (PoseToShadow) is not implemented")
+        if pixel_cal is not None and cal is None:
+            raise ValueError("AutoEncoder: pixel_cal needs cal (its camera indices are cal's)")
+        missing = [k for k in UV_IMAGES if _get(assets, k) is None]
+        if missing:
+            raise ValueError("AutoEncoder: assets must carry the UV images %s at 1024 x 1024 (the reference's "
+                             "geo_fn.* buffers); missing: %s" % (", ".join(UV_IMAGES), ", ".join(missing)))
+        uv = {k: torch.as_tensor(np.asarray(_get(assets, k))) for k in UV_IMAGES}
+        for k, t in uv.items():
+            if tuple(t.shape[:2]) != (1024, 1024):
+                raise ValueError("AutoEncoder: assets.%s must be 1024 x 1024 (got %s)" % (k, tuple(t.shape)))
+
+        topo = _get(assets, "topology")
+        self.geo_fn = GeometryModule(_get(topo, "vi"), uv["index_image"], uv["bary_image"], vt=_get(topo, "vt"),
+                                     v2uv=_get(topo, "v2uv"), vti=_get(topo, "vti"),
+                                     face_index_image=uv["face_index_image"], valid_mask=uv["valid_mask"])
+        self.lbs_fn = LBSModule(_get(assets, "lbs_model_json"), _get(assets, "lbs_config_dict"),
+                                _get(assets, "template_mesh"), _get(assets, "skeleton_scales"),
+                                _get(assets, "global_scaling"))
+        self.seam_sampler = SeamSampler(_get(assets, "seam_data_1024"))
+        self.seam_sampler_2k = SeamSampler(_get(assets, "seam_data_2048"))
+
+        tex_mean = _gaussian_blur(torch.as_tensor(np.asarray(_get(assets, "color_mean")), dtype=torch.float32)[None],
+                                  kernel_size=11)
+        self.register_buffer("tex_mean", F.interpolate(tex_mean, (2048, 2048), mode="bilinear"))
+        tex_var = _get(assets, "tex_var")
+        self.tex_std = tex_var if tex_var is not None else 64.0
+
+        self.register_buffer("face_cond_mask", torch.as_tensor(
+            np.asarray(_get(assets, "face_cond_mask")), dtype=torch.float32)[None, None])
+        meye = _values_to_uv_cpu(torch.as_tensor(np.asarray(_get(assets, "mouth_eyes_mask_geom"))[None, :, None]),
+                                 uv["index_image"], uv["bary_image"])
+        self.register_buffer("meye_mask", F.interpolate(meye, (2048, 2048), mode="bilinear"))
+
+        self.decoder = ConvDecoder(geo_fn=self.geo_fn, seam_sampler=self.seam_sampler, **decoder, assets=assets)
+        face_mask = np.asarray(_get(assets, "face_mask"))
+        self.encoder = Encoder(mask=1.0 - face_mask, **encoder)
+        self.encoder_face = FaceEncoder(mask=face_mask, **encoder_face)
+        self.decoder_view = UNetViewDecoder(self.geo_fn, seam_sampler=self.seam_sampler, **decoder_view)
+        self.shadow_net = ShadowUNet(ao_mean=_get(assets, "ambient_occlusion_mean"), interp_mode="bilinear",
+                                     biases=False, **shadow_net)
+        self.pose_to_shadow_enabled = False
+        self.upscale_net = UpscaleNet(in_channels=6, size=1024, upscale_factor=2, out_channels=3, **upscale_net)
+
+        cameras = _get(assets, "camera_ids")
+        self.pixel_cal_enabled = pixel_cal is not None
+        if self.pixel_cal_enabled:
+            self.pixel_cal = CameraPixelBias(**pixel_cal, cameras=cameras)
+        self.learn_blur_enabled = bool(learn_blur)
+        if self.learn_blur_enabled:
+            self.learn_blur = LearnableBlur(cameras)
+        self.cal_enabled = cal is not None
+        if self.cal_enabled:
+            self.cal = CalV5(**cal, cameras=cameras)
+        self.rendering_enabled = renderer is not None
+        if self.rendering_enabled:
+            self.renderer = RenderLayer(h=_get(renderer, "image_height"), w=_get(renderer, "image_width"),
+                                        vt=self.geo_fn.vt, vi=self.geo_fn.vi, vti=self.geo_fn.vti, flip_uvs=False)
+
+    def encode(self, registration_vertices, pose):
+        return encode(self.lbs_fn, self.geo_fn, self.encoder, self.encoder_face, registration_vertices, pose)
+
+    def forward(self, pose, campos, registration_vertices=None, ambient_occlusion=None, K=None, Rt=None,
+                camera_id=None, frame_id=None, embs=None, encode=True, iteration=None, **kwargs):
+        if not encode:
+            raise ValueError("AutoEncoder.forward: encode=False is not supported (the reference leaves face_embs "
+                             "unbound on that path)")
+        enc_preds = self.encode(registration_vertices, pose)
+        dec_preds = self.decoder(pose=pose, embs=enc_preds["embs"], face_embs=enc_preds["face_embs"])
+        geom_rec = self.lbs_fn.pose(dec_preds["geom_delta_rec"], pose)
+        dec_view_preds = self.decoder_view(geom_rec=geom_rec, tex_mean_rec=dec_preds["tex_mean_rec"],
+                                           camera_pos=campos)
+        shadow_preds = self.shadow_net(ao_map=ambient_occlusion)
+        tex_rec = self.forward_tex(dec_preds["tex_mean_rec"], dec_view_preds["tex_view_rec"],
+                                   shadow_preds["shadow_map"])
+        cam_idxs = None
+        if self.cal_enabled:
+            cam_idxs = self.cal.name_to_idx(camera_id)
+            tex_rec = self.cal(tex_rec, cam_idxs)
+        preds = {"geom": geom_rec, "tex_rec": tex_rec, **dec_preds, **shadow_preds, **dec_view_preds, **enc_preds}
+        if self.rendering_enabled:
+            tex_seg = torch.ones_like(tex_rec[:, :1])
+            renders = self.renderer(preds["geom"], tex=torch.cat([tex_rec, tex_seg], dim=1), K=K, Rt=Rt)
+            render_depth = renders["depth_img"][:, None].detach()
+            preds.update(rgb=renders["render"][:, :3], alpha=renders["render"][:, 3:],
+                         depth_disc_mask=depth_discontuity_mask(render_depth), depth=render_depth)
+        if self.learn_blur_enabled:
+            preds["rgb"] = self.learn_blur(preds["rgb"], camera_id)
+            preds["learn_blur_weights"] = self.learn_blur.reg(camera_id)
+        if self.pixel_cal_enabled:
+            preds["rgb"] = self.pixel_cal(cam_idxs, preds["rgb"])
+        return preds

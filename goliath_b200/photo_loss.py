@@ -118,3 +118,84 @@ def photometric_loss(pred: torch.Tensor, target: torch.Tensor, mask: torch.Tenso
     (mask [B,1,H,W] broadcast over the channels, 11x11 window).  Returns (loss, {"rgb_l1", "rgb_ssim"})."""
     loss, l1, ssim = _SsimL1.apply(pred, target, mask, l1_weight, ssim_weight)
     return loss, {"rgb_l1": l1, "rgb_ssim": 1.0 - ssim}
+
+
+def _indices_to_device(rows, device: torch.device) -> torch.Tensor:
+    """host int list -> int64 device tensor in one non-blocking copy from pinned memory (no host synchronisation)"""
+    if device.type != "cuda":
+        raise RuntimeError("the camera modules run on CUDA only (no CPU fallback): move them to the GPU first")
+    return torch.tensor(rows, dtype=torch.int64).pin_memory().to(device, non_blocking=True)
+
+
+class ParamHolder(torch.nn.Module):
+    """ca_code/utils/torchutils.py:56-72: `params` [len(key_list), *param_shape] over the sorted key list"""
+
+    def __init__(self, param_shape, key_list, init_value=None):
+        super().__init__()
+        if isinstance(param_shape, int):
+            param_shape = (param_shape,)
+        self.key_list = sorted(key_list)
+        self.params = torch.nn.Parameter(torch.zeros(len(self.key_list), *param_shape))
+        if init_value is not None:
+            self.params.data[:] = init_value
+
+    def to_idx(self, keys):
+        """host indices of `keys` in the sorted key list (a ValueError names an unknown key)"""
+        return [self.key_list.index(k) for k in keys]
+
+
+class CalV5(torch.nn.Module):
+    """ca_code/nn/color_cal.py:101-241 on post_render's calibration stage.  `holder.params` [n_cams, 6] = (w, b) per
+    camera in sorted name order; cameras whose name starts with "41" are grey (out = sum_c img_c w_c + sum_c b_c on
+    all three channels, initial w = (0.37, 0.52, 0.52)); the identity camera passes through and its row gets no
+    gradient.  In training the parameter gradient is scaled per item by gs_lrscale (grey) / col_lrscale (colour), as
+    the reference's scale_hook does.  `name_to_idx` maps names on the host and copies the indices without a sync."""
+
+    def __init__(self, cameras, identity_camera, gs_lrscale: float = 1e0, col_lrscale: float = 1e-1):
+        super().__init__()
+        if identity_camera not in cameras:   # the reference's fallback (an id given as a YAML int lands here too)
+            identity_camera = cameras[0]
+        self.identity_camera = identity_camera
+        self.cameras = cameras
+        self.gs_lrscale, self.col_lrscale = gs_lrscale, col_lrscale
+        self.holder = ParamHolder(3 + 3, cameras, init_value=torch.FloatTensor([1, 1, 1, 0, 0, 0]))
+        self.identity_idx = self.holder.to_idx([identity_camera])[0]
+        self.grey_idxs = [self.holder.to_idx([c])[0] for c in cameras if c.startswith("41")]
+        self.holder.params.data[torch.LongTensor(self.grey_idxs), :3] = torch.FloatTensor([0.37, 0.52, 0.52])
+        grey = torch.zeros(len(self.holder.key_list), dtype=torch.bool)
+        grey[self.grey_idxs] = True
+        self.register_buffer("grey_mask", grey, persistent=False)
+
+    def name_to_idx(self, cam_names) -> torch.Tensor:
+        return _indices_to_device(self.holder.to_idx(cam_names), self.holder.params.device)
+
+    def forward(self, image: torch.Tensor, cam_idxs: torch.Tensor) -> torch.Tensor:
+        params = self.holder.params[cam_idxs]
+        ident = cam_idxs == self.identity_idx
+        grey = self.grey_mask[cam_idxs] & ~ident
+        if self.training and params.requires_grad:
+            scale = torch.where(grey, self.gs_lrscale, self.col_lrscale).masked_fill(ident, 1.0).to(params.dtype)
+            params.register_hook(lambda g: g * scale[:, None])
+        w = torch.where(ident[:, None], 1.0, params[:, :3])
+        b = torch.where(ident[:, None], 0.0, params[:, 3:])
+        return post_render(image, cal_w=w, cal_b=b, grey=grey.to(torch.int32))
+
+
+class LearnableBlur(torch.nn.Module):
+    """ca_code/nn/dof_cal.py:20-56 on post_render's blur stage: softmax(weights_raw[camera]) mixes the image with its
+    3x3 and 7x7 Gaussian blurs.  Cameras index `weights_raw` in the list's order, as in the reference."""
+
+    def __init__(self, cameras):
+        super().__init__()
+        self.cameras = cameras
+        self.register_parameter("weights_raw", torch.nn.Parameter(torch.ones(len(cameras), 3, dtype=torch.float32)))
+
+    def name_to_idx(self, cameras) -> torch.Tensor:
+        return _indices_to_device([self.cameras.index(c) for c in cameras], self.weights_raw.device)
+
+    def reg(self, cameras):
+        return self.weights_raw[self.name_to_idx(cameras)]
+
+    def forward(self, img: torch.Tensor, cameras) -> torch.Tensor:
+        weights = torch.softmax(self.weights_raw[self.name_to_idx(cameras)], dim=-1)
+        return post_render(img, blur_weights=weights)

@@ -793,6 +793,25 @@ int gb_downconv_block_bwd(int B, int Cin, int Cout, int groups, int H, int W, co
                           float* gz2, float* gz1, float* gb1, float* gb2, float* gbr, float* gw1, float* gw2,
                           float* gwr, float* gx, void* workspace, void* stream);
 
+/* ---------------------------------------------------------------- body frame (row R9'''', csrc/body_frame.cu) */
+
+/* replaces geom.depth_discontuity_mask (ca_code/utils/geom.py:768-794) with its pool_ksize 3: Sobel x / y of depth
+ * [B,1,H,W] with zero padding, sqrt(gx^2 + gy^2) > threshold (evaluated in double), then the 3x3 stride-1 avg_pool > 0,
+ * i.e. any such pixel among the neighbours inside the image.  mask [B,1,H,W] uint8 (torch.bool) is written once.
+ * Forward only: the reference runs it under no_grad on a detached depth (mesh_vae.py:320-322). */
+int gb_depth_disc_mask(int B, int H, int W, const float* depth, float threshold, unsigned char* mask, void* stream);
+/* replaces rgb + CameraPixelBias(idx) (ca_code/models/mesh_vae.py:51-69 and :335-339):
+ *   out[b,c] = rgb[b,c] + bilinear(bias[idx[b]] [Hb,Wb] -> H x W, align_corners = False)
+ * rgb / out [B,C,H,W], bias [n_cams,1,Hb,Wb] (the reference's parameter is [n_cams,1,W/ds,H/ds]: Hb = W/ds is stretched
+ * over H), idx [B] int64 (an index outside [0, n_cams) adds nothing).  out may not alias rgb. */
+int gb_pixel_bias_fwd(int B, int C, int H, int W, int n_cams, int Hb, int Wb, const float* rgb, const float* bias,
+                      const long long* idx, float* out, void* stream);
+/* the bias gradient of the above: g_bias [n_cams,1,Hb,Wb] is WRITTEN, one thread per camera and texel, summing its
+ * upsample footprint over the C channels and over the items b with idx[b] == camera in batch order (no float atomics:
+ * the same bits on every call).  The rgb gradient is g_out itself. */
+int gb_pixel_bias_bwd(int B, int C, int H, int W, int n_cams, int Hb, int Wb, const long long* idx, const float* g_out,
+                      float* g_bias, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
