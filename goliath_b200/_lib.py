@@ -144,6 +144,10 @@ SIGNATURES = {
     "gb_depth_disc_mask": (_i, [_i] * 3 + [_vp, _f, _vp, _vp]),
     "gb_pixel_bias_fwd": (_i, [_i] * 7 + [_vp] * 4 + [_vp]),
     "gb_pixel_bias_bwd": (_i, [_i] * 7 + [_vp] * 3 + [_vp]),
+    "gb_face_tex_tail_fwd": (_i, [_i] * 5 + [_vp] * 7 + [_vp]),
+    "gb_face_tex_cond_fwd": (_i, [_i] * 6 + [_vp] * 3 + [_vp]),
+    "gb_pose_shadow_fwd": (_i, [_i] * 5 + [_vp, _f, _vp, _vp]),
+    "gb_pose_shadow_bwd": (_i, [_i] * 5 + [_vp, _f, _vp, _vp, _vp]),
 }
 
 

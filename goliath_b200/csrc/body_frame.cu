@@ -54,29 +54,6 @@ __global__ void __launch_bounds__(DD_TX * DD_TY) depth_disc_kernel(int H, int W,
   out[blockIdx.z * plane + (size_t)py * W + px] = any;
 }
 
-// torch's upsample_bilinear2d source index (align_corners=False, no scale factor): src = in/out * (dst + 0.5) - 0.5,
-// clamped at 0; i0 = floor, i1 = i0 + 1 except at the last input index, l1 = src - i0.
-struct Tap {
-  int i0, i1;
-  float l0, l1;
-};
-
-__device__ __forceinline__ Tap tap(int dst, float scale, int n_in) {
-  float s = scale * ((float)dst + 0.5f) - 0.5f;
-  s = s < 0.f ? 0.f : s;
-  Tap t;
-  t.i0 = (int)s;
-  t.i1 = t.i0 + (t.i0 < n_in - 1 ? 1 : 0);
-  t.l1 = s - (float)t.i0;
-  t.l0 = 1.f - t.l1;
-  return t;
-}
-
-// weight of input index `i` in output index `dst` (both taps count when they coincide at the border)
-__device__ __forceinline__ float tap_weight(const Tap& t, int i) {
-  return (t.i0 == i ? t.l0 : 0.f) + (t.i1 == i ? t.l1 : 0.f);
-}
-
 __global__ void __launch_bounds__(256) pixel_bias_fwd_kernel(int B, int C, int H, int W, int n_cams, int Hb, int Wb,
                                                              const float* __restrict__ rgb,
                                                              const float* __restrict__ bias,
@@ -89,18 +66,13 @@ __global__ void __launch_bounds__(256) pixel_bias_fwd_kernel(int B, int C, int H
   float v = 0.f;
   if (n >= 0 && n < n_cams) {
     const float* P = bias + (size_t)n * Hb * Wb;
-    const Tap ty = tap(y, (float)Hb / (float)H, Hb), tx = tap(x, (float)Wb / (float)W, Wb);
+    const gb::ResizeTap ty = gb::resize_tap(y, (float)Hb / (float)H, Hb);
+    const gb::ResizeTap tx = gb::resize_tap(x, (float)Wb / (float)W, Wb);
     v = ty.l0 * (tx.l0 * P[ty.i0 * Wb + tx.i0] + tx.l1 * P[ty.i0 * Wb + tx.i1]) +
         ty.l1 * (tx.l0 * P[ty.i1 * Wb + tx.i0] + tx.l1 * P[ty.i1 * Wb + tx.i1]);
   }
   const size_t plane = (size_t)H * W, o = (size_t)y * W + x;
   for (int c = 0; c < C; ++c) out[((size_t)b * C + c) * plane + o] = rgb[((size_t)b * C + c) * plane + o] + v;
-}
-
-// range of output indices whose taps can reach input index i (a superset; tap_weight decides)
-__device__ __forceinline__ void footprint(int i, float scale, int n_out, int& lo, int& hi) {
-  lo = max(0, (int)floorf(((float)i - 0.5f) / scale - 0.5f) - 2);
-  hi = min(n_out - 1, (int)ceilf(((float)i + 1.5f) / scale - 0.5f) + 2);
 }
 
 __global__ void __launch_bounds__(256) pixel_bias_bwd_kernel(int B, int C, int H, int W, int n_cams, int Hb, int Wb,
@@ -112,8 +84,8 @@ __global__ void __launch_bounds__(256) pixel_bias_bwd_kernel(int B, int C, int H
   const int n = t / (Hb * Wb), by = (t / Wb) % Hb, bx = t % Wb;
   const float sy = (float)Hb / (float)H, sx = (float)Wb / (float)W;
   int ylo, yhi, xlo, xhi;
-  footprint(by, sy, H, ylo, yhi);
-  footprint(bx, sx, W, xlo, xhi);
+  gb::resize_footprint(by, sy, H, ylo, yhi);
+  gb::resize_footprint(bx, sx, W, xlo, xhi);
   const size_t plane = (size_t)H * W;
   float acc = 0.f;
   for (int b = 0; b < B; ++b) {  // batch order
@@ -121,11 +93,11 @@ __global__ void __launch_bounds__(256) pixel_bias_bwd_kernel(int B, int C, int H
     const float* G = g_out + (size_t)b * C * plane;
     float item = 0.f;
     for (int y = ylo; y <= yhi; ++y) {
-      const float wy = tap_weight(tap(y, sy, Hb), by);
+      const float wy = gb::resize_tap_weight(gb::resize_tap(y, sy, Hb), by);
       if (wy == 0.f) continue;
       float row = 0.f;
       for (int x = xlo; x <= xhi; ++x) {
-        const float wx = tap_weight(tap(x, sx, Wb), bx);
+        const float wx = gb::resize_tap_weight(gb::resize_tap(x, sx, Wb), bx);
         if (wx == 0.f) continue;
         float s = 0.f;
         for (int c = 0; c < C; ++c) s += G[c * plane + (size_t)y * W + x];

@@ -77,4 +77,33 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
+// torch's upsample_bilinear2d source index (align_corners=False, no scale factor): src = in/out * (dst + 0.5) - 0.5 in
+// fp32, clamped at 0; i0 = floor, i1 = i0 + 1 except at the last input index, l1 = src - i0.  `scale` is in/out.
+struct ResizeTap {
+  int i0, i1;
+  float l0, l1;
+};
+
+__device__ __forceinline__ ResizeTap resize_tap(int dst, float scale, int n_in) {
+  float s = scale * ((float)dst + 0.5f) - 0.5f;
+  s = s < 0.f ? 0.f : s;
+  ResizeTap t;
+  t.i0 = (int)s;
+  t.i1 = t.i0 + (t.i0 < n_in - 1 ? 1 : 0);
+  t.l1 = s - (float)t.i0;
+  t.l0 = 1.f - t.l1;
+  return t;
+}
+
+// weight of input index `i` in an output index's taps (both taps count when they coincide at the border)
+__device__ __forceinline__ float resize_tap_weight(const ResizeTap& t, int i) {
+  return (t.i0 == i ? t.l0 : 0.f) + (t.i1 == i ? t.l1 : 0.f);
+}
+
+// range of output indices whose taps can reach input index i (a superset; resize_tap_weight decides)
+__device__ __forceinline__ void resize_footprint(int i, float scale, int n_out, int& lo, int& hi) {
+  lo = max(0, (int)floorf(((float)i - 0.5f) / scale - 0.5f) - 2);
+  hi = min(n_out - 1, (int)ceilf(((float)i + 1.5f) / scale - 0.5f) + 2);
+}
+
 }  // namespace gb

@@ -124,8 +124,10 @@ class ConvDecoder(tnn.Module):
         self.register_buffer("face_cond_mask", f32(_asset(assets, "face_cond_mask"))[None, None])
         self.register_buffer("body_cond_mask", f32(_asset(assets, "body_cond_mask"))[None, None])
 
-    def forward(self, pose, embs, face_embs):
-        for t, n in ((pose, "pose"), (embs, "embs"), (face_embs, "face_embs")):
+    def forward(self, pose, embs, face_embs, embs_conv=None):
+        """`embs_conv` [B, n_embs_enc_channels, S, S], when given, replaces the decoded `embs` map (as in
+        mesh_vae_drivable.py:614-615); the face merge is written into a copy, never into the caller's tensor."""
+        for t, n in ((pose, "pose"), (embs if embs_conv is None else embs_conv, "embs"), (face_embs, "face_embs")):
             if not t.is_cuda:
                 raise RuntimeError("ConvDecoder runs on CUDA only (no CPU fallback): %s is on %s" % (n, t.device))
         B = pose.shape[0]
@@ -133,7 +135,10 @@ class ConvDecoder(tnn.Module):
         non_head_mask = (self.body_cond_mask * (1.0 - self.face_cond_mask)).clip(0.0, 1.0)
         pose_masked = tile2d(local_pose, self.init_uv_size) * self.pose_cond_mask
         pose_conv = self.local_pose_conv_block(pose_masked) * non_head_mask
-        embs_conv = self.embs_conv_block(self.embs_fc(embs).reshape(B, 128, 4, 4))
+        if embs_conv is None:
+            embs_conv = self.embs_conv_block(self.embs_fc(embs).reshape(B, 128, 4, 4))
+        else:
+            embs_conv = embs_conv.clone()
         face_conv = self.face_embs_conv_block(self.face_embs_fc(face_embs).reshape(B, 32, 4, 4))
         # merging embeddings with spatial masks
         embs_conv[:, :, 32:, :32] = (face_conv * self.face_cond_mask[:, :, 32:, :32]
@@ -462,6 +467,47 @@ def _get(obj, name, default=None):
     return getattr(obj, name, default)
 
 
+def _uv_geometry(assets):
+    """the frame's GeometryModule from `assets.topology` and the four UV images the assets must carry at 1024 x 1024;
+    returns (geo_fn, {name: image})"""
+    from .geom import GeometryModule
+
+    missing = [k for k in UV_IMAGES if _get(assets, k) is None]
+    if missing:
+        raise ValueError("AutoEncoder: assets must carry the UV images %s at 1024 x 1024 (the reference's "
+                         "geo_fn.* buffers); missing: %s" % (", ".join(UV_IMAGES), ", ".join(missing)))
+    uv = {k: torch.as_tensor(np.asarray(_get(assets, k))) for k in UV_IMAGES}
+    for k, t in uv.items():
+        if tuple(t.shape[:2]) != (1024, 1024):
+            raise ValueError("AutoEncoder: assets.%s must be 1024 x 1024 (got %s)" % (k, tuple(t.shape)))
+    topo = _get(assets, "topology")
+    geo_fn = GeometryModule(_get(topo, "vi"), uv["index_image"], uv["bary_image"], vt=_get(topo, "vt"),
+                            v2uv=_get(topo, "v2uv"), vti=_get(topo, "vti"), face_index_image=uv["face_index_image"],
+                            valid_mask=uv["valid_mask"])
+    return geo_fn, uv
+
+
+def _image_stages(model, cameras, renderer, cal, pixel_cal, learn_blur):
+    """the frame's optional image-space modules under the reference's names and order: pixel_cal, learn_blur, cal,
+    renderer (a RenderLayer over model.geo_fn's topology)"""
+    from .mesh_render import RenderLayer
+    from .photo_loss import CalV5, LearnableBlur
+
+    model.pixel_cal_enabled = pixel_cal is not None
+    if model.pixel_cal_enabled:
+        model.pixel_cal = CameraPixelBias(**pixel_cal, cameras=cameras)
+    model.learn_blur_enabled = bool(learn_blur)
+    if model.learn_blur_enabled:
+        model.learn_blur = LearnableBlur(cameras)
+    model.cal_enabled = cal is not None
+    if model.cal_enabled:
+        model.cal = CalV5(**cal, cameras=cameras)
+    model.rendering_enabled = renderer is not None
+    if model.rendering_enabled:
+        model.renderer = RenderLayer(h=_get(renderer, "image_height"), w=_get(renderer, "image_width"),
+                                     vt=model.geo_fn.vt, vi=model.geo_fn.vi, vti=model.geo_fn.vti, flip_uvs=False)
+
+
 class AutoEncoder(tnn.Module):
     """mesh_vae.AutoEncoder (mesh_vae.py:72-341): the body avatar's frame on this project's stages, with the
     reference's constructor and state-dict keys (the shared geometry module and seam sampler repeat under
@@ -483,29 +529,14 @@ class AutoEncoder(tnn.Module):
     def __init__(self, encoder, encoder_face, decoder, decoder_view, shadow_net, upscale_net, assets,
                  pose_to_shadow=None, renderer=None, cal=None, pixel_cal=None, learn_blur: bool = True):
         super().__init__()
-        from .geom import GeometryModule
         from .lbs import LBSModule
-        from .mesh_render import RenderLayer
-        from .photo_loss import CalV5, LearnableBlur
         from .shadow import ShadowUNet
 
         if pose_to_shadow is not None:
             raise NotImplementedError("AutoEncoder: pose_to_shadow (PoseToShadow) is not implemented")
         if pixel_cal is not None and cal is None:
             raise ValueError("AutoEncoder: pixel_cal needs cal (its camera indices are cal's)")
-        missing = [k for k in UV_IMAGES if _get(assets, k) is None]
-        if missing:
-            raise ValueError("AutoEncoder: assets must carry the UV images %s at 1024 x 1024 (the reference's "
-                             "geo_fn.* buffers); missing: %s" % (", ".join(UV_IMAGES), ", ".join(missing)))
-        uv = {k: torch.as_tensor(np.asarray(_get(assets, k))) for k in UV_IMAGES}
-        for k, t in uv.items():
-            if tuple(t.shape[:2]) != (1024, 1024):
-                raise ValueError("AutoEncoder: assets.%s must be 1024 x 1024 (got %s)" % (k, tuple(t.shape)))
-
-        topo = _get(assets, "topology")
-        self.geo_fn = GeometryModule(_get(topo, "vi"), uv["index_image"], uv["bary_image"], vt=_get(topo, "vt"),
-                                     v2uv=_get(topo, "v2uv"), vti=_get(topo, "vti"),
-                                     face_index_image=uv["face_index_image"], valid_mask=uv["valid_mask"])
+        self.geo_fn, uv = _uv_geometry(assets)
         self.lbs_fn = LBSModule(_get(assets, "lbs_model_json"), _get(assets, "lbs_config_dict"),
                                 _get(assets, "template_mesh"), _get(assets, "skeleton_scales"),
                                 _get(assets, "global_scaling"))
@@ -534,20 +565,7 @@ class AutoEncoder(tnn.Module):
         self.pose_to_shadow_enabled = False
         self.upscale_net = UpscaleNet(in_channels=6, size=1024, upscale_factor=2, out_channels=3, **upscale_net)
 
-        cameras = _get(assets, "camera_ids")
-        self.pixel_cal_enabled = pixel_cal is not None
-        if self.pixel_cal_enabled:
-            self.pixel_cal = CameraPixelBias(**pixel_cal, cameras=cameras)
-        self.learn_blur_enabled = bool(learn_blur)
-        if self.learn_blur_enabled:
-            self.learn_blur = LearnableBlur(cameras)
-        self.cal_enabled = cal is not None
-        if self.cal_enabled:
-            self.cal = CalV5(**cal, cameras=cameras)
-        self.rendering_enabled = renderer is not None
-        if self.rendering_enabled:
-            self.renderer = RenderLayer(h=_get(renderer, "image_height"), w=_get(renderer, "image_width"),
-                                        vt=self.geo_fn.vt, vi=self.geo_fn.vi, vti=self.geo_fn.vti, flip_uvs=False)
+        _image_stages(self, _get(assets, "camera_ids"), renderer, cal, pixel_cal, learn_blur)
 
     def encode(self, registration_vertices, pose):
         return encode(self.lbs_fn, self.geo_fn, self.encoder, self.encoder_face, registration_vertices, pose)

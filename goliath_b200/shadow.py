@@ -8,13 +8,18 @@ Initialisation: the reference applies `blocks.weights_initializer`, whose `kaimi
 the weight-normalised layer's derived `weight` tensor and leaves `weight_v` / `weight_g` as the constructor made them.
 So `weight_v` keeps nn.Conv2d's default init (bounded by 1/sqrt(fan_in)), `weight_g` is the whole-tensor norm of
 `weight_v` (the effective weight equals `weight_v`), and every bias is zero — which is what the layers' constructors
-here already produce.  CUDA only; CPU tensors raise."""
+here already produce.  CUDA only; CPU tensors raise.
+
+`PoseToShadow` (ca_code/nn/shadow.py:429-471), the drivable body's shadow from the pose alone, runs its transposed
+convolutions on the fused layer kernels and sigmoid(. + beta) with the resize on csrc/body_drive.cu."""
 import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from torch.autograd import Function
 
-from .nn import Conv2dWN, Conv2dWNUB, FusedLeakyReLU
+from . import _lib
+from .nn import Conv2dWN, Conv2dWNUB, ConvTranspose2dWNUB, FusedLeakyReLU, LinearWN, glorot
 
 
 def _conv3x3(cin, cout, size, slope):
@@ -75,3 +80,66 @@ class ShadowUNet(nn.Module):
         shadow_map = F.interpolate(shadow_map_lowres, (self.uv_size, self.uv_size), mode=self.interp_mode,
                                    align_corners=self.align_corners)
         return {"shadow_map": shadow_map, "ao_map": ao_map, "shadow_map_lowres": shadow_map_lowres}
+
+
+class _PoseShadow(Function):
+    """bilinear(sigmoid(x + beta) -> size x size, align_corners=False) on csrc/body_drive.cu; the backward is a
+    fixed-order gather per low-resolution texel"""
+
+    @staticmethod
+    def forward(ctx, x, beta, size):
+        x = x.contiguous()
+        _lib.check_input(x, "input")
+        B, C, h, w = x.shape
+        out = torch.empty(B, C, size, size, device=x.device)
+        with torch.cuda.device(x.device):
+            _lib.check(_lib.lib().gb_pose_shadow_fwd(B * C, h, w, size, size, _lib.ptr(x), float(beta), _lib.ptr(out),
+                                                     _lib.stream_ptr(x.device)), "pose_shadow_fwd")
+        ctx.save_for_backward(x)
+        ctx.beta = float(beta)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_out):
+        (x,) = ctx.saved_tensors
+        B, C, h, w = x.shape
+        g_out = g_out.contiguous()
+        g_x = torch.empty_like(x)
+        with torch.cuda.device(x.device):
+            _lib.check(_lib.lib().gb_pose_shadow_bwd(B * C, h, w, g_out.shape[2], g_out.shape[3], _lib.ptr(x),
+                                                     ctx.beta, _lib.ptr(g_out), _lib.ptr(g_x),
+                                                     _lib.stream_ptr(x.device)), "pose_shadow_bwd")
+        return g_x, None, None
+
+
+def pose_shadow(x, beta, size):
+    """bilinear(sigmoid(x + beta) -> size x size, align_corners=False) for x [B, C, h, w]; two backward calls give the
+    same bits"""
+    return _PoseShadow.apply(x, beta, size)
+
+
+class PoseToShadow(nn.Module):
+    """ca_code/nn/shadow.py:429-471: the shadow map from the pose alone.  `fc_block` is a LinearWN (cuBLAS) +
+    LeakyReLU, `conv_block` five ConvTranspose2dWNUB (4^2 -> 128^2) on the fused layer kernels with the LeakyReLU in
+    their epilogue (`FusedLeakyReLU` keeps the reference's indices), and sigmoid(. + beta) with the resize to
+    `uv_size` one kernel each way (`pose_shadow`).  Keys and Glorot initialisation are the reference's."""
+
+    def __init__(self, n_pose_dims, uv_size, beta=1.0) -> None:
+        super().__init__()
+        self.n_pose_dims, self.uv_size = n_pose_dims, uv_size
+        self.fc_block = nn.Sequential(LinearWN(n_pose_dims, 256 * 4 * 4), nn.LeakyReLU(0.2))
+        layers = []
+        for cin, cout, size in ((256, 256, 8), (256, 128, 16), (128, 128, 32), (128, 64, 64)):
+            layer = ConvTranspose2dWNUB(cin, cout, size, size, 4, 2, 1)
+            layer.fused_slope = 0.2
+            layers += [layer, FusedLeakyReLU()]
+        self.conv_block = nn.Sequential(*layers, ConvTranspose2dWNUB(64, 1, 128, 128, 4, 2, 1))
+        self.beta = beta
+        self.apply(lambda m: glorot(m, 0.2))
+        glorot(self.conv_block[-1], 1.0)
+
+    def forward(self, pose: torch.Tensor):
+        if not pose.is_cuda:
+            raise RuntimeError("PoseToShadow runs on CUDA only (no CPU fallback): pose is on %s" % pose.device)
+        x = self.conv_block(self.fc_block(pose).reshape(-1, 256, 4, 4))
+        return {"shadow_map": pose_shadow(x, self.beta, self.uv_size)}

@@ -812,6 +812,33 @@ int gb_pixel_bias_fwd(int B, int C, int H, int W, int n_cams, int Hb, int Wb, co
 int gb_pixel_bias_bwd(int B, int C, int H, int W, int n_cams, int Hb, int Wb, const long long* idx, const float* g_out,
                       float* g_bias, void* stream);
 
+/* ---------------------------------------------------------------- drivable body (row R10, csrc/body_drive.cu) */
+
+/* replaces the last ConvTranspose2dWNUB of FaceDecoderFrontal.texmod and face.py:80-82 (ca_code/nn/face.py:58,78-82):
+ *   tex_raw = ConvTranspose2d(x, weight_v, k = 4, s = 2, p = 1) * scale[co] + bias      (scale = g / ||weight_v||_F)
+ *   tex     = 255 * (tex_raw + face_bias + 0.5)
+ * x [B,Cin,Hi,Wi] with Cin <= 32, weight_v [Cin,Cout,4,4] with Cout <= 4, scale [Cout], bias and face_bias
+ * [Cout,2Hi,2Wi]; tex_raw and tex [B,Cout,2Hi,2Wi] are each written once.  Forward only (the frame runs the face
+ * decoder under no_grad, mesh_vae_drivable.py:276-277). */
+int gb_face_tex_tail_fwd(int B, int Cin, int Cout, int Hi, int Wi, const float* x, const float* weight_v,
+                         const float* scale, const float* bias, const float* face_bias, float* tex_raw, float* tex,
+                         void* stream);
+/* replaces FaceEncoder's conditioning (ca_code/models/mesh_vae_drivable.py:721-724):
+ *   out[b,c] = (bilinear(x[b,c] [Hs,Ws] -> H x W, align_corners = False) / 255 - 0.5) * mask
+ * with torch's fp32 half-pixel source index, for any source size; x [B,C,Hs,Ws], mask [H,W], out [B,C,H,W].
+ * Forward only. */
+int gb_face_tex_cond_fwd(int B, int C, int Hs, int Ws, int H, int W, const float* x, const float* mask, float* out,
+                         void* stream);
+/* replaces PoseToShadow's sigmoid + resize (ca_code/nn/shadow.py:466-470):
+ *   out[n] = bilinear(sigmoid(x[n] + beta) [h,w] -> H x W, align_corners = False)
+ * x [N,h,w] (N = B * C planes), out [N,H,W]; torch's fp32 half-pixel index, the sigmoid evaluated at the taps. */
+int gb_pose_shadow_fwd(int N, int h, int w, int H, int W, const float* x, float beta, float* out, void* stream);
+/* the x gradient of the above: g_x [N,h,w] is WRITTEN, one thread per low-resolution texel, gathering its upsample
+ * footprint of g_out [N,H,W] in row-major order and multiplying by sigmoid' (no float atomics: the same bits on every
+ * call). */
+int gb_pose_shadow_bwd(int N, int h, int w, int H, int W, const float* x, float beta, const float* g_out, float* g_x,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif
