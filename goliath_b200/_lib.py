@@ -65,7 +65,9 @@ SIGNATURES = {
     "gb_rasterize_ranked_bwd": (_i, [_i, _i, _i] + [_vp] * 14 + [_vp]),
     "gb_rasterize_ranked_fwd_lists": (_i, [_i, _i, _i] + [_vp] * 10 + [_vp]),
     "gb_rasterize_ranked_bwd_lists": (_i, [_i, _i, _i] + [_vp] * 14 + [_vp]),
+    "gb_rasterize_ranked_fwd_sort_lists": (_i, [_i, _i, _i] + [_vp] * 12 + [_vp]),
     "gb_bin_tiles_ranked": (_i, [_i] + [_vp] * 7 + [_i, _i, _i, _i64] + [_vp, _vp, _i] + [_vp] * 6 + [_vp, _vp]),
+    "gb_bin_tiles_buckets": (_i, [_i] + [_vp] * 7 + [_i, _i, _i, _i64] + [_vp] * 8 + [_vp, _vp, _vp]),
     "gb_compute_raydirs_fwd": (_i, [_i, _i, _i] + [_vp] * 5 + [_f] + [_vp] * 3 + [_vp]),
     "gb_compute_raydirs_bwd": (_i, []),
     "gb_mvp_aabb_workspace_bytes": (_sz, [_i, _i]),

@@ -31,7 +31,11 @@
 //                            by the full key in place.  A tile with a run longer than kTieRun runs the passes over the
 //                            full key instead.  Longer buckets run the full-key passes chunk by chunk through global
 //                            memory (the bucket and the output array serve as the ping-pong pair, keys are gathered
-//                            by id).  The sorted ids overwrite the keys in the output array.
+//                            by id).  The sorted ids overwrite the keys in the output array.  The sort itself is
+//                            TileSort::sort_tile (csrc/splat_tile_sort.cuh).  gb_bin_tiles_buckets stops before this
+//                            kernel: the head step's forward (gb_rasterize_ranked_fwd_sort_lists) runs the same sort
+//                            in each blend CTA before it blends the tile, so a light tile's sort runs underneath a heavy
+//                            tile's blend instead of in a kernel of its own between the scatter and the blend.
 //   5. gather_records_kernel (packed callers only) the sorted 48-byte records, copied from the by-id table.
 //
 // Integer/byte work with a BIT-EXACT contract: gids_sorted, tile_bins and records are identical to the
@@ -39,6 +43,7 @@
 
 #include "common.cuh"
 #include "splat_record.cuh"
+#include "splat_tile_sort.cuh"
 
 #include <algorithm>
 
@@ -60,52 +65,17 @@ constexpr int kMaxSmemTiles = 20 * 1024;              // per-CTA tile counters (
 // the key sort of csrc/splat_bin.cu above it.
 constexpr int kMaxGaussians = 3 << 19;
 
-// Per-tile sort.  kSortCap = 5120 entries are sorted in registers + shared memory (10 per thread: 64 registers without
-// spills at two CTAs per SM).  The longest tile of the 300k-Gaussian bench head (1024x667, 16 ring cameras) holds
-// 4223 entries; the 2^20-Gaussian head (test_fullpath_gpu.py, ring camera 2) reaches 13754, and 300 to 444 of its
-// tiles (the counts above 6144 and above 4096) take the chunked path.
+// Per-tile sort (csrc/splat_tile_sort.cuh).  kSortCap = 5120 entries are sorted in registers + shared memory (10 per
+// thread: 64 registers without spills at two CTAs per SM).  The longest tile of the 300k-Gaussian bench head (1024x667,
+// 16 ring cameras) holds 4223 entries; the 2^20-Gaussian head (test_fullpath_gpu.py, ring camera 2) reaches 13754, and
+// 300 to 444 of its tiles (the counts above 6144 and above 4096) take the chunked path.
 constexpr int kSortThreads = 512;
-constexpr int kSortWarps = kSortThreads / 32;
-constexpr int kSortItems = 10;                        // entries per thread, at most
-constexpr int kSortCap = kSortThreads * kSortItems;
-constexpr int kDigitBits = 9;
-constexpr int kDigits = 1 << kDigitBits;              // == kSortThreads: thread t owns digit t in the scans
-static_assert(kDigits == kSortThreads, "one digit per thread");
-// Longest run of equal depth keys that one thread sorts by id in place after the depth passes.  The bench head's
-// tiles tie in ~70 % of tiles but in runs of at most 3 entries; a tile with a longer run re-sorts on the full key.
-constexpr int kTieRun = 16;
+using Sort = gbsort::TileSort<kSortThreads, 10>;
+constexpr int kSortCap = Sort::kCap;
+using gbsort::block_exclusive_scan;
 
 // Gaussians per CTA of tile_count_kernel: 2048 up to ~400k Gaussians, 4096 beyond (fewer counter flushes)
 inline int count_items(int G) { return G <= 2048 * 192 ? 2 : 4; }
-
-// exclusive prefix of v over the CTA (any multiple of 32 threads up to 1024); total = CTA sum
-__device__ __forceinline__ int block_exclusive_scan(int v, int* s_warp, int& total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int t = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += t;
-  }
-  if (lane == 31) s_warp[warp] = inc;
-  __syncthreads();
-  if (warp == 0) {
-    int w = (lane < (int)(blockDim.x >> 5)) ? s_warp[lane] : 0;
-    int winc = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int t = __shfl_up_sync(0xffffffffu, winc, o);
-      if (lane >= o) winc += t;
-    }
-    s_warp[lane] = winc - w;
-    if (lane == 31) s_warp[32] = winc;
-  }
-  __syncthreads();
-  total = s_warp[32];
-  const int r = s_warp[warp] + inc - v;
-  __syncthreads();
-  return r;
-}
 
 // tile rectangle of a Gaussian: same arithmetic as map_to_intersects_kernel (csrc/splat_bin.cu)
 __device__ __forceinline__ void tile_bbox(float cx, float cy, float radius, int tbx, int tby, int bw, int& x0,
@@ -355,257 +325,18 @@ __global__ void __launch_bounds__(kGaussBlock, 1) tile_scatter_kernel(
 }
 
 // ------------------------------------------------------------------ 4. per-tile sort by (depth, id)
-struct SortSmem {
-  unsigned short whist[kSortWarps][kDigits];  // per-warp digit counts, then their exclusive prefix over the warps
-  int base[kDigits];                          // scatter base of each digit
-  int run[kDigits];                           // chunked path: running base of each digit over the chunks
-  int warp[33];
-  unsigned red[4];                            // min / max of the depth keys and of the ids
-};
-
-// With ipt items per thread (ipt <= kSortItems), entry e of a chunk is held by warp e / (32 ipt), item (e / 32) % ipt,
-// lane e % 32: "earlier in the chunk" == (smaller warp, then smaller item, then smaller lane), which the per-warp
-// ranking below preserves.
-__device__ __forceinline__ int entry_of(int j, int ipt) {
-  return (threadIdx.x >> 5) * (32 * ipt) + j * 32 + (threadIdx.x & 31);
-}
-
-// item j of this thread is one of the m entries of the chunk
-__device__ __forceinline__ bool holds(int j, int ipt, int m) { return j < ipt && entry_of(j, ipt) < m; }
-
-// One stable counting pass on digit (key >> shift) & (kDigits - 1) over the m valid entries of a chunk held in
-// registers, ipt per thread: dst[j] = destination of item j.  whole: the chunk is the whole list (bases = exclusive
-// scan of this chunk's counts); else the bases come from s.run, which is advanced by this chunk's counts.
-__device__ __forceinline__ void radix_positions(const unsigned long long (&k)[kSortItems], int m, int ipt, int shift,
-                                                bool whole, SortSmem& s, int (&dst)[kSortItems]) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  // items held by this warp and by this thread: item j is valid iff j < mine
-  const int wbase = warp * (32 * ipt);
-  const int ours = min(ipt, max(0, (m - wbase + 31) >> 5)), mine = min(ipt, max(0, (m - wbase - lane + 31) >> 5));
-  for (int d = lane; d < kDigits; d += 32) s.whist[warp][d] = 0;
-  __syncwarp();
-#pragma unroll
-  for (int j = 0; j < kSortItems; ++j) {  // dst[j] = rank among the equal digits of this warp's earlier entries
-    dst[j] = 0;
-    if (j >= ours) continue;  // warp-uniform
-    const bool valid = j < mine;
-    const unsigned dgt = (unsigned)(k[j] >> shift) & (kDigits - 1);
-    // lanes holding the same digit: one ballot per digit bit (__match_any_sync serialises over the ~30 distinct
-    // digits a warp holds)
-    unsigned peers = __ballot_sync(0xffffffffu, valid);
-#pragma unroll
-    for (int b = 0; b < kDigitBits; ++b) {
-      const unsigned bal = __ballot_sync(0xffffffffu, (dgt >> b) & 1u);
-      peers &= ((dgt >> b) & 1u) ? bal : ~bal;
-    }
-    const unsigned lower = peers & ((1u << lane) - 1u);
-    unsigned prev = 0;
-    if (valid) prev = s.whist[warp][dgt];
-    __syncwarp();
-    dst[j] = (int)(prev + __popc(lower));
-    if (valid && lower == 0u) s.whist[warp][dgt] = (unsigned short)(prev + __popc(peers));
-    __syncwarp();
-  }
-  __syncthreads();
-  {
-    const int d = threadIdx.x;  // one digit per thread
-    int run = 0;
-#pragma unroll
-    for (int w = 0; w < kSortWarps; ++w) {
-      const int c = s.whist[w][d];
-      s.whist[w][d] = (unsigned short)run;
-      run += c;
-    }
-    int total;
-    if (whole) {
-      s.base[d] = block_exclusive_scan(run, s.warp, total);
-    } else {
-      const int b = s.run[d];
-      s.base[d] = b;
-      s.run[d] = b + run;
-    }
-  }
-  __syncthreads();
-#pragma unroll
-  for (int j = 0; j < kSortItems; ++j) {
-    const unsigned dgt = (unsigned)(k[j] >> shift) & (kDigits - 1);
-    dst[j] = (j < mine) ? s.base[dgt] + s.whist[warp][dgt] + dst[j] : -1;
-  }
-}
-
-// One pass of the shared-memory sort: the n keys (ipt per thread) go to s_key in digit order, and every thread
-// reloads its items from there.
-__device__ __forceinline__ void smem_pass(unsigned long long (&k)[kSortItems], int n, int ipt, int shift, SortSmem& s,
-                                          unsigned long long* s_key) {
-  int dst[kSortItems];
-  radix_positions(k, n, ipt, shift, true, s, dst);
-#pragma unroll
-  for (int j = 0; j < kSortItems; ++j)
-    if (dst[j] >= 0) s_key[dst[j]] = k[j];
-  __syncthreads();
-#pragma unroll
-  for (int j = 0; j < kSortItems; ++j)
-    if (holds(j, ipt, n)) k[j] = s_key[entry_of(j, ipt)];
-  // the next pass overwrites s_key only after the barriers inside radix_positions
-}
-
-__device__ __forceinline__ void minmax_to_smem(unsigned kmin, unsigned kmax, unsigned imin, unsigned imax, SortSmem& s) {
-  kmin = __reduce_min_sync(0xffffffffu, kmin);
-  kmax = __reduce_max_sync(0xffffffffu, kmax);
-  imin = __reduce_min_sync(0xffffffffu, imin);
-  imax = __reduce_max_sync(0xffffffffu, imax);
-  if ((threadIdx.x & 31) == 0) {
-    atomicMin(&s.red[0], kmin);
-    atomicMax(&s.red[1], kmax);
-    atomicMin(&s.red[2], imin);
-    atomicMax(&s.red[3], imax);
-  }
-}
-
-__device__ __forceinline__ int bits_of(unsigned span) { return span ? 32 - __clz((int)span) : 0; }
-
-// bucket: the tile's ids in arbitrary order and out: their depth keys at the same slots (tile_scatter_kernel); out
-// receives the same ids sorted by (depth key, id).  Both are [cap] arrays indexed by tile_bins.  The shared-memory path
-// reads every key and id of the tile before it writes out; the chunked path for buckets longer than kSortCap uses both
-// arrays as scratch, and so takes its keys from depth_keys[id].
+// One CTA per tile in launch order: Sort::sort_tile on the tile's bucket (ids) and output slots (depth keys in, sorted
+// ids out).
 __global__ void __launch_bounds__(kSortThreads, 2) tile_sort_kernel(const int* __restrict__ order,
                                                                     const int2* __restrict__ tile_bins,
                                                                     const unsigned* __restrict__ depth_keys,
                                                                     int* bucket, int* out) {
   extern __shared__ unsigned long long s_key[];  // kSortCap keys
-  __shared__ SortSmem s;
+  __shared__ Sort::Smem s;
   const int tile = order ? order[blockIdx.x] : (int)blockIdx.x;
   const int2 range = tile_bins[tile];
-  const int n = range.y - range.x;
-  if (n <= 0) return;  // uniform over the CTA
-  if (threadIdx.x == 0) {
-    s.red[0] = s.red[2] = 0xffffffffu;
-    s.red[1] = s.red[3] = 0u;
-  }
-  __syncthreads();
-
-  if (n <= kSortCap) {
-    const int ipt = (n + kSortThreads - 1) / kSortThreads;  // the tile spread over all warps
-    int id[kSortItems];
-    unsigned dk[kSortItems];
-#pragma unroll
-    for (int j = 0; j < kSortItems; ++j) {
-      const bool h = holds(j, ipt, n);
-      id[j] = h ? bucket[range.x + entry_of(j, ipt)] : -1;
-      dk[j] = h ? (unsigned)out[range.x + entry_of(j, ipt)] : 0u;
-    }
-    unsigned kmin = 0xffffffffu, kmax = 0u, imin = 0xffffffffu, imax = 0u;
-#pragma unroll
-    for (int j = 0; j < kSortItems; ++j) {
-      if (id[j] < 0) continue;
-      kmin = min(kmin, dk[j]); kmax = max(kmax, dk[j]);
-      imin = min(imin, (unsigned)id[j]); imax = max(imax, (unsigned)id[j]);
-    }
-    minmax_to_smem(kmin, kmax, imin, imax, s);
-    __syncthreads();
-    kmin = s.red[0];
-    imin = s.red[2];
-    const int bi = bits_of(s.red[3] - imin), bits = bits_of(s.red[1] - kmin) + bi;
-    unsigned long long k[kSortItems];
-#pragma unroll
-    for (int j = 0; j < kSortItems; ++j)
-      k[j] = ((unsigned long long)(dk[j] - kmin) << bi) | (unsigned long long)((unsigned)id[j] - imin);
-    // stable passes over the depth bits only: s_key ends in depth order, equal depth keys in bucket order
-    for (int shift = bi; shift < bits; shift += kDigitBits) smem_pass(k, n, ipt, shift, s, s_key);
-    if (bits == bi) {  // one depth key over the whole tile: no pass ran
-#pragma unroll
-      for (int j = 0; j < kSortItems; ++j)
-        if (holds(j, ipt, n)) s_key[entry_of(j, ipt)] = k[j];
-      __syncthreads();
-    }
-    // ties: find every run of equal depth keys (read only), then the thread holding its first entry sorts the run by
-    // id in place.  A run longer than kTieRun sends the whole tile through the passes on the full key instead.
-    static_assert(kTieRun < 32 && kSortItems * 5 <= 64, "run lengths are packed 5 bits per item");
-    unsigned long long runs = 0ull;  // 5 bits per item: length of the run it starts (0: none)
-    bool too_long = false;
-#pragma unroll
-    for (int j = 0; j < kSortItems; ++j) {
-      const int e = j * kSortThreads + threadIdx.x;
-      if (j >= ipt || e >= n) continue;
-      const unsigned long long d = s_key[e] >> bi;
-      if (e > 0 && (s_key[e - 1] >> bi) == d) continue;  // not the first entry of its run
-      int len = 1;
-      while (len <= kTieRun && e + len < n && (s_key[e + len] >> bi) == d) ++len;
-      if (len > kTieRun) too_long = true;
-      else runs |= (unsigned long long)len << (5 * j);
-    }
-    if (__syncthreads_or(too_long)) {
-#pragma unroll
-      for (int j = 0; j < kSortItems; ++j) k[j] = holds(j, ipt, n) ? s_key[entry_of(j, ipt)] : 0ull;
-      for (int shift = 0; shift < bits; shift += kDigitBits) smem_pass(k, n, ipt, shift, s, s_key);
-    } else {
-#pragma unroll
-      for (int j = 0; j < kSortItems; ++j) {
-        const int e = j * kSortThreads + threadIdx.x, len = (int)(runs >> (5 * j)) & 31;
-        for (int a = e + 1; a < e + len; ++a) {  // insertion sort of s_key[e, e + len)
-          const unsigned long long v = s_key[a];
-          int b = a;
-          for (; b > e && s_key[b - 1] > v; --b) s_key[b] = s_key[b - 1];
-          s_key[b] = v;
-        }
-      }
-      __syncthreads();
-    }
-    const unsigned long long imask = (1ull << bi) - 1ull;
-    for (int e = threadIdx.x; e < n; e += kSortThreads) out[range.x + e] = (int)(imin + (unsigned)(s_key[e] & imask));
-    return;
-  }
-
-  // ---- long bucket: the full-key passes chunk by chunk (kSortCap entries in registers at a time) through global memory,
-  // ids ping-ponging between bucket and out (each pass recomputes the keys from the ids); one CTA, slow but exact
-  {
-    unsigned kmin = 0xffffffffu, kmax = 0u, imin = 0xffffffffu, imax = 0u;
-    for (int i = threadIdx.x; i < n; i += kSortThreads) {
-      const int g = bucket[range.x + i];
-      const unsigned d = depth_keys[g];
-      kmin = min(kmin, d); kmax = max(kmax, d);
-      imin = min(imin, (unsigned)g); imax = max(imax, (unsigned)g);
-    }
-    minmax_to_smem(kmin, kmax, imin, imax, s);
-  }
-  __syncthreads();
-  const unsigned kmin = s.red[0], imin = s.red[2];
-  const int bi = bits_of(s.red[3] - imin), bits = bits_of(s.red[1] - kmin) + bi;
-  const unsigned long long imask = (1ull << bi) - 1ull;
-  auto key_of = [&](int g) {
-    return ((unsigned long long)(depth_keys[g] - kmin) << bi) | (unsigned long long)((unsigned)g - imin);
-  };
-  int* src = bucket + range.x;
-  int* dstp = out + range.x;
-  for (int shift = 0; shift < bits; shift += kDigitBits) {
-    // digit histogram of the whole bucket -> running bases
-    unsigned* s_cnt = reinterpret_cast<unsigned*>(s_key);
-    s_cnt[threadIdx.x] = 0u;
-    __syncthreads();
-    for (int i = threadIdx.x; i < n; i += kSortThreads)
-      atomicAdd(&s_cnt[(unsigned)(key_of(src[i]) >> shift) & (kDigits - 1)], 1u);
-    __syncthreads();
-    int total;
-    s.run[threadIdx.x] = block_exclusive_scan((int)s_cnt[threadIdx.x], s.warp, total);
-    __syncthreads();
-    for (int c0 = 0; c0 < n; c0 += kSortCap) {
-      const int m = min(kSortCap, n - c0);
-      unsigned long long k[kSortItems];
-#pragma unroll
-      for (int j = 0; j < kSortItems; ++j)
-        k[j] = holds(j, kSortItems, m) ? key_of(src[c0 + entry_of(j, kSortItems)]) : 0ull;
-      int dst[kSortItems];
-      radix_positions(k, m, kSortItems, shift, false, s, dst);
-#pragma unroll
-      for (int j = 0; j < kSortItems; ++j)
-        if (dst[j] >= 0) dstp[dst[j]] = (int)(imin + (unsigned)(k[j] & imask));
-      __syncthreads();  // s.whist / s.base are reused by the next chunk; global writes visible to the CTA
-    }
-    int* t = src; src = dstp; dstp = t;
-  }
-  if (src != out + range.x) {  // an even number of passes (or none) left the result in the bucket
-    for (int i = threadIdx.x; i < n; i += kSortThreads) out[range.x + i] = src[i];
-  }
+  if (range.y <= range.x) return;  // uniform over the CTA
+  Sort::sort_tile(range, depth_keys, bucket, out, s_key, s);
 }
 
 // Late colours (gb_bin_tiles_pack_ev with an event): tile_scatter leaves the colour quarter of the by-id records
@@ -712,7 +443,8 @@ static int bin_tiles_impl(int G, const float* xys, const float* depths, const in
                           const float* colors3, const float* opacity, const float* compensation, int img_h, int img_w,
                           int block_width, int64_t cap, int32_t* tile_bins, int32_t* tile_order, int tile_sched,
                           int32_t* gids_sorted, float* records, int32_t* n_out, int32_t* overflow, void* workspace,
-                          void* colors_ready, void* stream, int32_t* ext_ids, float* ext_rec, int32_t* ext_identity);
+                          void* colors_ready, void* stream, int32_t* ext_ids, float* ext_rec, int32_t* ext_identity,
+                          int32_t* ext_bucket);
 
 GB_API int gb_bin_tiles_pack_ev(int G, const float* xys, const float* depths, const int32_t* radii, const float* conics,
                                 const float* colors3, const float* opacity, const float* compensation, int img_h,
@@ -721,7 +453,7 @@ GB_API int gb_bin_tiles_pack_ev(int G, const float* xys, const float* depths, co
                                 void* workspace, void* colors_ready, void* stream) {
   return bin_tiles_impl(G, xys, depths, radii, conics, colors3, opacity, compensation, img_h, img_w, block_width, cap,
                         tile_bins, tile_order, tile_sched, gids_sorted, records, n_out, overflow, workspace, colors_ready,
-                        stream, nullptr, nullptr, nullptr);
+                        stream, nullptr, nullptr, nullptr, nullptr);
 }
 
 // Binning WITHOUT the sorted-record gather, for the blend kernels that stage records from the per-Gaussian table
@@ -737,14 +469,30 @@ GB_API int gb_bin_tiles_ranked(int G, const float* xys, const float* depths, con
   if (!ranks_sorted || !rec_by_rank || !rank_to_gid) return (int)cudaErrorInvalidValue;
   return bin_tiles_impl(G, xys, depths, radii, conics, colors3, opacity, compensation, img_h, img_w, block_width, cap,
                         tile_bins, tile_order, tile_sched, nullptr, nullptr, n_out, overflow, workspace, colors_ready, stream,
-                        ranks_sorted, rec_by_rank, rank_to_gid);
+                        ranks_sorted, rec_by_rank, rank_to_gid, nullptr);
+}
+
+// gb_bin_tiles_ranked up to the bucket scatter, for the forward that sorts each tile itself
+// (gb_rasterize_ranked_fwd_sort_lists): every tile's ids in arbitrary order in bucket [cap] and their 32-bit depth keys
+// at the same slots of ranks_keys [cap], which that forward overwrites with the sorted ids.  tile_bins, tile_order,
+// rec_by_rank, rank_to_gid, n_out and overflow as gb_bin_tiles_ranked.  One launch fewer than gb_bin_tiles_ranked.
+GB_API int gb_bin_tiles_buckets(int G, const float* xys, const float* depths, const int32_t* radii, const float* conics,
+                                const float* colors3, const float* opacity, const float* compensation, int img_h,
+                                int img_w, int block_width, int64_t cap, int32_t* tile_bins, int32_t* tile_order,
+                                int32_t* ranks_keys, int32_t* bucket, float* rec_by_rank, int32_t* rank_to_gid,
+                                int32_t* n_out, int32_t* overflow, void* workspace, void* colors_ready, void* stream) {
+  if (!ranks_keys || !bucket || !rec_by_rank || !rank_to_gid) return (int)cudaErrorInvalidValue;
+  return bin_tiles_impl(G, xys, depths, radii, conics, colors3, opacity, compensation, img_h, img_w, block_width, cap,
+                        tile_bins, tile_order, 0, nullptr, nullptr, n_out, overflow, workspace, colors_ready, stream,
+                        ranks_keys, rec_by_rank, rank_to_gid, bucket);
 }
 
 static int bin_tiles_impl(int G, const float* xys, const float* depths, const int32_t* radii, const float* conics,
                           const float* colors3, const float* opacity, const float* compensation, int img_h, int img_w,
                           int block_width, int64_t cap, int32_t* tile_bins, int32_t* tile_order, int tile_sched,
                           int32_t* gids_sorted, float* records, int32_t* n_out, int32_t* overflow, void* workspace,
-                          void* colors_ready, void* stream, int32_t* ext_ids, float* ext_rec, int32_t* ext_identity) {
+                          void* colors_ready, void* stream, int32_t* ext_ids, float* ext_rec, int32_t* ext_identity,
+                          int32_t* ext_bucket) {
   if (!gb_bin_tiles_supported(G) || block_width < 1 || cap < 0) return (int)cudaErrorInvalidValue;
   cudaStream_t s = (cudaStream_t)stream;
   const int tbx = gb::cdiv(img_w, block_width), tby = gb::cdiv(img_h, block_width);
@@ -754,7 +502,7 @@ static int bin_tiles_impl(int G, const float* xys, const float* depths, const in
   char* ws = (char*)workspace;
   int* counts = (int*)(ws + l.counts);
   int* cursor = (int*)(ws + l.cursor);
-  int* bucket = (int*)(ws + l.bucket);
+  int* bucket = ext_bucket ? ext_bucket : (int*)(ws + l.bucket);
   int4* rects = (int4*)(ws + l.rects);
   const bool ranked = ext_ids != nullptr;  // outputs for the blend that stages records by id: no sorted-record gather
   float4* rec_by_id = ranked ? (float4*)ext_rec : (float4*)(ws + l.rec_by_id);
@@ -801,9 +549,12 @@ static int bin_tiles_impl(int G, const float* xys, const float* depths, const in
   tile_scatter_kernel<<<gb::cdiv(G, per_cta), kGaussBlock, scat_smem, s>>>(
       G, rects, (const float2*)xys, conics, late ? nullptr : colors3, depths, opacity, compensation, tbx, (long long)cap,
       per_cta, smem_tiles, stage_cap, cursor, bucket, (unsigned*)ids_sorted, rec_by_id);
-  tile_sort_kernel<<<T, kSortThreads, sort_smem, s>>>(tile_order, (const int2*)tile_bins, (const unsigned*)depths, bucket,
-                                                      ids_sorted);
-  gb::count_launches(2);
+  gb::count_launches(1);
+  if (!ext_bucket) {  // else the caller's forward sorts each bucket
+    tile_sort_kernel<<<T, kSortThreads, sort_smem, s>>>(tile_order, (const int2*)tile_bins, (const unsigned*)depths, bucket,
+                                                        ids_sorted);
+    gb::count_launches(1);
+  }
   if (late) {
     GB_CUDA(cudaStreamWaitEvent(s, (cudaEvent_t)colors_ready, 0));
     rec_colors_kernel<<<gb::cdiv(G, 256), 256, 0, s>>>(G, radii, colors3, depths, rec_by_id);

@@ -31,6 +31,7 @@
 
 #include "common.cuh"
 #include "splat_blend_common.cuh"
+#include "splat_tile_sort.cuh"
 
 namespace {
 
@@ -120,19 +121,55 @@ __device__ __forceinline__ Tile make_tile(int tile_id, int tbx) {
 //               and writes hit_count[8 tile + w] = the number of leading entries the backward needs: up to and
 //               including the last hit any pixel of the warp blended (the backward's `idx <= final_idx` walk).  Block 0
 //               sets hit_count[8T], the backward's draw counter, to zero.  Only stores are added: pixels stay identical.
-template <int C, bool LIST, bool RANKED, bool HITS = false>
-__global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
+// SORT (with LIST, RANKED and HITS): the CTA first sorts its tile's bucket by (depth, id) with all its threads
+//               (FwdSort::sort_tile, the algorithm of the binning's tile_sort_kernel): bucket holds the tile's ids in
+//               arbitrary order and `sorted` their depth keys at the same slots (gb_bin_tiles_buckets); `sorted`
+//               receives the ids in blend order, the array the backward's hit lists index, and the producer stages from
+//               it.  The sort's buffers alias the stage ring and the hit lists, which are not live before the blend.
+//               Pixels and hit lists are those of the HITS variant run on tile_sort_kernel's output.
+// 15 entries per thread: the longest tile of the bench head (4223 entries) stays in shared memory; longer tiles take the
+// chunked path through global memory inside the CTA.
+using FwdSort = gbsort::TileSort<kFwdThreads, 15>;
+
+template <bool LIST>
+struct FwdRing {
+  float4 rec[kFwdStages][kStageRecs * 3];
+  int hits[LIST ? kPixelWarps : 1][LIST ? kStageRecs + 4 : 4];
+};
+template <bool LIST, bool SORT>
+struct FwdSmem {
+  FwdRing<LIST> f;
+};
+template <bool LIST>
+struct FwdSmem<LIST, true> {
+  union {
+    FwdRing<LIST> f;
+    struct {
+      unsigned long long key[FwdSort::kCap];
+      FwdSort::Smem s;
+    } sort;
+  };
+};
+
+template <int C, bool LIST, bool RANKED, bool HITS, bool SORT>
+__device__ __forceinline__ void blend_fwd_body(
     int img_w, int img_h, int tbx, const int* order, int sched, const int2* __restrict__ tile_bins,
     const float4* __restrict__ rec /* RANKED: the by-rank table */, const int* __restrict__ ranks /* RANKED only */,
     const float* __restrict__ background, float* __restrict__ final_Ts, int* __restrict__ final_idx,
-    float* __restrict__ out_img, int* __restrict__ hit_list = nullptr, int* __restrict__ hit_count = nullptr) {
+    float* __restrict__ out_img, int* __restrict__ hit_list, int* __restrict__ hit_count,
+    const unsigned* __restrict__ depth_keys /* SORT only */, int* bucket /* SORT only */,
+    int* sorted /* SORT only: depth keys in, ids in blend order out */) {
   static_assert(!HITS || LIST, "hit lists are the LIST variant's per-stage lists");
-  __shared__ __align__(128) float4 s_rec[kFwdStages][kStageRecs * 3];
+  static_assert(!SORT || (LIST && RANKED && HITS), "the sorting forward is the ranked hit-list forward");
+  __shared__ __align__(128) FwdSmem<LIST, SORT> sm;
+  float4 (&s_rec)[kFwdStages][kStageRecs * 3] = sm.f.rec;
+  auto& s_hits = sm.f.hits;
   __shared__ __align__(8) unsigned long long s_full[kFwdStages];
   __shared__ __align__(8) unsigned long long s_empty[kFwdStages];
   __shared__ int s_ndone;  // pixel warps whose 32 pixels are saturated
   __shared__ int s_tile;
-  __shared__ __align__(16) int s_hits[LIST ? kPixelWarps : 1][LIST ? kStageRecs + 4 : 4];
+  // SORT: the ids are read back from `sorted`, which this CTA has just written (plain loads, not the read-only path)
+  const int* rk = SORT ? sorted : ranks;
 
   const int tr = threadIdx.x, lane = tr & 31, warp = tr >> 5;
   if (tr == 0) {
@@ -145,10 +182,13 @@ __global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
     s_ndone = 0;
     fence_mbar_init();
   }
-  __syncthreads();  // the only CTA-wide barrier of this kernel
+  __syncthreads();  // the only CTA-wide barrier of this kernel besides the sort's
   if (s_tile < 0) return;
   const Tile tl = make_tile(s_tile, tbx);
   const int2 range = tile_bins[tl.tile_id];
+  if constexpr (SORT) {
+    if (range.y > range.x) FwdSort::sort_tile(range, depth_keys, bucket, sorted, sm.sort.key, sm.sort.s);
+  }
   const int num_batches = (range.y - range.x + kStageRecs - 1) / kStageRecs;
 
   if (RANKED && warp == kPixelWarps) {  // --------------------- producer warp, all lanes: gathers by rank
@@ -160,7 +200,7 @@ __global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
       const int start = range.x + b * kStageRecs;
       const int count = min(kStageRecs, range.y - start);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) r[k] = (b < num_batches && lane + 32 * k < count) ? ranks[start + lane + 32 * k] : -1;
+      for (int k = 0; k < 4; ++k) r[k] = (b < num_batches && lane + 32 * k < count) ? rk[start + lane + 32 * k] : -1;
     };
     load_ranks(0);
     for (int b = 0; b < num_batches; ++b) {
@@ -387,6 +427,29 @@ __global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
       out_img[pix * 3 + 2] = acc[2] + T * background[2];
     }
   }
+}
+
+template <int C, bool LIST, bool RANKED, bool HITS = false>
+__global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
+    int img_w, int img_h, int tbx, const int* order, int sched, const int2* __restrict__ tile_bins,
+    const float4* __restrict__ rec, const int* __restrict__ ranks, const float* __restrict__ background,
+    float* __restrict__ final_Ts, int* __restrict__ final_idx, float* __restrict__ out_img,
+    int* __restrict__ hit_list = nullptr, int* __restrict__ hit_count = nullptr) {
+  blend_fwd_body<C, LIST, RANKED, HITS, false>(img_w, img_h, tbx, order, sched, tile_bins, rec, ranks, background,
+                                               final_Ts, final_idx, out_img, hit_list, hit_count, nullptr, nullptr,
+                                               nullptr);
+}
+
+// The sorting forward.  The sort's 15 keys per thread need more than the 56 registers of four CTAs per SM: three CTAs
+// (72 registers, 864 threads) hold 396 tiles at a time.
+template <int C>
+__global__ void __launch_bounds__(kFwdThreads, 3) blend_fwd_sort_kernel(
+    int img_w, int img_h, int tbx, const int* order, const int2* __restrict__ tile_bins, const float4* __restrict__ rec,
+    const float* __restrict__ background, float* __restrict__ final_Ts, int* __restrict__ final_idx,
+    float* __restrict__ out_img, int* __restrict__ hit_list, int* __restrict__ hit_count,
+    const unsigned* __restrict__ depth_keys, int* bucket, int* sorted) {
+  blend_fwd_body<C, true, true, true, true>(img_w, img_h, tbx, order, 0, tile_bins, rec, nullptr, background, final_Ts,
+                                            final_idx, out_img, hit_list, hit_count, depth_keys, bucket, sorted);
 }
 
 // ------------------------------------------------------------------ backward
@@ -1475,6 +1538,24 @@ static int launch_fwd_any(int img_h, int img_w, int channels, const int32_t* til
   return 0;
 }
 
+// the sorting forward (SORT): gb_rasterize_ranked_fwd_sort_lists
+static int launch_fwd_sort(int img_h, int img_w, int channels, const int32_t* tile_bins, const int32_t* tile_order,
+                           const float* depths, int32_t* bucket, int32_t* ranks, const float* records,
+                           const float* background, float* out_img, float* final_Ts, int32_t* final_idx,
+                           int32_t* hit_list, int32_t* hit_count, cudaStream_t s) {
+  const int tbx = gb::cdiv(img_w, 16), tby = gb::cdiv(img_h, 16);
+#define GB_FWD_SORT(CC)                                                                                                 \
+  blend_fwd_sort_kernel<CC><<<tbx * tby, kFwdThreads, 0, s>>>(img_w, img_h, tbx, tile_order, (const int2*)tile_bins,     \
+                                                            (const float4*)records, background, final_Ts, final_idx,    \
+                                                            out_img, hit_list, hit_count, (const unsigned*)depths,      \
+                                                            bucket, ranks)
+  if (channels == 3) GB_FWD_SORT(3); else GB_FWD_SORT(4);
+#undef GB_FWD_SORT
+  gb::count_launches(1);
+  GB_CHECK_LAUNCH();
+  return 0;
+}
+
 static int launch_bwd_any(int img_h, int img_w, int channels, const int32_t* gids_sorted, const int32_t* ranks,
                           const int32_t* tile_bins, const int32_t* tile_order, int sched, const float* records,
                           const float* background, const float* final_Ts, const int32_t* final_idx, const float* v_output,
@@ -1593,6 +1674,22 @@ GB_API int gb_rasterize_ranked_fwd_lists(int img_h, int img_w, int channels, con
   if ((channels != 3 && channels != 4) || !ranks_sorted || !hit_list || !hit_count) return (int)cudaErrorInvalidValue;
   return gbblend::launch_fwd_any(img_h, img_w, channels, tile_bins, tile_order, 0, rec_by_rank, ranks_sorted, background,
                                  out_img, final_Ts, final_idx, (cudaStream_t)stream, hit_list, hit_count);
+}
+// gb_rasterize_ranked_fwd_lists on the unsorted buckets of gb_bin_tiles_buckets: each CTA sorts its tile's bucket
+// (ids) by (depth key, id) before it blends, writing the sorted ids over the depth keys in ranks_keys [cap]: the same
+// ranks_sorted as gb_bin_tiles_ranked's, read by the backward.  depths [G] are the depth keys the chunked path of tiles
+// longer than the in-CTA sort's capacity reads by id.  Outputs identical to gb_bin_tiles_ranked +
+// gb_rasterize_ranked_fwd_lists.
+GB_API int gb_rasterize_ranked_fwd_sort_lists(int img_h, int img_w, int channels, const int32_t* tile_bins,
+                                              const int32_t* tile_order, const float* depths, int32_t* bucket,
+                                              int32_t* ranks_keys, const float* rec_by_rank, const float* background,
+                                              float* out_img, float* final_Ts, int32_t* final_idx, int32_t* hit_list,
+                                              int32_t* hit_count, void* stream) {
+  if (img_h <= 0 || img_w <= 0) return 0;
+  if ((channels != 3 && channels != 4) || !depths || !bucket || !ranks_keys || !hit_list || !hit_count)
+    return (int)cudaErrorInvalidValue;
+  return gbblend::launch_fwd_sort(img_h, img_w, channels, tile_bins, tile_order, depths, bucket, ranks_keys, rec_by_rank,
+                                  background, out_img, final_Ts, final_idx, hit_list, hit_count, (cudaStream_t)stream);
 }
 GB_API int gb_rasterize_ranked_bwd_lists(int img_h, int img_w, int channels, const int32_t* ranks_sorted,
                                          const int32_t* tile_bins, const int32_t* hit_list, int32_t* hit_count,

@@ -79,8 +79,8 @@ def _blend_plan(T, schedule=True):
 def _bin_tiles(xys, depths, radii, conics, colors, opacity, comp, H, W, cap, plan, outs, ranked=False, n_out=None,
                colors_ready=None):
     """Bucket binning (csrc/splat_bin_tiles.cu) on the current stream, into the caller's `outs`: (gids [cap], records
-    [cap,12]) for gb_bin_tiles_pack_ev, or with `ranked` (ranks [cap], records [G,12], gids [G]) for
-    gb_bin_tiles_ranked.  `n_out` (device int32) receives the intersection count, `colors_ready` is the raw handle of
+    [cap,12]) for gb_bin_tiles_pack_ev, or with `ranked` (ranks [cap], bucket [cap], records [G,12], gids [G]) for
+    gb_bin_tiles_buckets, which leaves each tile unsorted for gb_rasterize_ranked_fwd_sort_lists.  `n_out` (device int32) receives the intersection count, `colors_ready` is the raw handle of
     an event to wait for before the colours are read; either may be None.  Returns (bins [T,2], order)."""
     G = xys.size(0)
     dev = xys.device
@@ -91,11 +91,13 @@ def _bin_tiles(xys, depths, radii, conics, colors, opacity, comp, H, W, cap, pla
     order = torch.empty(plan.order_len, device=dev, dtype=torch.int32)
     ws = _workspace(dev, L.gb_bin_tiles_workspace_bytes(G, T, cap))
     with torch.cuda.device(dev):
-        _lib.check((L.gb_bin_tiles_ranked if ranked else L.gb_bin_tiles_pack_ev)(
-            G, _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(colors), _lib.ptr(opacity),
-            _lib.ptr(comp), H, W, 16, cap, _lib.ptr(bins), _lib.ptr(order), plan.sched, *map(_lib.ptr, outs),
-            _lib.ptr(n_out), _lib.ptr(_overflow_flag(dev)), _lib.ptr(ws), colors_ready, _lib.stream_ptr(dev)),
-            "bin_tiles_ranked" if ranked else "bin_tiles_pack")
+        args = (G, _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(colors),
+                _lib.ptr(opacity), _lib.ptr(comp), H, W, 16, cap, _lib.ptr(bins), _lib.ptr(order))
+        tail = (_lib.ptr(n_out), _lib.ptr(_overflow_flag(dev)), _lib.ptr(ws), colors_ready, _lib.stream_ptr(dev))
+        if ranked:  # launch-order tiles (the ranked plan never takes the SM-affine schedule)
+            _lib.check(L.gb_bin_tiles_buckets(*args, *map(_lib.ptr, outs), *tail), "bin_tiles_buckets")
+        else:
+            _lib.check(L.gb_bin_tiles_pack_ev(*args, plan.sched, *map(_lib.ptr, outs), *tail), "bin_tiles_pack")
     return bins, order
 
 
@@ -283,9 +285,10 @@ class _BinBlend(Function):
         # from the by-id table, the sorted 48-byte records are never materialised (csrc/splat_blend_mom.cu, RANKED)
         if plan.ranked:
             gids = torch.empty(G, **i32)            # identity (the C ABI's rank_to_gid)
-            ranks = torch.empty(cap, **i32)         # per tile: Gaussian ids in blend order
+            ranks = torch.empty(cap, **i32)         # per tile: depth keys, then (after the forward) ids in blend order
+            bucket = torch.empty(cap, **i32)        # per tile: Gaussian ids in arbitrary order
             records = torch.empty(G, 12, **f32)     # one record per Gaussian, by id
-            outs = (ranks, records, gids)
+            outs = (ranks, bucket, records, gids)
         else:
             gids = torch.empty(cap, **i32)
             ranks = gids  # unused
@@ -297,14 +300,15 @@ class _BinBlend(Function):
         with torch.cuda.device(dev):
             st = _lib.stream_ptr(dev)
             if plan.ranked:
-                # the forward stores each pixel warp's hits (sorted indices; 8 x cap int32 needs no device-side count)
-                # so that the backward walks them instead of culling every tile again
+                # each forward CTA sorts its tile's bucket into `ranks` before it blends the tile, and stores each
+                # pixel warp's hits (sorted indices; 8 x cap int32 needs no device-side count) so that the backward
+                # walks them instead of culling every tile again
                 hit_list = torch.empty(8 * cap, **i32)
                 hit_count = torch.empty(16 * tb[0] * tb[1] + 2, **i32)
-                _lib.check(L.gb_rasterize_ranked_fwd_lists(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(ranks),
-                                                           _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(out4),
-                                                           _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(hit_list),
-                                                           _lib.ptr(hit_count), st), "rasterize_ranked_forward")
+                _lib.check(L.gb_rasterize_ranked_fwd_sort_lists(
+                    H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(depths), _lib.ptr(bucket), _lib.ptr(ranks),
+                    _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(out4), _lib.ptr(final_Ts), _lib.ptr(final_idx),
+                    _lib.ptr(hit_list), _lib.ptr(hit_count), st), "rasterize_ranked_forward")
             else:
                 _lib.check(plan.fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4),
                                     _lib.ptr(out4), _lib.ptr(final_Ts), _lib.ptr(final_idx), st),

@@ -234,6 +234,23 @@ int gb_rasterize_ranked_bwd_lists(int img_h, int img_w, int channels, const int3
                                   const float* v_output_alpha, float* v_xy, float* v_conic, float* v_colors,
                                   float* v_opacity, void* stream);
 
+/* The head step's pair: gb_bin_tiles_buckets is gb_bin_tiles_ranked (launch-order tiles) without the per-tile sort: it
+ * leaves each tile's Gaussian ids in arbitrary order in bucket [cap] int32 and their 32-bit depth keys at the same
+ * slots of ranks_keys [cap] int32.  gb_rasterize_ranked_fwd_sort_lists sorts each tile's bucket by (depth key, id) in
+ * the CTA that then blends it, writes the sorted ids over ranks_keys (then identical to gb_bin_tiles_ranked's
+ * ranks_sorted) and gives gb_rasterize_ranked_fwd_lists' out_img, final_Ts, final_idx, hit_list and hit_count.
+ * depths [G] are the same depths the binning took.  gb_rasterize_ranked_bwd_lists runs on the result unchanged. */
+int gb_bin_tiles_buckets(int G, const float* xys, const float* depths, const int32_t* radii, const float* conics,
+                         const float* colors3, const float* opacity, const float* compensation, int img_h, int img_w,
+                         int block_width, int64_t cap, int32_t* tile_bins, int32_t* tile_order, int32_t* ranks_keys,
+                         int32_t* bucket, float* rec_by_rank, int32_t* rank_to_gid, int32_t* n_out, int32_t* overflow,
+                         void* workspace, void* colors_ready, void* stream);
+int gb_rasterize_ranked_fwd_sort_lists(int img_h, int img_w, int channels, const int32_t* tile_bins,
+                                       const int32_t* tile_order, const float* depths, int32_t* bucket,
+                                       int32_t* ranks_keys, const float* rec_by_rank, const float* background,
+                                       float* out_img, float* final_Ts, int32_t* final_idx, int32_t* hit_list,
+                                       int32_t* hit_count, void* stream);
+
 /* launch order of the tiles, longest list first: order [T] int32 */
 int gb_tile_order(int num_tiles, const int32_t* tile_bins, int32_t* order, void* stream);
 
