@@ -150,6 +150,7 @@ SIGNATURES = {
     "gb_face_tex_cond_fwd": (_i, [_i] * 6 + [_vp] * 3 + [_vp]),
     "gb_pose_shadow_fwd": (_i, [_i] * 5 + [_vp, _f, _vp, _vp]),
     "gb_pose_shadow_bwd": (_i, [_i] * 5 + [_vp, _f, _vp, _vp, _vp]),
+    "gb_head_lights_fwd": (_i, [_i] * 3 + [_vp] * 11 + [_vp]),
 }
 
 

@@ -112,10 +112,10 @@ def sample_uv(values_uv: torch.Tensor, uv_coords: torch.Tensor, v2uv=None) -> to
 
 class GeometryModule(torch.nn.Module):
     """The part of the reference's GeometryModule (geom.py:186-278) the decoders use: `vn(verts)`, `to_uv(values)` and,
-    given vt [N_uv,2] and v2uv [V,n_max], `from_uv(values_uv)`.  vi [F,3]; index_image / bary_image [U,U,3] are the
-    reference's precomputed assets.  vti [F,3], face_index_image [U,U] and valid_mask [U,U,1] are registered only when
-    given, so a full module holds the reference's eight buffers (a checkpoint's `geo_fn.*` keys load strictly) and
-    the smaller holders keep their keys."""
+    given vt [N_uv,2] (and optionally v2uv [V,n_max]), `from_uv(values_uv)`.  vi [F,3]; index_image / bary_image
+    [U,U,3] are the reference's precomputed assets.  vt, v2uv, vti [F,3], face_index_image [U,U] and valid_mask
+    [U,U,1] are each registered only when given, so a full module holds the reference's eight buffers (seven for the
+    head, which has no v2uv), a checkpoint's `geo_fn.*` keys load strictly, and the smaller holders keep their keys."""
 
     def __init__(self, vi: torch.Tensor, index_image: torch.Tensor, bary_image: torch.Tensor, vt=None, v2uv=None,
                  vti=None, face_index_image=None, valid_mask=None):
@@ -125,6 +125,7 @@ class GeometryModule(torch.nn.Module):
         self.register_buffer("bary_image", torch.as_tensor(bary_image).to(torch.float32))
         if vt is not None:
             self.register_buffer("vt", torch.as_tensor(vt).to(torch.float32))
+        if v2uv is not None:
             self.register_buffer("v2uv", torch.as_tensor(v2uv).to(torch.int32))
         if vti is not None:
             self.register_buffer("vti", torch.as_tensor(vti).to(torch.int32))
@@ -135,14 +136,17 @@ class GeometryModule(torch.nn.Module):
         self._uv_table, self._uv_key = None, None
 
     def from_uv(self, values_uv):
-        """geom.py:273-275: sample_uv(values_uv, vt, v2uv) with the gather table built once per (buffers, map size)"""
+        """geom.py:273-275: sample_uv(values_uv, vt, v2uv) with the gather table built once per (buffers, map size);
+        one row per UV coordinate when the module has no v2uv"""
         from .seams import gather
 
         _lib.check_input(values_uv, "values_uv")
         H, W = values_uv.shape[2], values_uv.shape[3]
-        key = (self.vt.device, self.vt.data_ptr(), self.vt._version, self.v2uv.data_ptr(), self.v2uv._version, H, W)
+        v2uv = getattr(self, "v2uv", None)
+        key = (self.vt.device, self.vt.data_ptr(), self.vt._version, None if v2uv is None else v2uv.data_ptr(),
+               None if v2uv is None else v2uv._version, H, W)
         if self._uv_key != key:
-            self._uv_table, self._uv_key = sample_uv_table(self.vt, self.v2uv, H, W), key
+            self._uv_table, self._uv_key = sample_uv_table(self.vt, v2uv, H, W), key
         return gather(values_uv, self._uv_table, rows_last=True)
 
     def vn(self, verts):

@@ -10,7 +10,10 @@
   2 pi norm_scale[0] (the reference's quirk: item 0's scale for the whole batch) and the constant light positions are
   torch ops on device tensors.  With a fixed batch size the frame can be captured in a CUDA graph.
 
-The dict handed to `mod` has the reference's keys, shapes and dtypes."""
+The dict handed to `mod` has the reference's keys, shapes and dtypes.
+
+`SingleLightCycleDecorator` (light_decorator.py:167-218) is host-side, as in the reference: one unit point light per
+item on a circle of radius 1100 around the head, read from the head translation on the host."""
 import ctypes
 
 import cv2
@@ -142,5 +145,52 @@ class EnvSpinDecorator(th.nn.Module):
         data["envbg"] = envbg.to(device)
         data["light_type"] = "envmap"
         data["n_lights"] = light_intensity.shape[1] * th.ones(batch_size, 1, device=device)
+        data["is_fullylit_frame"] = th.zeros(1, device=device)
+        return self.mod(**data)
+
+
+def single_light_position(index, cycle, light_rotate_axis, trans=None):
+    """light_decorator.py:185-208: the float32 [3] light position of frame `index` on a circle of radius 1100 about
+    axis 0 (the y-z plane), 1 (x-z at height 300, then rescaled to 1100) or any other value (x-y), plus `trans`"""
+    index = index % cycle
+    angle = (abs(index) / cycle) * 2 * np.pi
+    if light_rotate_axis == 0:
+        lpos = np.asarray([0.0, 1100.0 * np.sin(angle), 1100.0 * np.cos(angle)]).astype(np.float32)
+    elif light_rotate_axis == 1:
+        lpos = np.asarray([-1.0 * 1100.0 * np.sin(angle), 300.0, 1100.0 * np.cos(angle)]).astype(np.float32)
+    else:
+        lpos = np.asarray([1100.0 * np.cos(angle), 1100.0 * np.sin(angle), 0.0]).astype(np.float32)
+    lpos = 1100.0 * lpos / np.linalg.norm(lpos)
+    if trans is not None:
+        lpos += trans
+    return lpos
+
+
+class SingleLightCycleDecorator(th.nn.Module):
+    """Sets one unit-intensity point light per item, cycling with data["index"] (cycle frames per turn), and
+    n_lights = 1: light_intensity [B,1,1], light_pos [B,1,3] (head_pose[:, :3, 3] or pose[:, :3] added, read on the
+    host), n_lights [B] int32, is_fullylit_frame [1]."""
+
+    def __init__(self, mod: th.nn.Module, cycle: int = 256, light_rotate_axis: int = 0) -> None:
+        super().__init__()
+        self.mod = mod
+        self.cycle = cycle
+        self.light_rotate_axis = light_rotate_axis
+
+    def forward(self, **data):
+        device = data["campos"].device
+        batch_size = data["campos"].size(0)
+        trans = None
+        if "head_pose" in data:
+            trans = data["head_pose"][:, :3, 3].detach().cpu().numpy()
+        elif "pose" in data:
+            trans = data["pose"][:, :3].detach().cpu().numpy()
+        index = data["index"]
+        index = index.tolist() if th.is_tensor(index) else list(index)
+        pos = np.stack([single_light_position(index[i], self.cycle, self.light_rotate_axis,
+                                              None if trans is None else trans[i]) for i in range(batch_size)])
+        data["light_intensity"] = th.ones(batch_size, 1, 1, device=device)
+        data["light_pos"] = th.from_numpy(pos).float().to(device)[:, None]
+        data["n_lights"] = th.ones(batch_size, device=device).int()
         data["is_fullylit_frame"] = th.zeros(1, device=device)
         return self.mod(**data)

@@ -467,22 +467,23 @@ def _get(obj, name, default=None):
     return getattr(obj, name, default)
 
 
-def _uv_geometry(assets):
-    """the frame's GeometryModule from `assets.topology` and the four UV images the assets must carry at 1024 x 1024;
-    returns (geo_fn, {name: image})"""
+def _uv_geometry(assets, with_v2uv=True, size=1024):
+    """the frame's GeometryModule from `assets.topology` and the four UV images the assets must carry at size x size
+    (the head's module has no v2uv: with_v2uv=False); returns (geo_fn, {name: image})"""
     from .geom import GeometryModule
 
     missing = [k for k in UV_IMAGES if _get(assets, k) is None]
     if missing:
-        raise ValueError("AutoEncoder: assets must carry the UV images %s at 1024 x 1024 (the reference's "
-                         "geo_fn.* buffers); missing: %s" % (", ".join(UV_IMAGES), ", ".join(missing)))
+        raise ValueError("AutoEncoder: assets must carry the UV images %s at %d x %d (the reference's "
+                         "geo_fn.* buffers); missing: %s" % (", ".join(UV_IMAGES), size, size, ", ".join(missing)))
     uv = {k: torch.as_tensor(np.asarray(_get(assets, k))) for k in UV_IMAGES}
     for k, t in uv.items():
-        if tuple(t.shape[:2]) != (1024, 1024):
-            raise ValueError("AutoEncoder: assets.%s must be 1024 x 1024 (got %s)" % (k, tuple(t.shape)))
+        if tuple(t.shape[:2]) != (size, size):
+            raise ValueError("AutoEncoder: assets.%s must be %d x %d (got %s)" % (k, size, size, tuple(t.shape)))
     topo = _get(assets, "topology")
-    geo_fn = GeometryModule(_get(topo, "vi"), uv["index_image"], uv["bary_image"], vt=_get(topo, "vt"),
-                            v2uv=_get(topo, "v2uv"), vti=_get(topo, "vti"), face_index_image=uv["face_index_image"],
+    v2uv = _get(topo, "v2uv") if with_v2uv else None
+    geo_fn = GeometryModule(_get(topo, "vi"), uv["index_image"], uv["bary_image"], vt=_get(topo, "vt"), v2uv=v2uv,
+                            vti=_get(topo, "vti"), face_index_image=uv["face_index_image"],
                             valid_mask=uv["valid_mask"])
     return geo_fn, uv
 

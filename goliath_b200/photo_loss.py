@@ -169,7 +169,9 @@ class CalV5(torch.nn.Module):
     def name_to_idx(self, cam_names) -> torch.Tensor:
         return _indices_to_device(self.holder.to_idx(cam_names), self.holder.params.device)
 
-    def forward(self, image: torch.Tensor, cam_idxs: torch.Tensor) -> torch.Tensor:
+    def rows(self, cam_idxs: torch.Tensor):
+        """post_render's calibration arguments for the cameras `cam_idxs`: (cal_w, cal_b) [B,3] and grey [B] int32,
+        with the training gradient scale hooked onto the gathered rows"""
         params = self.holder.params[cam_idxs]
         ident = cam_idxs == self.identity_idx
         grey = self.grey_mask[cam_idxs] & ~ident
@@ -178,7 +180,11 @@ class CalV5(torch.nn.Module):
             params.register_hook(lambda g: g * scale[:, None])
         w = torch.where(ident[:, None], 1.0, params[:, :3])
         b = torch.where(ident[:, None], 0.0, params[:, 3:])
-        return post_render(image, cal_w=w, cal_b=b, grey=grey.to(torch.int32))
+        return w, b, grey.to(torch.int32)
+
+    def forward(self, image: torch.Tensor, cam_idxs: torch.Tensor) -> torch.Tensor:
+        w, b, grey = self.rows(cam_idxs)
+        return post_render(image, cal_w=w, cal_b=b, grey=grey)
 
 
 class LearnableBlur(torch.nn.Module):
@@ -196,6 +202,9 @@ class LearnableBlur(torch.nn.Module):
     def reg(self, cameras):
         return self.weights_raw[self.name_to_idx(cameras)]
 
+    def weights(self, cameras) -> torch.Tensor:
+        """post_render's blur weights [B,3] for `cameras`: softmax(weights_raw[camera])"""
+        return torch.softmax(self.weights_raw[self.name_to_idx(cameras)], dim=-1)
+
     def forward(self, img: torch.Tensor, cameras) -> torch.Tensor:
-        weights = torch.softmax(self.weights_raw[self.name_to_idx(cameras)], dim=-1)
-        return post_render(img, blur_weights=weights)
+        return post_render(img, blur_weights=self.weights(cameras))

@@ -856,6 +856,24 @@ int gb_pose_shadow_fwd(int N, int h, int w, int H, int W, const float* x, float 
 int gb_pose_shadow_bwd(int N, int h, int w, int H, int W, const float* x, float beta, const float* g_out, float* g_x,
                        void* stream);
 
+/* ---------------------------------------------------------------- head frame (row R11, csrc/head_frame.cu) */
+
+/* replaces the head-relative light work of rgca.AutoEncoder.forward (ca_code/models/rgca.py:175-193), one CTA per
+ * batch item:
+ *   headrel_Rt [B,3,4]         = Rt @ [head_pose; 0 0 0 1]
+ *   headrel_campos [B,3]       = (campos - t) @ R                          (R | t = head_pose [B,3,4])
+ *   headrel_light_pos [B,L,3]  = (light_pos - t) @ R
+ *   headrel_light_sh [B,3,81]  = sum over all L lights of dir2sh(8, normalize(headrel_light_pos)) * intensity
+ *   lightrot_out [B,3,3]       = lightrot @ R                              (both NULL when there is no lightrot)
+ * light_intensity [B,L,C] with C = 1 (used for all three channels, rgca.py:175) or 3.  The direction follows
+ * F.normalize's max(|v|, 1e-12); the basis is sh.dir2sh's.  Double arithmetic from the fp32 inputs; the sum over L
+ * runs in index order with no atomics, so two calls give the same bits.  Forward only (none of the inputs carries a
+ * gradient in the reference's use). */
+int gb_head_lights_fwd(int B, int L, int C, const float* head_pose, const float* campos, const float* Rt,
+                       const float* light_pos, const float* light_intensity, const float* lightrot, float* headrel_Rt,
+                       float* headrel_campos, float* headrel_light_pos, float* headrel_light_sh, float* lightrot_out,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif
