@@ -83,8 +83,9 @@ SIGNATURES = {
     "gb_deconv4x4s2_wnub_bwd": (_i, [_i] * 5 + [_vp] * 5 + [_f, _i] + [_vp] * 4 + [_vp]),
     "gb_conv4x4s2_wnub_fwd": (_i, [_i] * 5 + [_vp] * 4 + [_f, _i, _vp, _vp]),
     "gb_conv4x4s2_wnub_bwd": (_i, [_i] * 5 + [_vp] * 5 + [_f, _i] + [_vp] * 4 + [_vp]),
-    "gb_conv2d_wnub_fwd": (_i, [_i] * 6 + [_vp] * 4 + [_i, _f, _i, _vp, _vp]),
-    "gb_conv2d_wnub_bwd": (_i, [_i] * 6 + [_vp] * 5 + [_f, _i, _i] + [_vp] * 4 + [_vp]),
+    "gb_conv2d_wnub_fwd": (_i, [_i] * 6 + [_vp, _i64] + [_vp] * 3 + [_i, _f, _i, _vp, _vp]),
+    "gb_conv2d_wnub_bwd_workspace_bytes": (_sz, [_i] * 6),
+    "gb_conv2d_wnub_bwd": (_i, [_i] * 6 + [_vp, _i64] + [_vp] * 4 + [_f, _i, _i] + [_vp] * 5 + [_vp]),
     "gb_mvp_slab_to_prims_fwd": (_i, [_i] * 6 + [_vp] * 3 + [_f, _f, _i, _vp, _vp]),
     "gb_mvp_slab_to_prims_bwd": (_i, [_i] * 6 + [_vp] * 3 + [_f, _f, _i] + [_vp] * 3 + [_vp]),
     "gb_mvp_prim_transform_fwd": (_i, [_i, _i] + [_vp] * 3 + [_f, _i] + [_vp] * 3 + [_vp]),
@@ -127,10 +128,9 @@ SIGNATURES = {
     "gb_mvp_raymarch_bwd":(_i, [_i] * 4 + [_vp, _vp, _f] + [_vp] * 5 + [_i] * 3 + [_vp] + [_i] * 3 + [_vp] * 8
                             + [_i, _f, _f, _i, _i, _vp]),
     "gb_upconv_block_fwd": (_i, [_i] * 6 + [_vp] * 10 + [_f] + [_vp] * 3 + [_vp]),
-    "gb_upconv_block_bwd": (_i, [_i] * 6 + [_vp] * 10 + [_f] + [_vp] * 10 + [_vp]),
+    "gb_upconv_block_bwd_workspace_bytes": (_sz, [_i] * 6),
+    "gb_upconv_block_bwd": (_i, [_i] * 6 + [_vp] * 10 + [_f] + [_vp] * 11 + [_vp]),
     "gb_sparse_rows_apply": (_i, [_i] * 3 + [_vp] * 4 + [_i64] * 3 + [_vp] + [_i64] * 3 + [_vp]),
-    "gb_conv3x3_ub_slice_fwd": (_i, [_i] * 5 + [_vp, _i64] + [_vp] * 4 + [_vp]),
-    "gb_conv3x3_ub_slice_bwd": (_i, [_i] * 5 + [_vp, _i64] + [_vp] * 6 + [_vp]),
     "gb_body_tex_compose_workspace_bytes": (_sz, [_i, _i]),
     "gb_body_tex_compose_fwd": (_i, [_i] * 3 + [_vp] * 5 + [_f] + [_vp] * 3 + [_vp]),
     "gb_body_tex_compose_bwd": (_i, [_i] * 3 + [_vp] * 5 + [_f] + [_vp] * 9 + [_vp]),

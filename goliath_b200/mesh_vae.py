@@ -46,10 +46,10 @@ class _ConvSlices(Function):
         with torch.cuda.device(x.device):
             for i, (v, g, b) in enumerate(((va, ga, ba), (vb, gb, bb))):
                 out = torch.empty(B, Cout, H, W, device=x.device)
-                _lib.check(_lib.lib().gb_conv3x3_ub_slice_fwd(
-                    B, c, Cout, H, W, x.data_ptr() + 4 * i * c * H * W, C2 * H * W, _lib.ptr(v.contiguous()),
-                    _lib.ptr(_wn_scale(v, g)), _lib.ptr(b.contiguous()), _lib.ptr(out), _lib.stream_ptr(x.device)),
-                    "conv3x3_ub_slice_fwd")
+                _lib.check(_lib.lib().gb_conv2d_wnub_fwd(
+                    B, c, Cout, H, W, 3, x.data_ptr() + 4 * i * c * H * W, C2 * H * W, _lib.ptr(v.contiguous()),
+                    _lib.ptr(_wn_scale(v, g)), _lib.ptr(b.contiguous()), 2, 1.0, 0, _lib.ptr(out),
+                    _lib.stream_ptr(x.device)), "conv2d_wnub_fwd")
                 outs.append(out)
         ctx.save_for_backward(x, va, ga, vb, gb)
         return tuple(outs)
@@ -61,15 +61,17 @@ class _ConvSlices(Function):
         c, Cout = va.shape[1], va.shape[0]
         gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
         grads = []
+        L = _lib.lib()
+        ws = torch.empty(L.gb_conv2d_wnub_bwd_workspace_bytes(B, c, Cout, H, W, 3) // 4, device=x.device)
         with torch.cuda.device(x.device):
             for i, (v, g, go) in enumerate(((va, ga, g_a), (vb, gb, g_b))):
                 gbias = torch.empty(Cout, H, W, device=x.device)
-                gw = torch.zeros_like(v)
-                _lib.check(_lib.lib().gb_conv3x3_ub_slice_bwd(
-                    B, c, Cout, H, W, x.data_ptr() + 4 * i * c * H * W, C2 * H * W, _lib.ptr(v.contiguous()),
-                    _lib.ptr(_wn_scale(v, g)), _lib.ptr(go.contiguous()), _lib.ptr(gbias),
-                    None if gx is None else gx.data_ptr() + 4 * i * c * H * W, _lib.ptr(gw),
-                    _lib.stream_ptr(x.device)), "conv3x3_ub_slice_bwd")
+                gw = torch.empty_like(v)
+                _lib.check(L.gb_conv2d_wnub_bwd(
+                    B, c, Cout, H, W, 3, x.data_ptr() + 4 * i * c * H * W, C2 * H * W, _lib.ptr(v.contiguous()),
+                    _lib.ptr(_wn_scale(v, g)), None, _lib.ptr(go.contiguous()), 1.0, 0, 2, None, _lib.ptr(gbias),
+                    None if gx is None else gx.data_ptr() + 4 * i * c * H * W, _lib.ptr(gw), _lib.ptr(ws),
+                    _lib.stream_ptr(x.device)), "conv2d_wnub_bwd")
                 grads += list(_wn_chain(v, g, gw)) + [gbias]
         return (gx, *grads)
 

@@ -131,13 +131,12 @@ class _ConvS1WN(Function):
                 mode = 2
             else:
                 raise RuntimeError("bias must be [Cout] or [Cout, H, W]")
-        scale = (weight_g.reshape(-1) / weight_v.norm()).contiguous()
         out = torch.empty(B, Cout, H, W, device=x.device, dtype=torch.float32)
         with torch.cuda.device(x.device):
             _lib.check(_lib.lib().gb_conv2d_wnub_fwd(
-                B, Cin, Cout, H, W, K, _lib.ptr(x), _lib.ptr(weight_v), _lib.ptr(scale), _lib.ptr(b), mode,
-                float(slope if slope is not None else 1.0), int(slope is not None), _lib.ptr(out),
-                _lib.stream_ptr(x.device)), "conv2d_wnub_fwd")
+                B, Cin, Cout, H, W, K, _lib.ptr(x), Cin * H * W, _lib.ptr(weight_v),
+                _lib.ptr(_wn_scale(weight_v, weight_g)), _lib.ptr(b), mode, float(slope if slope is not None else 1.0),
+                int(slope is not None), _lib.ptr(out), _lib.stream_ptr(x.device)), "conv2d_wnub_fwd")
         ctx.save_for_backward(x, weight_v, weight_g, out)
         ctx.slope, ctx.mode = slope, mode
         return out
@@ -149,26 +148,23 @@ class _ConvS1WN(Function):
         Cout, K = v.shape[0], v.shape[2]
         dev = x.device
         gout = gout.contiguous()
-        vnorm = v.norm()
-        scale = (g.reshape(-1) / vnorm).contiguous()
-        gz = torch.empty_like(out)
+        gz = torch.empty_like(out) if ctx.slope is not None else None
         gb = None
         if ctx.mode == 1:
-            gb = torch.zeros(Cout, device=dev, dtype=torch.float32)
+            gb = torch.empty(Cout, device=dev, dtype=torch.float32)
         elif ctx.mode == 2:
             gb = torch.empty(Cout, H, W, device=dev, dtype=torch.float32)
         gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
-        gw = torch.zeros_like(v)
+        gw = torch.empty_like(v)
+        L = _lib.lib()
+        ws = torch.empty(L.gb_conv2d_wnub_bwd_workspace_bytes(B, Cin, Cout, H, W, K) // 4, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_conv2d_wnub_bwd(
-                B, Cin, Cout, H, W, K, _lib.ptr(x), _lib.ptr(v), _lib.ptr(scale), _lib.ptr(out), _lib.ptr(gout),
-                float(ctx.slope if ctx.slope is not None else 1.0), int(ctx.slope is not None), ctx.mode, _lib.ptr(gz),
-                _lib.ptr(gb), _lib.ptr(gx), _lib.ptr(gw), _lib.stream_ptr(dev)), "conv2d_wnub_bwd")
-        # weight-norm chain rule, g per OUTPUT channel (dim 0), norm over the whole tensor
-        w = g * v / vnorm
-        gg = (gw * v).sum(dim=(1, 2, 3), keepdim=True) / vnorm
-        gv = g * gw / vnorm - (gw * w).sum() * v / (vnorm * vnorm)
-        return gx, gv, gg.view_as(g), gb, None
+            _lib.check(L.gb_conv2d_wnub_bwd(
+                B, Cin, Cout, H, W, K, _lib.ptr(x), Cin * H * W, _lib.ptr(v), _lib.ptr(_wn_scale(v, g)), _lib.ptr(out),
+                _lib.ptr(gout), float(ctx.slope if ctx.slope is not None else 1.0), int(ctx.slope is not None),
+                ctx.mode, _lib.ptr(gz), _lib.ptr(gb), _lib.ptr(gx), _lib.ptr(gw), _lib.ptr(ws), _lib.stream_ptr(dev)),
+                "conv2d_wnub_bwd")
+        return (gx, *_wn_chain(v, g, gw), gb, None)
 
 
 class _Conv4x4s2WN(Function):
@@ -470,7 +466,7 @@ def _wn_scale(v, g):
 
 
 class _UpConvBlock(Function):
-    """UpConvBlockDeep forward / backward on csrc/upconv_wnub.cu (two kernels forward, eight backward)."""
+    """UpConvBlockDeep forward / backward on csrc/upconv_wnub.cu (two kernels forward, ten or twelve backward)."""
 
     @staticmethod
     def forward(ctx, x, v1, g1, b1, v2, g2, b2, vr, gr, br, slope, groups):
@@ -517,14 +513,16 @@ class _UpConvBlock(Function):
         gx = torch.empty_like(x) if need_gx else None
         gb1 = torch.empty(Cin, H, W, device=dev)
         gb2 = torch.empty(Cout, H, W, device=dev)
-        gbr = torch.zeros(Cout, device=dev)
-        gw1, gw2, gwr = torch.zeros_like(v1), torch.zeros_like(v2), torch.zeros_like(vr)
+        gbr = torch.empty(Cout, device=dev)
+        gw1, gw2, gwr = torch.empty_like(v1), torch.empty_like(v2), torch.empty_like(vr)
+        L = _lib.lib()
+        ws = torch.empty(L.gb_upconv_block_bwd_workspace_bytes(B, Cin, Cout, ctx.groups, Hi, Wi) // 4, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_upconv_block_bwd(
+            _lib.check(L.gb_upconv_block_bwd(
                 B, Cin, Cout, ctx.groups, Hi, Wi, _lib.ptr(x), _lib.ptr(v1), _lib.ptr(s1), _lib.ptr(v2), _lib.ptr(s2),
                 _lib.ptr(vr), _lib.ptr(sr), _lib.ptr(h1), _lib.ptr(mask), _lib.ptr(gout), ctx.slope, _lib.ptr(gz2),
                 _lib.ptr(gz1), _lib.ptr(gu), _lib.ptr(gb1), _lib.ptr(gb2), _lib.ptr(gbr), _lib.ptr(gw1), _lib.ptr(gw2),
-                _lib.ptr(gwr), _lib.ptr(gx), _lib.stream_ptr(dev)), "upconv_block_bwd")
+                _lib.ptr(gwr), _lib.ptr(gx), _lib.ptr(ws), _lib.stream_ptr(dev)), "upconv_block_bwd")
         gv1, gg1 = _wn_chain(v1, g1, gw1)
         gv2, gg2 = _wn_chain(v2, g2, gw2)
         gvr, ggr = _wn_chain(vr, gr, gwr)

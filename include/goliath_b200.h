@@ -553,18 +553,24 @@ int gb_deconv4x4s2_tc_fwd(int B, int Cin, int Cin_pad, int Cout, int Hi, int Wi,
 /* ---------------------------------------------------------------- hand-MVP decoders (row R8) */
 
 /* replaces conv2d + bias add (+ LeakyReLU) of la.Conv2dWNUB / Conv2dWN (ca_code/nn/layers.py:276-327,468-472;
- * users: hand_mvp.py:297-321 TransDecoder, hand_mvp.py:269-294 PoseEncoder via blocks.py:232-280 ConvBlock), stride 1,
+ * users: hand_mvp.py:297-321 TransDecoder, hand_mvp.py:269-294 PoseEncoder via blocks.py:232-280 ConvBlock, and
+ * th.split + la.Conv2dWNUB of mesh_vae.py:615-621, verts_conv / tex_conv on a channel slice read in place), stride 1,
  * K = 1 or 3, padding (K-1)/2, with the weight-norm scale folded in: out = act(scale[co] * conv(x, v) + bias).
- * x [B,Cin,H,W], v [Cout,Cin,K,K], scale [Cout] = g / ||v||_F; bias_mode 0 none, 1 tied [Cout], 2 untied [Cout,H,W]. */
-int gb_conv2d_wnub_fwd(int B, int Cin, int Cout, int H, int W, int K, const float* x, const float* v, const float* scale,
-                       const float* bias, int bias_mode, float slope, int apply_act, float* out, void* stream);
+ * x [B,Cin,H,W] with items x_bs >= Cin*H*W floats apart; v [Cout,Cin,K,K], scale [Cout] = g / ||v||_F; bias_mode 0 none,
+ * 1 tied [Cout], 2 untied [Cout,H,W]. */
+int gb_conv2d_wnub_fwd(int B, int Cin, int Cout, int H, int W, int K, const float* x, long long x_bs, const float* v,
+                       const float* scale, const float* bias, int bias_mode, float slope, int apply_act, float* out,
+                       void* stream);
 
-/* backward of the above.  gz [B,Cout,H,W] scratch; g_bias: [Cout,H,W] written (mode 2) or [Cout] ACCUMULATED (mode 1,
- * caller zeroes) or NULL; gx [B,Cin,H,W] or NULL; gw [Cout,Cin,K,K] = dL/d(effective weight at unit scale),
- * ACCUMULATED (caller zeroes it and applies the weight-norm chain rule). */
-int gb_conv2d_wnub_bwd(int B, int Cin, int Cout, int H, int W, int K, const float* x, const float* v, const float* scale,
-                       const float* out, const float* gout, float slope, int apply_act, int bias_mode, float* gz,
-                       float* g_bias, float* gx, float* gw, void* stream);
+/* replaces the autograd graph of the layer above.  gz [B,Cout,H,W] scratch when apply_act, else unused (may be NULL);
+ * g_bias: [Cout,H,W] (mode 2) or [Cout] (mode 1) written, or NULL; gx [B,Cin,H,W] with items x_bs floats apart, or
+ * NULL; gw [Cout,Cin,K,K] = dL/d(effective weight at unit scale) written (the caller applies the weight-norm chain
+ * rule).  Every sum runs in a fixed order (no float atomics), so the gradients are bitwise repeatable.
+ * `workspace`: gb_conv2d_wnub_bwd_workspace_bytes(B, Cin, Cout, H, W, K) bytes. */
+size_t gb_conv2d_wnub_bwd_workspace_bytes(int B, int Cin, int Cout, int H, int W, int K);
+int gb_conv2d_wnub_bwd(int B, int Cin, int Cout, int H, int W, int K, const float* x, long long x_bs, const float* v,
+                       const float* scale, const float* out, const float* gout, float slope, int apply_act,
+                       int bias_mode, float* gz, float* g_bias, float* gx, float* gw, void* workspace, void* stream);
 
 /* replaces the slab -> primitive-template sequence: relu(25*rgb+100) (hand_mvp.py:472), relu(alpha) (:434),
  * cat/view/permute/reshape (hand_mvp.py:172-185) and the valid-primitive gather (ca_code/utils/render_raymarcher.py:44-46)
@@ -694,14 +700,16 @@ int gb_upconv_block_fwd(int B, int Cin, int Cout, int groups, int Hi, int Wi, co
                         const float* vr, const float* sr, const float* br, float slope, float* h1, float* out,
                         unsigned char* mask, void* stream);
 /* backward of the above (replaces the autograd graph of the same lines).  Scratch gz2 [B,Cout,H,W], gz1 and gu
- * [B,Cin,H,W]; gb1 [Cin,H,W] and gb2 [Cout,H,W] written (batch sums); gbr [Cout], gw1, gw2 and gwr ACCUMULATED (caller
- * zeroes them): gradients of the effective weights at unit scale.  gx [B,Cin,Hi,Wi] or NULL is a gather over the
- * upsample's footprint (no atomics). */
+ * [B,Cin,H,W]; gb1 [Cin,H,W], gb2 [Cout,H,W], gbr [Cout] and the effective-weight gradients at unit scale gw1, gw2, gwr
+ * are all WRITTEN.  gx [B,Cin,Hi,Wi] or NULL is a gather over the upsample's footprint.  Every sum runs in a fixed order
+ * (no float atomics), so the gradients are bitwise repeatable.
+ * `workspace`: gb_upconv_block_bwd_workspace_bytes(B, Cin, Cout, groups, Hi, Wi) bytes. */
+size_t gb_upconv_block_bwd_workspace_bytes(int B, int Cin, int Cout, int groups, int Hi, int Wi);
 int gb_upconv_block_bwd(int B, int Cin, int Cout, int groups, int Hi, int Wi, const float* x, const float* v1,
                         const float* s1, const float* v2, const float* s2, const float* vr, const float* sr,
                         const float* h1, const unsigned char* mask, const float* gout, float slope, float* gz2,
                         float* gz1, float* gu, float* gb1, float* gb2, float* gbr, float* gw1, float* gw2, float* gwr,
-                        float* gx, void* stream);
+                        float* gx, void* workspace, void* stream);
 
 /* replaces impaint_batch / resample_tex (ca_code/utils/seams.py:14-41: index_put of src texels into dst texels,
  * (1-w) tex + w grid_sample(tex, 2(uv-0.5)) with align_corners=False and border padding) and sample_uv
@@ -713,16 +721,6 @@ int gb_upconv_block_bwd(int B, int Cin, int Cout, int groups, int Hi, int Wi, co
 int gb_sparse_rows_apply(int B, int C, int n_rows, const int* row_ptr, const int* col, const float* coef,
                          const float* in, long long in_bs, long long in_cs, long long in_rs, float* out,
                          long long out_bs, long long out_cs, long long out_rs, void* stream);
-
-/* replaces th.split + la.Conv2dWNUB of mesh_vae.py:615-621 (verts_conv / tex_conv, 3x3 "same", untied bias, no
- * activation, on channels [0,4) / [4,8) of the seam-sampled map) without a copy of the slice: item b of x (and of gx)
- * starts at b * x_bs floats.  v [Cout,Cin,3,3], scale [Cout], bias [Cout,H,W], out [B,Cout,H,W]. */
-int gb_conv3x3_ub_slice_fwd(int B, int Cin, int Cout, int H, int W, const float* x, long long x_bs, const float* v,
-                            const float* scale, const float* bias, float* out, void* stream);
-/* g_bias [Cout,H,W] written; gw [Cout,Cin,3,3] ACCUMULATED (unit scale); gx written on channels [0,Cin) of each item,
- * or NULL. */
-int gb_conv3x3_ub_slice_bwd(int B, int Cin, int Cout, int H, int W, const float* x, long long x_bs, const float* v,
-                            const float* scale, const float* gout, float* g_bias, float* gx, float* gw, void* stream);
 
 /* replaces the 2048^2 part of mesh_vae.AutoEncoder.forward_tex (ca_code/models/mesh_vae.py:211-222: bilinear x2
  * upsample with align_corners=False, `+ upscale_net(x)`, `* tex_std + tex_mean`, `* shadow_map`) together with the

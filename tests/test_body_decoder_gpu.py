@@ -57,11 +57,14 @@ def test_upconv_block_vs_oracle(cuda, cin, cout, size, groups, B):
     finally:
         torch.backends.cudnn.allow_tf32 = tf32
     out, gr = run(blk, torch.float32)
+    out2, gr2 = run(blk, torch.float32)
     assert _maxrel(out, o64) <= 1e-4
     assert set(gr) == set(g64)
     for n in g64:
         bound = max(1e-4, 4 * _nrel(g32[n], g64[n]))
         assert _nrel(gr[n], g64[n]) <= bound, (n, _nrel(gr[n], g64[n]), bound)
+        assert torch.equal(gr[n], gr2[n]), n      # fixed-order sums: the same bits on every run
+    assert torch.equal(out, out2)
 
 
 def _gpu_seams(g, cuda):

@@ -218,7 +218,8 @@ def test_composer_repeatable_sync_free_and_graphed(cuda):
     leaves = [inp["tex_mean_rec"].clone().requires_grad_(), tvr.clone().requires_grad_(),
               smap.clone().requires_grad_()]
     ob = comp.upscale_net.out_block
-    wrt = leaves + [ob.weight_v, ob.weight_g, ob.bias, comp.upscale_net.conv_block[0].bias]
+    cb = comp.upscale_net.conv_block[0]
+    wrt = leaves + [ob.weight_v, ob.weight_g, ob.bias, cb.weight_v, cb.weight_g, cb.bias]
 
     def step():
         return torch.autograd.grad((comp(*leaves) * w).sum(), wrt)
@@ -230,8 +231,7 @@ def test_composer_repeatable_sync_free_and_graphed(cuda):
         second = step()
     finally:
         torch.cuda.set_sync_debug_mode(0)
-    # every gradient the composite kernel and the seam gathers produce is bitwise repeatable (conv_block's weight
-    # gradient comes from the stride-1 kernel's atomic reduction and is left out)
+    # every gradient the composite kernel, the seam gathers and the stride-1 convolution produce is bitwise repeatable
     for a, b in zip(first, second):
         assert torch.equal(a, b)
     with torch.no_grad():

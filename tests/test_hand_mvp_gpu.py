@@ -52,14 +52,24 @@ def test_conv_block_vs_reference(cuda, tag, cin, cout, k):
     names = json.loads(str(g[tag + "_names"]))
     assert sorted(names) == sorted(n for n, _ in blk.named_parameters()), "parameter names must match the reference's"
     blk.load_state_dict({n: f("%s_p_%s" % (tag, n)) for n in names})
-    x = f(tag + "_x").requires_grad_()
-    y = blk(x)
+    params = list(blk.named_parameters())
+
+    def run():
+        x = f(tag + "_x").requires_grad_()
+        y = blk(x)
+        grads = torch.autograd.grad((y * f(tag + "_w")).sum(), [x] + [p for _, p in params])
+        return y.detach(), dict(zip(["x"] + [n for n, _ in params], grads))
+
+    y, gr = run()
+    y2, gr2 = run()
     assert_close(t2n(y), g[tag + "_y"], what="ConvBlock output", **_tol(g[tag + "_y"], 1e-4))
-    (y * f(tag + "_w")).sum().backward()
-    assert_close(t2n(x.grad), g[tag + "_gx"], what="ConvBlock grad input", **_tol(g[tag + "_gx"], 2e-4))
-    for n, p in blk.named_parameters():
+    assert_close(t2n(gr["x"]), g[tag + "_gx"], what="ConvBlock grad input", **_tol(g[tag + "_gx"], 2e-4))
+    for n, _ in params:
         r = g["%s_g_%s" % (tag, n)]
-        assert_close(t2n(p.grad), r, what="ConvBlock grad " + n, **_tol(r, 5e-4))
+        assert_close(t2n(gr[n]), r, what="ConvBlock grad " + n, **_tol(r, 5e-4))
+    assert torch.equal(y, y2)
+    for n in gr:
+        assert torch.equal(gr[n], gr2[n]), n      # fixed-order sums: the same bits on every run
 
 
 def test_pose_encoder_vs_reference(cuda):
