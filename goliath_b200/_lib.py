@@ -80,9 +80,11 @@ SIGNATURES = {
     "gb_nchw_to_nhwc_split": (_i, [_i] * 5 + [_vp] * 3 + [_vp]),
     "gb_deconv4x4s2_tc_fwd": (_i, [_i] * 6 + [_vp] * 6 + [_f, _i, _vp, _vp, _i, _vp, _vp]),
     "gb_deconv4x4s2_wnub_fwd": (_i, [_i] * 5 + [_vp] * 4 + [_f, _i, _vp, _vp]),
-    "gb_deconv4x4s2_wnub_bwd": (_i, [_i] * 5 + [_vp] * 5 + [_f, _i] + [_vp] * 4 + [_vp]),
+    "gb_deconv4x4s2_wnub_bwd_workspace_bytes": (_sz, [_i] * 5),
+    "gb_deconv4x4s2_wnub_bwd": (_i, [_i] * 5 + [_vp] * 5 + [_f, _i] + [_vp] * 5 + [_vp]),
     "gb_conv4x4s2_wnub_fwd": (_i, [_i] * 5 + [_vp] * 4 + [_f, _i, _vp, _vp]),
-    "gb_conv4x4s2_wnub_bwd": (_i, [_i] * 5 + [_vp] * 5 + [_f, _i] + [_vp] * 4 + [_vp]),
+    "gb_conv4x4s2_wnub_bwd_workspace_bytes": (_sz, [_i] * 5),
+    "gb_conv4x4s2_wnub_bwd": (_i, [_i] * 5 + [_vp] * 5 + [_f, _i] + [_vp] * 5 + [_vp]),
     "gb_conv2d_wnub_fwd": (_i, [_i] * 6 + [_vp, _i64] + [_vp] * 3 + [_i, _f, _i, _vp, _vp]),
     "gb_conv2d_wnub_bwd_workspace_bytes": (_sz, [_i] * 6),
     "gb_conv2d_wnub_bwd": (_i, [_i] * 6 + [_vp, _i64] + [_vp] * 4 + [_f, _i, _i] + [_vp] * 5 + [_vp]),

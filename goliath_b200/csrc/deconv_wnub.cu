@@ -13,16 +13,13 @@
 // 8x16 weights of the current input channel come from shared memory (weights as broadcast float4).  The tensor-core
 // phase-GEMM version (3xTF32, TMA-fed: csrc/deconv_tc.cu) serves the inference forward; the last layers are bound by the
 // untied-bias + output traffic (1.07 GB for 16->125 @1024^2), not by FLOPs.
-#include <cstdlib>
-#include <cstring>
-
-#include "common.cuh"
+#include "wn_conv.cuh"
 
 namespace {
 
 constexpr int TQ = 16;        // quads (input positions) per CTA edge -> 32x32 output tile
 constexpr int CO_T = 8;       // output channels per CTA pass
-constexpr int CI_CHUNK = 8;   // input channels staged per step
+constexpr int TQ_CI = 8;      // input channels staged per step
 constexpr int HALO = TQ + 2;
 
 // SCALE_IN = false: the weight-norm scale belongs to the output channel and is applied to the accumulator.
@@ -34,8 +31,8 @@ __global__ void __launch_bounds__(TQ* TQ) deconv4x4s2_fwd_kernel(
     const float* __restrict__ v /* [Cin,Cout,4,4] */, const float* __restrict__ scale /* [Cout] */,
     const float* __restrict__ bias /* [Cout,2Hi,2Wi] or null */, float slope, int apply_act,
     float* __restrict__ out /* [B,Cout,2Hi,2Wi] */) {
-  __shared__ float s_x[CI_CHUNK][HALO][HALO + 1];
-  __shared__ __align__(16) float s_w[CI_CHUNK][CO_T][16];
+  __shared__ float s_x[TQ_CI][HALO][HALO + 1];
+  __shared__ __align__(16) float s_w[TQ_CI][CO_T][16];
   const int tiles_x = (Wi + TQ - 1) / TQ;
   const int tile = blockIdx.x;
   const int ty0 = (tile / tiles_x) * TQ, tx0 = (tile % tiles_x) * TQ;
@@ -51,10 +48,10 @@ __global__ void __launch_bounds__(TQ* TQ) deconv4x4s2_fwd_kernel(
   for (int c = 0; c < CO_T; ++c) { acc[c][0] = acc[c][1] = acc[c][2] = acc[c][3] = 0.f; }
 
   const float* xb = x + (size_t)b * Cin * Hi * Wi;
-  for (int ci0 = 0; ci0 < Cin; ci0 += CI_CHUNK) {
+  for (int ci0 = 0; ci0 < Cin; ci0 += TQ_CI) {
     __syncthreads();
     // stage the input tile with a 1-pixel halo (zeros outside the image / beyond Cin)
-    for (int i = tid; i < CI_CHUNK * HALO * HALO; i += TQ * TQ) {
+    for (int i = tid; i < TQ_CI * HALO * HALO; i += TQ * TQ) {
       const int ci = i / (HALO * HALO), r = (i / HALO) % HALO, c = i % HALO;
       const int yy = ty0 - 1 + r, xx = tx0 - 1 + c;
       float val = 0.f;
@@ -62,7 +59,7 @@ __global__ void __launch_bounds__(TQ* TQ) deconv4x4s2_fwd_kernel(
       s_x[ci][r][c] = val;
     }
     // stage the weights of (ci chunk) x (co block): v[ci][co][ky][kx]
-    for (int i = tid; i < CI_CHUNK * CO_T * 16; i += TQ * TQ) {
+    for (int i = tid; i < TQ_CI * CO_T * 16; i += TQ * TQ) {
       const int ci = i / (CO_T * 16), co = (i / 16) % CO_T, k = i % 16;
       float val = 0.f;
       if (ci0 + ci < Cin && co0 + co < Cout) {
@@ -73,7 +70,7 @@ __global__ void __launch_bounds__(TQ* TQ) deconv4x4s2_fwd_kernel(
     }
     __syncthreads();
 #pragma unroll 2
-    for (int ci = 0; ci < CI_CHUNK; ++ci) {
+    for (int ci = 0; ci < TQ_CI; ++ci) {
       // 3x3 neighbourhood of the input position (rows m-1..m+1, cols n-1..n+1)
       const float a00 = s_x[ci][qy][qx], a01 = s_x[ci][qy][qx + 1], a02 = s_x[ci][qy][qx + 2];
       const float a10 = s_x[ci][qy + 1][qx], a11 = s_x[ci][qy + 1][qx + 1], a12 = s_x[ci][qy + 1][qx + 2];
@@ -362,30 +359,15 @@ GB_API int gb_deconv4x4s2_wnub_fwd(int B, int Cin, int Cout, int Hi, int Wi, con
 }
 
 // =====================================================================================================
-// Backward (training): three kernels, all hand-written (no cuDNN):
-//   1. deconv_act_bwd_kernel : gz = gout * act'(out)  and  g_bias = sum_b gz      (element-wise, HBM)
+// Backward (training), all hand-written (no cuDNN), gather-only, every sum in a fixed order:
+//   1. act_bwd_kernel (wn_conv.cuh): gz = gout * act'(out) and g_bias = sum_b gz; without an activation gz is gout and
+//      g_bias its batch sum (batch_sum_kernel)
 //   2. deconv4x4s2_bwd_data_kernel   : gx[ci,y,x] = sum_co scale[co] sum_{ky,kx} gz[co,2y-1+ky,2x-1+kx] v[ci,co,ky,kx]
-//   3. deconv4x4s2_bwd_weight_kernel : gw[ci,co,ky,kx] = sum_{b,y,x} x[ci,y,x] gz[co,2y-1+ky,2x-1+kx]
+//   3. deconv4x4s2_bwd_weight_kernel : gw[ci,co,ky,kx] = sum_{b,y,x} x[ci,y,x] gz[co,2y-1+ky,2x-1+kx], as per-CTA
+//      partials that split_sum_kernel adds in CTA order
 // (gw is the gradient of the EFFECTIVE weight divided by nothing: the weight-norm chain rule on the tiny
 //  [Cin,Cout,4,4] tensors is finished by the caller.)
 namespace {
-
-__global__ void __launch_bounds__(256) deconv_act_bwd_kernel(int B, long long per_item /* Cout*Ho*Wo */,
-                                                             const float* __restrict__ gout,
-                                                             const float* __restrict__ out, float slope, int apply_act,
-                                                             float* __restrict__ gz, float* __restrict__ gbias) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= per_item) return;
-  float acc = 0.f;
-  for (int b = 0; b < B; ++b) {
-    const size_t o = (size_t)b * per_item + i;
-    float g = gout[o];
-    if (apply_act) g = out[o] > 0.f ? g : g * slope;
-    gz[o] = g;
-    acc += g;
-  }
-  if (gbias) gbias[i] = acc;
-}
 
 constexpr int BD_T = 16;          // input pixels per CTA edge
 constexpr int BD_CO = 8;          // output channels staged per step
@@ -470,22 +452,26 @@ __global__ void __launch_bounds__(BD_T* BD_T) deconv4x4s2_bwd_data_kernel(
 }
 
 // weight gradient: warp tile = 16 ci x 8 co (lane: cig = lane>>3 -> 4 ci, co = lane&7 -> 16 taps), 8 warps split the
-// pixels of each staged 16x16 input tile; every CTA walks many tiles and flushes its sums once.
-constexpr int BW_TX = 16, BW_TY = 8;            // input tile staged per step: 8 rows x 16 columns = 128 pixels
-constexpr int BW_CI = 16;
-constexpr int BW_CO = 8;
-constexpr int BW_GX = 2 * BW_TX + 2, BW_GY = 2 * BW_TY + 2;
+// pixels of each staged 16x16 input tile; every CTA walks many tiles, adds its warps in order and writes its sums to
+// part[blockIdx.x] ([Cin, Cout, 4, 4]).
+constexpr int NW_TX = 16, NW_TY = 8;            // input tile staged per step: 8 rows x 16 columns = 128 pixels
+constexpr int NW_CI = 16;
+constexpr int NW_CO = 8;
+constexpr int NW_GX = 2 * NW_TX + 2, NW_GY = 2 * NW_TY + 2;
+static_assert(NW_TX == BW_TX && NW_TY == BW_TY && NW_CI == BW_CI && NW_CO == BW_CO,
+              "wgrad_split sizes this kernel's grid with wn_conv.cuh's weight-gradient tile");
 
 __global__ void __launch_bounds__(256) deconv4x4s2_bwd_weight_kernel(
     int B, int Cin, int Cout, int Hi, int Wi, const float* __restrict__ x, const float* __restrict__ gz,
-    float* __restrict__ gw /* [Cin,Cout,4,4], accumulated */) {
-  __shared__ float s_x[BW_CI][BW_TX * BW_TY];
-  __shared__ float s_g[BW_CO][BW_GY][BW_GX + 1];
-  const int ci0 = blockIdx.y * BW_CI, co0 = blockIdx.z * BW_CO;
+    float* __restrict__ part /* [gridDim.x][Cin,Cout,4,4] */) {
+  __shared__ float s_x[NW_CI][NW_TX * NW_TY];
+  __shared__ float s_g[NW_CO][NW_GY][NW_GX + 1];
+  __shared__ float s_r[32 * (4 * 16 + 1)];
+  const int ci0 = blockIdx.y * NW_CI, co0 = blockIdx.z * NW_CO;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int cig = lane >> 3, col = lane & 7;
   const int Ho = 2 * Hi, Wo = 2 * Wi;
-  const int tiles_x = (Wi + BW_TX - 1) / BW_TX, tiles_y = (Hi + BW_TY - 1) / BW_TY;
+  const int tiles_x = (Wi + NW_TX - 1) / NW_TX, tiles_y = (Hi + NW_TY - 1) / NW_TY;
   const int total = B * tiles_x * tiles_y;
   float acc[4][16];
 #pragma unroll
@@ -495,17 +481,17 @@ __global__ void __launch_bounds__(256) deconv4x4s2_bwd_weight_kernel(
 
   for (int t = blockIdx.x; t < total; t += gridDim.x) {
     const int b = t / (tiles_x * tiles_y), tt = t % (tiles_x * tiles_y);
-    const int ty0 = (tt / tiles_x) * BW_TY, tx0 = (tt % tiles_x) * BW_TX;
+    const int ty0 = (tt / tiles_x) * NW_TY, tx0 = (tt % tiles_x) * NW_TX;
     __syncthreads();
-    for (int i = tid; i < BW_CI * BW_TX * BW_TY; i += 256) {
-      const int ci = i / (BW_TX * BW_TY), p = i % (BW_TX * BW_TY);
-      const int yy = ty0 + p / BW_TX, xx = tx0 + p % BW_TX;
+    for (int i = tid; i < NW_CI * NW_TX * NW_TY; i += 256) {
+      const int ci = i / (NW_TX * NW_TY), p = i % (NW_TX * NW_TY);
+      const int yy = ty0 + p / NW_TX, xx = tx0 + p % NW_TX;
       float val = 0.f;
       if (ci0 + ci < Cin && yy < Hi && xx < Wi) val = x[(((size_t)b * Cin + ci0 + ci) * Hi + yy) * Wi + xx];
       s_x[ci][p] = val;
     }
-    for (int i = tid; i < BW_CO * BW_GY * BW_GX; i += 256) {
-      const int co = i / (BW_GY * BW_GX), r = (i / BW_GX) % BW_GY, c = i % BW_GX;
+    for (int i = tid; i < NW_CO * NW_GY * NW_GX; i += 256) {
+      const int co = i / (NW_GY * NW_GX), r = (i / NW_GX) % NW_GY, c = i % NW_GX;
       const int Y = 2 * ty0 - 1 + r, X = 2 * tx0 - 1 + c;
       float val = 0.f;
       if (co0 + co < Cout && Y >= 0 && Y < Ho && X >= 0 && X < Wo) val = gz[(((size_t)b * Cout + co0 + co) * Ho + Y) * Wo + X];
@@ -513,8 +499,8 @@ __global__ void __launch_bounds__(256) deconv4x4s2_bwd_weight_kernel(
     }
     __syncthreads();
     // this warp's 16 pixels of the tile (one row)
-    for (int pp = 0; pp < (BW_TX * BW_TY) / 8; ++pp) {
-      const int p = warp * ((BW_TX * BW_TY) / 8) + pp, py = p / BW_TX, px = p % BW_TX;
+    for (int pp = 0; pp < (NW_TX * NW_TY) / 8; ++pp) {
+      const int p = warp * ((NW_TX * NW_TY) / 8) + pp, py = p / NW_TX, px = p % NW_TX;
       float xv[4];
 #pragma unroll
       for (int a = 0; a < 4; ++a) xv[a] = s_x[cig * 4 + a][p];
@@ -528,17 +514,11 @@ __global__ void __launch_bounds__(256) deconv4x4s2_bwd_weight_kernel(
         }
     }
   }
-  // flush: one RED per (ci, co, tap) per warp
-  const int co = co0 + col;
-#pragma unroll
-  for (int a = 0; a < 4; ++a) {
-    const int ci = ci0 + cig * 4 + a;
-    if (ci < Cin && co < Cout) {
-#pragma unroll
-      for (int k = 0; k < 16; k += 4)
-        gb::red_add_v4(gw + ((size_t)ci * Cout + co) * 16 + k, acc[a][k], acc[a][k + 1], acc[a][k + 2], acc[a][k + 3]);
-    }
-  }
+  float* dst = part + (size_t)blockIdx.x * Cin * Cout * 16;
+  store_warp_ordered_sums<16>(acc, s_r, [&](int l, int a, int k, float r) {
+    const int ci = ci0 + (l >> 3) * 4 + a, co = co0 + (l & 7);
+    if (ci < Cin && co < Cout) dst[((size_t)ci * Cout + co) * 16 + k] = r;
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -704,7 +684,7 @@ constexpr int WW_SMEM = 2 * (WW_XBYTES + WW_GBYTES);      // 121600
 
 __global__ void __launch_bounds__(256, 1) deconv4x4s2_bwd_weight_wide_kernel(
     int B, int Cin, int Cout, int Hi, int Wi, const float* __restrict__ x, const float* __restrict__ gz,
-    float* __restrict__ gw /* [Cin,Cout,4,4], accumulated */) {
+    float* __restrict__ part /* [gridDim.x][Cin,Cout,4,4] */) {
   extern __shared__ __align__(16) unsigned char dsm[];
   const int ci0 = blockIdx.y * WW_CI, co0 = blockIdx.z * WW_CO;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -771,16 +751,14 @@ __global__ void __launch_bounds__(256, 1) deconv4x4s2_bwd_weight_wide_kernel(
       }
     }
   }
-  const int co = co0 + col;
-#pragma unroll
-  for (int a = 0; a < 4; ++a) {
-    const int ci = ci0 + a * 4 + cig;
-    if (ci < Cin && co < Cout) {
-#pragma unroll
-      for (int t = 0; t < 16; t += 4)
-        gb::red_add_v4(gw + ((size_t)ci * Cout + co) * 16 + t, acc[a][t], acc[a][t + 1], acc[a][t + 2], acc[a][t + 3]);
-    }
-  }
+  // the staged tiles are dead: the reduction reuses their shared memory
+  gb::cp_async_wait<0>();
+  __syncthreads();
+  float* dst = part + (size_t)blockIdx.x * Cin * Cout * 16;
+  store_warp_ordered_sums<16>(acc, reinterpret_cast<float*>(dsm), [&](int l, int a, int k, float r) {
+    const int ci = ci0 + a * 4 + (l >> 3), co = co0 + (l & 7);
+    if (ci < Cin && co < Cout) dst[((size_t)ci * Cout + co) * 16 + k] = r;
+  });
 }
 
 // The backward launches, shared by the transposed convolution and the stride-2 convolution (whose forward is this
@@ -807,70 +785,90 @@ int launch_bwd_data(bool wide, int B, int Cin, int Cout, int Hi, int Wi, const f
   return 1;
 }
 
-int launch_bwd_weight(bool wide, int B, int Cin, int Cout, int Hi, int Wi, const float* x, const float* gz, float* gw,
-                      cudaStream_t s) {
-  if (wide) {
+// The backward's kernels for a transposed convolution Cin -> Cout on an Hi x Wi input, and its weight gradient's split
+// (CTAs per channel block, each writing one [Cin, Cout, 4, 4] partial).  The wide kernels need 16-byte rows and a full
+// tile; the transposed convolution takes them for the layers of the wide forward (Cin <= 32), where its data gradient
+// follows the same choice, and the stride-2 convolution (`conv`: its weight gradient, with the sides exchanged) at any
+// channel count.  The launch and the workspace size both come from here.
+struct BwdPlan {
+  bool wide;
+  int split;
+  size_t part_bytes;
+};
+
+BwdPlan bwd_plan(bool conv, int B, int Cin, int Cout, int Hi, int Wi) {
+  BwdPlan p;
+  p.wide = (conv || Cin <= 32) && Wi % 4 == 0 && Wi >= 32 && Hi >= 16;
+  if (p.wide) {
+    // one CTA per SM at a time (120 KB of shared memory): two FULL waves
+    const int total = B * gb::cdiv(Hi, WW_Y) * gb::cdiv(Wi, WW_X);
+    const int pairs = gb::cdiv(Cin, WW_CI) * gb::cdiv(Cout, WW_CO);
+    p.split = max(1, min((gb::kNumSMs * 2) / pairs, total));
+  } else {
+    p.split = wgrad_split(B, Cin, Cout, 1, Hi, Wi, 3);  // ~3 CTAs per SM in total
+  }
+  p.part_bytes = sizeof(float) * p.split * Cin * Cout * 16;
+  return p;
+}
+
+// gw [Cin,Cout,4,4] written; two launches
+int launch_bwd_weight(const BwdPlan& p, int B, int Cin, int Cout, int Hi, int Wi, const float* x, const float* gz,
+                      float* gw, float* part, cudaStream_t s) {
+  if (p.wide) {
     static bool configured = false;
     if (!configured) {
       GB_CUDA(cudaFuncSetAttribute(deconv4x4s2_bwd_weight_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WW_SMEM));
       configured = true;
     }
-    const int total = B * gb::cdiv(Hi, WW_Y) * gb::cdiv(Wi, WW_X);
-    const int pairs = gb::cdiv(Cin, WW_CI) * gb::cdiv(Cout, WW_CO);
-    int split = (gb::kNumSMs * 2) / pairs;  // one CTA per SM at a time (120 KB of shared memory): two FULL waves
-    split = max(1, min(split, total));
-    dim3 grid(split, gb::cdiv(Cin, WW_CI), gb::cdiv(Cout, WW_CO));
-    deconv4x4s2_bwd_weight_wide_kernel<<<grid, 256, WW_SMEM, s>>>(B, Cin, Cout, Hi, Wi, x, gz, gw);
-    return 1;
+    dim3 grid(p.split, gb::cdiv(Cin, WW_CI), gb::cdiv(Cout, WW_CO));
+    deconv4x4s2_bwd_weight_wide_kernel<<<grid, 256, WW_SMEM, s>>>(B, Cin, Cout, Hi, Wi, x, gz, part);
+  } else {
+    dim3 grid(p.split, gb::cdiv(Cin, NW_CI), gb::cdiv(Cout, NW_CO));
+    deconv4x4s2_bwd_weight_kernel<<<grid, 256, 0, s>>>(B, Cin, Cout, Hi, Wi, x, gz, part);
   }
-  const int total = B * gb::cdiv(Hi, BW_TY) * gb::cdiv(Wi, BW_TX);
-  const int pairs = gb::cdiv(Cin, BW_CI) * gb::cdiv(Cout, BW_CO);
-  int split = gb::cdiv(gb::kNumSMs * 3, pairs);  // ~3 CTAs per SM in total
-  split = max(1, min(split, total));
-  dim3 grid(split, gb::cdiv(Cin, BW_CI), gb::cdiv(Cout, BW_CO));
-  deconv4x4s2_bwd_weight_kernel<<<grid, 256, 0, s>>>(B, Cin, Cout, Hi, Wi, x, gz, gw);
-  return 1;
+  const int n = Cin * Cout * 16;
+  split_sum_kernel<<<gb::cdiv(n, 256), 256, 0, s>>>(p.split, n, part, gw);
+  return 2;
 }
 
-// gz = gout * act'(out) and the untied-bias gradient, unless gz aliases gout (no activation, no separate bias gradient)
+// With an activation: gz = gout * act'(out) and the untied-bias gradient.  Without one, gz is gout and the bias
+// gradient its batch sum (NULL at B == 1, where the caller aliases it to gout).
 int launch_act_bwd(int B, long long per_item, const float* out, const float* gout, float slope, int apply_act, float* gz,
                    float* g_bias, cudaStream_t s) {
-  if (gz == gout && !apply_act && !g_bias) return 0;
-  deconv_act_bwd_kernel<<<(unsigned)gb::cdiv64(per_item, 256), 256, 0, s>>>(B, per_item, gout, out, slope, apply_act, gz,
-                                                                            g_bias);
-  return 1;
+  const unsigned grid = (unsigned)gb::cdiv64(per_item, 256);
+  if (apply_act) {
+    act_bwd_kernel<<<grid, 256, 0, s>>>(B, per_item, gout, nullptr, out, slope, gz, g_bias);
+    return 1;
+  }
+  if (g_bias) {
+    batch_sum_kernel<<<grid, 256, 0, s>>>(B, per_item, gout, g_bias);
+    return 1;
+  }
+  return 0;
 }
 
 }  // namespace
 
-// GOLIATH_B200_DECONV_BWD=narrow keeps the round-1 backward kernels on every layer (A/B timing, tests)
-static bool wide_bwd_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("GOLIATH_B200_DECONV_BWD");
-    v = (e && !strcmp(e, "narrow")) ? 0 : 1;
-  }
-  return v == 1;
+GB_API size_t gb_deconv4x4s2_wnub_bwd_workspace_bytes(int B, int Cin, int Cout, int Hi, int Wi) {
+  if (B <= 0 || Cin <= 0 || Cout <= 0 || Hi <= 0 || Wi <= 0) return 0;
+  return bwd_plan(false, B, Cin, Cout, Hi, Wi).part_bytes;
 }
 
-// Backward of gb_deconv4x4s2_wnub_fwd.  gz [B,Cout,2Hi,2Wi] is scratch (pre-activation gradient; may be gout itself when
-// apply_act == 0 and g_bias == NULL: nothing is copied), g_bias
-// [Cout,2Hi,2Wi] or NULL, gx [B,Cin,Hi,Wi] or NULL, gw [Cin,Cout,4,4] is ACCUMULATED into (caller zeroes it) and is the
-// gradient w.r.t. the un-normalised direction tensor v at unit scale (d out / d (scale*v) contracted with v's slot):
-// gw[ci,co,k] = sum x * gz; the caller applies the weight-norm chain rule.
+// Backward of gb_deconv4x4s2_wnub_fwd.  gz [B,Cout,2Hi,2Wi]: scratch for the pre-activation gradient when apply_act,
+// else unused (gout is that gradient); g_bias [Cout,2Hi,2Wi] written, or NULL; gx [B,Cin,Hi,Wi] or NULL; gw
+// [Cin,Cout,4,4] written, or NULL: the gradient w.r.t. the un-normalised direction tensor v at unit scale
+// (d out / d (scale*v) contracted with v's slot), gw[ci,co,k] = sum x * gz; the caller applies the weight-norm chain
+// rule.  workspace: gb_deconv4x4s2_wnub_bwd_workspace_bytes(..) bytes.
 GB_API int gb_deconv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Hi, int Wi, const float* x, const float* v,
                                    const float* scale, const float* out, const float* gout, float slope, int apply_act,
-                                   float* gz, float* g_bias, float* gx, float* gw, void* stream) {
+                                   float* gz, float* g_bias, float* gx, float* gw, void* workspace, void* stream) {
   if (B <= 0 || Cin <= 0 || Cout <= 0 || Hi <= 0 || Wi <= 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
-  const long long per_item = (long long)Cout * 4 * Hi * Wi;
-  // gz == gout with no activation and no separate bias gradient: the pre-activation gradient IS gout (the caller
-  // aliases the untied-bias gradient to it when B == 1) — no 3 x 524 MB copy pass at the 16->125 @1024^2 layer
-  int launches = launch_act_bwd(B, per_item, out, gout, slope, apply_act, gz, g_bias, s);
-  // high-resolution layers (the wide forward's condition, plus 16-byte staging: Wi % 4 == 0): wide backward kernels
-  const bool wide = Cin <= 32 && Wi % 4 == 0 && Wi >= 32 && Hi >= 16 && wide_bwd_enabled();
-  if (gx) launches += launch_bwd_data<false>(wide, B, Cin, Cout, Hi, Wi, gz, v, scale, nullptr, 1.f, 0, gx, s);
-  if (gw) launches += launch_bwd_weight(wide, B, Cin, Cout, Hi, Wi, x, gz, gw, s);
+  int launches = launch_act_bwd(B, (long long)Cout * 4 * Hi * Wi, out, gout, slope, apply_act, gz, g_bias, s);
+  const float* g = apply_act ? gz : gout;
+  const BwdPlan p = bwd_plan(false, B, Cin, Cout, Hi, Wi);
+  if (gx) launches += launch_bwd_data<false>(p.wide, B, Cin, Cout, Hi, Wi, g, v, scale, nullptr, 1.f, 0, gx, s);
+  if (gw) launches += launch_bwd_weight(p, B, Cin, Cout, Hi, Wi, x, g, gw, (float*)workspace, s);
   gb::count_launches(launches);
   GB_CHECK_LAUNCH();
   return 0;
@@ -910,17 +908,26 @@ GB_API int gb_conv4x4s2_wnub_fwd(int B, int Cin, int Cout, int Ho, int Wo, const
   return 0;
 }
 
-// Backward of gb_conv4x4s2_wnub_fwd, with the conventions of gb_deconv4x4s2_wnub_bwd: gz [B,Cout,Ho,Wo] scratch (may be
-// gout itself when apply_act == 0 and g_bias == NULL), g_bias [Cout,Ho,Wo] or NULL, gx [B,Cin,2Ho,2Wo] or NULL,
-// gw [Cout,Cin,4,4] ACCUMULATED at unit scale (gw[o,i,k] = sum gz * x); the caller applies the weight-norm chain rule.
+GB_API size_t gb_conv4x4s2_wnub_bwd_workspace_bytes(int B, int Cin, int Cout, int Ho, int Wo) {
+  if (B <= 0 || Cin <= 0 || Cout <= 0 || Ho <= 0 || Wo <= 0) return 0;
+  return bwd_plan(true, B, Cout, Cin, Ho, Wo).part_bytes;
+}
+
+// Backward of gb_conv4x4s2_wnub_fwd, with the conventions of gb_deconv4x4s2_wnub_bwd: gz [B,Cout,Ho,Wo] scratch when
+// apply_act, else unused; g_bias [Cout,Ho,Wo] or NULL; gx [B,Cin,2Ho,2Wo] or NULL; gw [Cout,Cin,4,4] written at unit
+// scale (gw[o,i,k] = sum gz * x), or NULL; the caller applies the weight-norm chain rule.  workspace:
+// gb_conv4x4s2_wnub_bwd_workspace_bytes(..) bytes.
 GB_API int gb_conv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Ho, int Wo, const float* x, const float* v,
                                  const float* scale, const float* out, const float* gout, float slope, int apply_act,
-                                 float* gz, float* g_bias, float* gx, float* gw, void* stream) {
+                                 float* gz, float* g_bias, float* gx, float* gw, void* workspace, void* stream) {
   if (B <= 0 || Cin <= 0 || Cout <= 0 || Ho <= 0 || Wo <= 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
   int launches = launch_act_bwd(B, (long long)Cout * Ho * Wo, out, gout, slope, apply_act, gz, g_bias, s);
-  if (gx) launches += launch_deconv_fwd<true>(B, Cout, Cin, Ho, Wo, gz, v, scale, nullptr, 1.f, 0, gx, s);
-  if (gw) launches += launch_bwd_weight(Wo % 4 == 0 && Wo >= 32 && Ho >= 16, B, Cout, Cin, Ho, Wo, gz, x, gw, s);
+  const float* g = apply_act ? gz : gout;
+  if (gx) launches += launch_deconv_fwd<true>(B, Cout, Cin, Ho, Wo, g, v, scale, nullptr, 1.f, 0, gx, s);
+  if (gw)
+    launches += launch_bwd_weight(bwd_plan(true, B, Cout, Cin, Ho, Wo), B, Cout, Cin, Ho, Wo, g, x, gw,
+                                  (float*)workspace, s);
   gb::count_launches(launches);
   GB_CHECK_LAUNCH();
   return 0;

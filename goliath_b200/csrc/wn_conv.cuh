@@ -1,7 +1,8 @@
 // goliath_b200/csrc/wn_conv.cuh — the grouped, weight-normalised KxK convolution (K = 1 | 3, pad (K-1)/2, stride
 // S = 1 | 2) that the stride-1 layer (conv_wnub.cu) and the body's residual blocks (upconv_wnub.cu, downconv_wnub.cu)
 // are made of, fp32 SIMT (sm_90a): the forward with its epilogue fused, the data gradient, the weight gradient and the
-// activation / bias backward.  Those files hold only launchers and the C ABI.
+// activation / bias backward.  Those files hold only launchers and the C ABI.  The stride-2 4x4 layers (deconv_wnub.cu)
+// keep their own tiles and use the activation backward, the batch sum and the ordered weight-gradient reduction.
 //
 // The weight-norm scale is per output channel and applied in the epilogue (forward) or to the staged weights (data
 // gradient); the weight gradient is that of the effective weight at unit scale, and the caller finishes the chain rule.
@@ -343,6 +344,31 @@ __global__ void __launch_bounds__(256) chan_sum_kernel(int B, int C, int HW, con
   if (threadIdx.x == 0) out[c] = s[0];
 }
 
+// The end of a weight-gradient CTA of 8 warps whose lanes each hold acc[4][KK] (4 input channels x KK taps of one
+// output channel): the warps are added in warp order through s_r [32][4 KK + 1], then every (lane, a, k) sum is handed
+// to store(lane, a, k, value), which maps it to its place in the CTA's partial.  The first step begins while other
+// warps may still be in their main loop, so s_r must not alias anything they read.
+template <int KK, class Store>
+__device__ __forceinline__ void store_warp_ordered_sums(const float (&acc)[4][KK], float* s_r, Store store) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int w = 0; w < 8; ++w) {
+    if (warp == w) {
+#pragma unroll
+      for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int k = 0; k < KK; ++k) {
+          float& r = s_r[lane * (4 * KK + 1) + a * KK + k];
+          r = (w ? r : 0.f) + acc[a][k];
+        }
+    }
+    __syncthreads();
+  }
+  for (int i = threadIdx.x; i < 32 * 4 * KK; i += 256) {
+    const int l = i / (4 * KK), a = (i / KK) % 4, k = i % KK;
+    store(l, a, k, s_r[l * (4 * KK + 1) + a * KK + k]);
+  }
+}
+
 // Weight gradient of a grouped KxK convolution with stride S and pad (K-1)/2, at unit scale:
 //   gw[o, i_local, ky, kx] = sum_{b,y,x} gz[b,o,y,x] * in[b, g*cin_g + i_local, S y + ky - P, S x + kx - P]
 // CTA blockIdx.x sums its share of the (item, tile) list; its eight warps are added in warp order through shared
@@ -404,21 +430,11 @@ __global__ void __launch_bounds__(256)
           for (int a = 0; a < 4; ++a) acc[a][ky * K + kx] += s_x[cig * 4 + a][py * S + ky][px * S + kx] * gv;
     }
   }
-  for (int w = 0; w < 8; ++w) {
-    if (warp == w) {
-#pragma unroll
-      for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int k = 0; k < KK; ++k) s_r[lane][a * KK + k] = (w ? s_r[lane][a * KK + k] : 0.f) + acc[a][k];
-    }
-    __syncthreads();
-  }
   float* dst = part + (size_t)blockIdx.x * Cout * cin_g * KK;
-  for (int i = tid; i < 32 * 4 * KK; i += 256) {
-    const int l = i / (4 * KK), a = (i / KK) % 4, k = i % KK;
+  store_warp_ordered_sums<KK>(acc, &s_r[0][0], [&](int l, int a, int k, float r) {
     const int ci = ci0 + (l >> 3) * 4 + a, co = co0 + (l & 7);
-    if (ci < cin_g && co < cout_g) dst[((size_t)(g * cout_g + co) * cin_g + ci) * KK + k] = s_r[l][a * KK + k];
-  }
+    if (ci < cin_g && co < cout_g) dst[((size_t)(g * cout_g + co) * cin_g + ci) * KK + k] = r;
+  });
 }
 
 __global__ void __launch_bounds__(256) split_sum_kernel(int n_split, int n, const float* __restrict__ part,

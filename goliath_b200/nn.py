@@ -4,9 +4,10 @@ checkpoints load (`weight_v`, `weight_g`, `bias`): `ConvTranspose2dWNUB`, `Linea
 (layers.py:200-204,468-480; SURVEY.md §0.6):  w = g * v / ||v||_F.
 
 The stride-2 4x4 transposed convolution + untied bias + LeakyReLU runs as ONE hand-written sm_90a kernel in the
-forward, and its backward as three more (activation/bias gradient, data gradient, weight gradient) — no cuDNN
-(csrc/deconv_wnub.cu).  The stride-2 4x4 convolution of the RGCA encoder (`Conv2dWNUB(.., 4, 2, 1)`) runs on the same
-kernels with the two sides of the layer exchanged.  Round-1 status: fp32 SIMT kernels; LinearWN is a plain library
+forward, and its backward as up to four more (activation/bias gradient, data gradient, weight gradient as per-CTA
+partials, their sum in CTA order) — no cuDNN, no float atomics, so two runs give the same bits (csrc/deconv_wnub.cu).
+The stride-2 4x4 convolution of the RGCA encoder (`Conv2dWNUB(.., 4, 2, 1)`) runs on the same kernels with the two
+sides of the layer exchanged.  Round-1 status: fp32 SIMT kernels; LinearWN is a plain library
 GEMM (cuBLAS via F.linear).
 
 The body model's residual blocks run as fused blocks instead of layer by layer: `UpConvBlockDeep` (decoder,
@@ -32,8 +33,7 @@ class _Deconv4x4s2WNUB(Function):
         Cout = weight_v.shape[1]
         if weight_v.shape != (Cin, Cout, 4, 4):
             raise RuntimeError("weight_v must be [Cin, Cout, 4, 4]")
-        vnorm = weight_v.norm()
-        scale = (weight_g.reshape(-1) / vnorm).contiguous()
+        scale = _wn_scale(weight_v, weight_g)
         b = None if bias is None else bias.contiguous()
         if b is not None and b.shape != (Cout, 2 * Hi, 2 * Wi):
             raise RuntimeError("untied bias must be [Cout, 2*Hi, 2*Wi]")
@@ -55,32 +55,25 @@ class _Deconv4x4s2WNUB(Function):
         Cout = v.shape[1]
         dev = x.device
         gout = gout.contiguous()
-        vnorm = v.norm()
-        scale = (g.reshape(-1) / vnorm).contiguous()
         # the untied bias has one entry per output element, so with B == 1 its gradient IS the pre-activation gradient:
         # alias instead of writing it a second time; without an activation the pre-activation gradient is gout itself
         alias_bias = ctx.has_bias and B == 1
-        if B == 1 and ctx.slope is None:
-            gz = gout                                    # nothing to compute, nothing to copy
-        else:
-            gz = torch.empty_like(out)                   # scratch: gradient w.r.t. the pre-activation
+        gz = gout if ctx.slope is None else torch.empty_like(out)
         gb = None
         if ctx.has_bias and not alias_bias:
             gb = torch.empty(Cout, 2 * Hi, 2 * Wi, device=dev, dtype=torch.float32)
         gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
-        gw = torch.zeros_like(v)                         # d L / d (effective weight), accumulated by the kernel
+        gw = torch.empty_like(v)
+        L = _lib.lib()
+        ws = torch.empty(L.gb_deconv4x4s2_wnub_bwd_workspace_bytes(B, Cin, Cout, Hi, Wi) // 4, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_deconv4x4s2_wnub_bwd(
-                B, Cin, Cout, Hi, Wi, _lib.ptr(x), _lib.ptr(v), _lib.ptr(scale), _lib.ptr(out), _lib.ptr(gout),
+            _lib.check(L.gb_deconv4x4s2_wnub_bwd(
+                B, Cin, Cout, Hi, Wi, _lib.ptr(x), _lib.ptr(v), _lib.ptr(_wn_scale(v, g)), _lib.ptr(out), _lib.ptr(gout),
                 float(ctx.slope if ctx.slope is not None else 1.0), int(ctx.slope is not None), _lib.ptr(gz), _lib.ptr(gb),
-                _lib.ptr(gx), _lib.ptr(gw), _lib.stream_ptr(dev)), "deconv4x4s2_wnub_bwd")
+                _lib.ptr(gx), _lib.ptr(gw), _lib.ptr(ws), _lib.stream_ptr(dev)), "deconv4x4s2_wnub_bwd")
         if alias_bias:
             gb = gz.view(Cout, 2 * Hi, 2 * Wi)
-        # weight-norm chain rule on the small [Cin,Cout,4,4] tensors:  w = g * v / n,  n = ||v||_F
-        w = g * v / vnorm
-        gg = (gw * v).sum(dim=(0, 2, 3), keepdim=True) / vnorm
-        gv = g * gw / vnorm - (gw * w).sum() * v / (vnorm * vnorm)
-        return gx, gv, gg.view_as(g), gb, None
+        return (gx, *_wn_chain(v, g, gw), gb, None)
 
 
 class ConvTranspose2dWNUB(nn.Module):
@@ -185,7 +178,7 @@ class _Conv4x4s2WN(Function):
         b = None if bias is None else bias.contiguous()
         if b is not None and b.shape != (Cout, Ho, Wo):
             raise RuntimeError("untied bias must be [Cout, H/2, W/2]")
-        scale = (weight_g.reshape(-1) / weight_v.norm()).contiguous()
+        scale = _wn_scale(weight_v, weight_g)
         out = torch.empty(B, Cout, Ho, Wo, device=x.device, dtype=torch.float32)
         with torch.cuda.device(x.device):
             _lib.check(_lib.lib().gb_conv4x4s2_wnub_fwd(
@@ -204,29 +197,25 @@ class _Conv4x4s2WN(Function):
         Cout, Ho, Wo = out.shape[1:]
         dev = x.device
         gout = gout.contiguous()
-        vnorm = v.norm()
-        scale = (g.reshape(-1) / vnorm).contiguous()
         # as in _Deconv4x4s2WNUB: with B == 1 the untied-bias gradient is the pre-activation gradient, and without an
         # activation that is gout itself
         alias_bias = ctx.has_bias and B == 1
-        gz = gout if B == 1 and ctx.slope is None else torch.empty_like(out)
+        gz = gout if ctx.slope is None else torch.empty_like(out)
         gb = None
         if ctx.has_bias and not alias_bias:
             gb = torch.empty(Cout, Ho, Wo, device=dev, dtype=torch.float32)
         gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
-        gw = torch.zeros_like(v)                         # d L / d (effective weight), accumulated by the kernel
+        gw = torch.empty_like(v)
+        L = _lib.lib()
+        ws = torch.empty(L.gb_conv4x4s2_wnub_bwd_workspace_bytes(B, Cin, Cout, Ho, Wo) // 4, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_conv4x4s2_wnub_bwd(
-                B, Cin, Cout, Ho, Wo, _lib.ptr(x), _lib.ptr(v), _lib.ptr(scale), _lib.ptr(out), _lib.ptr(gout),
+            _lib.check(L.gb_conv4x4s2_wnub_bwd(
+                B, Cin, Cout, Ho, Wo, _lib.ptr(x), _lib.ptr(v), _lib.ptr(_wn_scale(v, g)), _lib.ptr(out), _lib.ptr(gout),
                 float(ctx.slope if ctx.slope is not None else 1.0), int(ctx.slope is not None), _lib.ptr(gz), _lib.ptr(gb),
-                _lib.ptr(gx), _lib.ptr(gw), _lib.stream_ptr(dev)), "conv4x4s2_wnub_bwd")
+                _lib.ptr(gx), _lib.ptr(gw), _lib.ptr(ws), _lib.stream_ptr(dev)), "conv4x4s2_wnub_bwd")
         if alias_bias:
             gb = gz.view(Cout, Ho, Wo)
-        # weight-norm chain rule, g per OUTPUT channel (dim 0), norm over the whole tensor (as _ConvS1WN)
-        w = g * v / vnorm
-        gg = (gw * v).sum(dim=(1, 2, 3), keepdim=True) / vnorm
-        gv = g * gw / vnorm - (gw * w).sum() * v / (vnorm * vnorm)
-        return gx, gv, gg.view_as(g), gb, None
+        return (gx, *_wn_chain(v, g, gw), gb, None)
 
 
 class Conv2dWNUB(nn.Module):
@@ -366,7 +355,7 @@ def tower_forward_tc(tower: nn.Sequential, x: torch.Tensor) -> torch.Tensor:
             cache = getattr(layer, "_tc_cache", None)
             fresh = cache is None or cache[0] != key
             if fresh:
-                scale = (layer.weight_g.reshape(-1) / layer.weight_v.norm()).contiguous()
+                scale = _wn_scale(layer.weight_v, layer.weight_g)
                 ws = torch.empty(L.gb_deconv_tc_weight_bytes(_pad32(Cin), Cout) // 4, device=dev) if tc_ok else None
                 layer._tc_cache = (key, scale, ws)
             else:
@@ -453,10 +442,12 @@ def glorot(m: nn.Module, alpha: float = 1.0) -> None:
 
 
 def _wn_chain(v, g, gw):
-    """weight-norm chain rule (g per output channel, norm over the whole tensor) from the effective-weight gradient"""
+    """weight-norm chain rule (g per output channel, norm over the whole tensor) from the effective-weight gradient.
+    g has v's rank with extent 1 outside the output-channel dimension (dim 0 of a convolution's v, dim 1 of a
+    transposed convolution's); g's gradient sums over those dimensions."""
     vnorm = v.norm()
     w = g * v / vnorm
-    gg = (gw * v).sum(dim=tuple(range(1, v.dim())), keepdim=True) / vnorm
+    gg = (gw * v).sum(dim=tuple(d for d in range(v.dim()) if g.shape[d] == 1), keepdim=True) / vnorm
     gv = g * gw / vnorm - (gw * w).sum() * v / (vnorm * vnorm)
     return gv, gg.view_as(g)
 

@@ -518,11 +518,14 @@ int gb_deconv4x4s2_wnub_fwd(int B, int Cin, int Cout, int Hi, int Wi, const floa
                             void* stream);
 
 /* backward of the above (replaces the cuDNN backward-data / backward-filter calls autograd makes for
- * layers.py:380-396).  gz [B,Cout,2Hi,2Wi] scratch; g_bias [Cout,2Hi,2Wi] or NULL; gx [B,Cin,Hi,Wi] or NULL;
- * gw [Cin,Cout,4,4] = dL/d(effective weight), ACCUMULATED (caller zeroes it and applies the weight-norm chain rule). */
+ * layers.py:380-396).  gz [B,Cout,2Hi,2Wi] scratch when apply_act, else unused (may be NULL); g_bias [Cout,2Hi,2Wi]
+ * written, or NULL; gx [B,Cin,Hi,Wi] or NULL; gw [Cin,Cout,4,4] = dL/d(effective weight at unit scale) written (the
+ * caller applies the weight-norm chain rule).  Every sum runs in a fixed order (no float atomics), so the gradients
+ * are bitwise repeatable.  `workspace`: gb_deconv4x4s2_wnub_bwd_workspace_bytes(B, Cin, Cout, Hi, Wi) bytes. */
+size_t gb_deconv4x4s2_wnub_bwd_workspace_bytes(int B, int Cin, int Cout, int Hi, int Wi);
 int gb_deconv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Hi, int Wi, const float* x, const float* v,
                             const float* scale, const float* out, const float* gout, float slope, int apply_act,
-                            float* gz, float* g_bias, float* gx, float* gw, void* stream);
+                            float* gz, float* g_bias, float* gx, float* gw, void* workspace, void* stream);
 
 /* replaces conv2d + untied-bias add (ca_code/nn/layers.py:276-327) + the LeakyReLU that follows each
  * la.Conv2dWNUB(cin, cout, h, w, 4, 2, 1) of the RGCA texture encoder (ca_code/models/rgca.py:281-298) for k=4, s=2,
@@ -532,12 +535,14 @@ int gb_deconv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Hi, int Wi, const floa
 int gb_conv4x4s2_wnub_fwd(int B, int Cin, int Cout, int Ho, int Wo, const float* x, const float* v,
                           const float* scale, const float* bias, float slope, int apply_act, float* out, void* stream);
 
-/* backward of the above, with the conventions of gb_deconv4x4s2_wnub_bwd.  gz [B,Cout,Ho,Wo] scratch; g_bias
- * [Cout,Ho,Wo] or NULL; gx [B,Cin,2Ho,2Wo] or NULL; gw [Cout,Cin,4,4] = dL/d(effective weight), ACCUMULATED (caller
- * zeroes it and applies the weight-norm chain rule). */
+/* backward of the above, with the conventions of gb_deconv4x4s2_wnub_bwd.  gz [B,Cout,Ho,Wo] scratch when
+ * apply_act, else unused; g_bias [Cout,Ho,Wo] written, or NULL; gx [B,Cin,2Ho,2Wo] or NULL; gw [Cout,Cin,4,4] =
+ * dL/d(effective weight at unit scale) written (the caller applies the weight-norm chain rule).  Bitwise repeatable.
+ * `workspace`: gb_conv4x4s2_wnub_bwd_workspace_bytes(B, Cin, Cout, Ho, Wo) bytes. */
+size_t gb_conv4x4s2_wnub_bwd_workspace_bytes(int B, int Cin, int Cout, int Ho, int Wo);
 int gb_conv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Ho, int Wo, const float* x, const float* v,
                           const float* scale, const float* out, const float* gout, float slope, int apply_act,
-                          float* gz, float* g_bias, float* gx, float* gw, void* stream);
+                          float* gz, float* g_bias, float* gx, float* gw, void* workspace, void* stream);
 
 /* ---- tensor-core (wgmma + TMA) forward of the same layer, inference path; Cin_pad % 32 == 0,
  * Cout % 16 == 0, 16 <= Cout <= 256.  Activations are NHWC split into a tf32 "hi" part and the fp32 remainder "lo"

@@ -75,6 +75,12 @@ def test_host_side_sizing_functions():
     assert small >= 300_000 * (6 * 4 + 48)                   # keys/ids ping-pong + rank_of + by-rank records
     assert small % 256 == 0
     assert L.gb_tile_schedule_ints(T) == T + 132 + 1         # one queue per SM of an H100 + the draw counter
+    # the stride-2 4x4 layers' weight-gradient partials: at least one [Cin, Cout, 4, 4] per layer, none for no work
+    for B, Cin, Cout, H, W in ((1, 16, 125, 64, 48), (2, 264, 40, 8, 8), (1, 256, 256, 16, 16), (1, 3, 5, 17, 33)):
+        assert L.gb_deconv4x4s2_wnub_bwd_workspace_bytes(B, Cin, Cout, H, W) >= Cin * Cout * 16 * 4
+        assert L.gb_conv4x4s2_wnub_bwd_workspace_bytes(B, Cin, Cout, H, W) >= Cin * Cout * 16 * 4
+    assert L.gb_deconv4x4s2_wnub_bwd_workspace_bytes(0, 16, 125, 64, 48) == 0
+    assert L.gb_conv4x4s2_wnub_bwd_workspace_bytes(1, 3, 32, 0, 512) == 0
     before = L.gb_get_blend_mode()
     try:
         for m in (0, 1, 2, 3, 4):

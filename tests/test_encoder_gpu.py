@@ -62,7 +62,7 @@ CASES = ([s + (0.2, True, s[1] != 3) for s in ENCODER_LAYERS] + [
 @pytest.mark.parametrize("B,Cin,Cout,Ho,Wo,slope,has_bias,need_gx", CASES)
 def test_conv4x4s2_vs_torch(cuda, B, Cin, Cout, Ho, Wo, slope, has_bias, need_gx):
     """Forward and every gradient of the fused stride-2 layer against torch fp64 conv2d autograd on the CPU of the
-    reference formula (layers.py:200-204,303-327)."""
+    reference formula (layers.py:200-204,303-327); two runs on the same inputs give the same bits."""
     from goliath_b200 import nn as gnn
 
     gen = torch.Generator().manual_seed(Cin * 13 + Cout + Wo)
@@ -85,21 +85,26 @@ def test_conv4x4s2_vs_torch(cuda, B, Cin, Cout, Ho, Wo, slope, has_bias, need_gx
         y = F.leaky_relu(y, slope)
     y.backward(go.double())
     layer = layer.to(cuda)
-    xc = x.to(cuda).requires_grad_(need_gx)
-    yc = layer(xc, slope=slope)
-    yc.backward(go.to(cuda))
+    runs = []
+    for _ in range(2):
+        layer.zero_grad(set_to_none=True)
+        xc = x.to(cuda).requires_grad_(need_gx)
+        yc = layer(xc, slope=slope)
+        yc.backward(go.to(cuda))
+        checks = [("weight_v", layer.weight_v.grad, v.grad), ("weight_g", layer.weight_g.grad, g.grad)]
+        if has_bias:
+            checks.append(("bias", layer.bias.grad, bias.grad))
+        if need_gx:
+            checks.append(("x", xc.grad, xr.grad))
+        else:
+            assert xc.grad is None
+        runs.append(checks)
     what = "(%d, %d, %d, %d, %d)" % (B, Cin, Cout, Ho, Wo)
     assert_close(t2n(yc), y.detach().numpy(), rtol=1e-4, atol=1e-5 * float(y.abs().max()), what="forward " + what)
-    checks = [("weight_v", layer.weight_v.grad, v.grad), ("weight_g", layer.weight_g.grad, g.grad)]
-    if has_bias:
-        checks.append(("bias", layer.bias.grad, bias.grad))
-    if need_gx:
-        checks.append(("x", xc.grad, xr.grad))
-    else:
-        assert xc.grad is None
-    for name, got, want in checks:
+    for (name, got, want), (_, again, _) in zip(*runs):
         want = want.numpy()
         assert_close(t2n(got), want, rtol=2e-4, atol=2e-5 * float(np.abs(want).max()), what="grad %s %s" % (name, what))
+        assert torch.equal(got, again), "grad %s %s differs between two runs" % (name, what)
 
 
 def _encoder_from_recipe(cuda, n_embs, n_verts, batch):

@@ -58,12 +58,13 @@ def test_deconv_kernel_vs_torch(cuda, shape):
 
 @pytest.mark.parametrize("shape,slope", [((1, 16, 125, 64, 48), None), ((1, 16, 125, 64, 48), 0.2), ((2, 32, 16, 32, 64), 0.2),
                                          ((1, 8, 12, 24, 36), 0.2), ((1, 20, 6, 16, 32), None), ((1, 3, 5, 17, 33), 0.2),
-                                         ((2, 264, 40, 8, 8), 0.2)])
+                                         ((2, 264, 40, 8, 8), 0.2), ((2, 40, 24, 12, 20), None)])
 def test_deconv_backward_vs_torch(cuda, shape, slope):
     """Every gradient of the fused layer (input, weight_v, weight_g, untied bias) against torch autograd of the reference
     formula in fp64 (layers.py:200-204,380-396): the wide backward kernels (Cin <= 32, Wi % 4 == 0, >= 32 x 16: full and
     partial tiles, one and two channel blocks, batch 2, with and without the fused LeakyReLU, incl. the B == 1 aliasing of
-    the bias gradient) and the narrow ones."""
+    the bias gradient) and the narrow ones, with weight gradients split over several CTAs (16 at the first shape, 2 at
+    (2, 264, 40, 8, 8)).  Two runs on the same inputs give the same bits."""
     from goliath_b200 import nn as gnn
 
     B, Cin, Cout, Hi, Wi = shape
@@ -84,16 +85,20 @@ def test_deconv_backward_vs_torch(cuda, shape, slope):
     if slope is not None:
         y = torch.nn.functional.leaky_relu(y, slope)
     y.backward(go.double())
-    # ours
+    # ours, twice
     layer = layer.to(cuda)
-    xc = x.to(cuda).requires_grad_()
-    yc = layer(xc, slope=slope)
-    yc.backward(go.to(cuda))
+    runs = []
+    for _ in range(2):
+        layer.zero_grad(set_to_none=True)
+        xc = x.to(cuda).requires_grad_()
+        yc = layer(xc, slope=slope)
+        yc.backward(go.to(cuda))
+        runs.append((xc.grad, layer.weight_v.grad, layer.weight_g.grad, layer.bias.grad))
     assert_close(t2n(yc), y.detach().numpy(), rtol=1e-4, atol=1e-5 * float(y.abs().max()), what="forward")
-    for name, got, want in (("x", xc.grad, xr.grad), ("weight_v", layer.weight_v.grad, v.grad),
-                            ("weight_g", layer.weight_g.grad, g.grad), ("bias", layer.bias.grad, bias.grad)):
+    for name, got, again, want in zip(("x", "weight_v", "weight_g", "bias"), *runs, (xr.grad, v.grad, g.grad, bias.grad)):
         want = want.numpy()
         assert_close(t2n(got), want, rtol=2e-4, atol=2e-5 * float(np.abs(want).max()), what="grad %s %s" % (name, shape))
+        assert torch.equal(got, again), "grad %s %s differs between two runs" % (name, shape)
 
 
 def test_linear_wn_vs_reference(cuda):
