@@ -22,7 +22,9 @@ SIGNATURES = {
     "gb_sg_evaluate_fwd": (_i, [_vp] * 7 + [_i] * 4 + [_vp]),
     "gb_sg_evaluate_bwd": (_i, [_vp] * 10 + [_i] * 4 + [_vp]),
     "gb_project_gaussians_fwd": (_i, [_i, _vp, _vp, _f, _vp, _vp, _f, _f, _f, _f, _i, _i, _i, _f] + [_vp] * 7 + [_vp]),
+    "gb_project_gaussians_fwd_acc": (_i, [_i, _vp, _vp, _f, _vp, _vp, _f, _f, _f, _f, _i, _i, _i, _f] + [_vp] * 8 + [_vp]),
     "gb_project_gaussians_bwd": (_i, [_i, _vp, _vp, _f, _vp, _vp, _f, _f] + [_vp] * 13 + [_vp]),
+    "gb_splat_project_bwd": (_i, [_i, _vp, _vp, _f, _vp, _vp, _f, _f] + [_vp] * 11 + [_vp]),
     "gb_cumsum_workspace_bytes": (_sz, [_i]),
     "gb_cumsum_i32": (_i, [_i, _vp, _vp, _vp, _vp]),
     "gb_map_gaussian_to_intersects": (_i, [_i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
@@ -66,6 +68,8 @@ SIGNATURES = {
     "gb_rasterize_ranked_fwd_lists": (_i, [_i, _i, _i] + [_vp] * 10 + [_vp]),
     "gb_rasterize_ranked_bwd_lists": (_i, [_i, _i, _i] + [_vp] * 14 + [_vp]),
     "gb_rasterize_ranked_fwd_sort_lists": (_i, [_i, _i, _i] + [_vp] * 12 + [_vp]),
+    "gb_rasterize_ranked_fwd_sort_finish": (_i, [_i, _i] + [_vp] * 14 + [_vp]),
+    "gb_rasterize_ranked_bwd_lists_finish": (_i, [_i, _i] + [_vp] * 15 + [_vp]),
     "gb_bin_tiles_ranked": (_i, [_i] + [_vp] * 7 + [_i, _i, _i, _i64] + [_vp, _vp, _i] + [_vp] * 6 + [_vp, _vp]),
     "gb_bin_tiles_buckets": (_i, [_i] + [_vp] * 7 + [_i, _i, _i, _i64] + [_vp] * 8 + [_vp, _vp, _vp]),
     "gb_compute_raydirs_fwd": (_i, [_i, _i, _i] + [_vp] * 5 + [_f] + [_vp] * 3 + [_vp]),

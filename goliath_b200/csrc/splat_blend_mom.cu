@@ -151,16 +151,18 @@ struct FwdSmem<LIST, true> {
   };
 };
 
-template <int C, bool LIST, bool RANKED, bool HITS, bool SORT>
+template <int C, bool LIST, bool RANKED, bool HITS, bool SORT, bool FINISH = false>
 __device__ __forceinline__ void blend_fwd_body(
     int img_w, int img_h, int tbx, const int* order, int sched, const int2* __restrict__ tile_bins,
     const float4* __restrict__ rec /* RANKED: the by-rank table */, const int* __restrict__ ranks /* RANKED only */,
     const float* __restrict__ background, float* __restrict__ final_Ts, int* __restrict__ final_idx,
     float* __restrict__ out_img, int* __restrict__ hit_list, int* __restrict__ hit_count,
     const unsigned* __restrict__ depth_keys /* SORT only */, int* bucket /* SORT only */,
-    int* sorted /* SORT only: depth keys in, ids in blend order out */) {
+    int* sorted /* SORT only: depth keys in, ids in blend order out */,
+    float* __restrict__ alpha_img = nullptr /* FINISH only */, float* __restrict__ depth_img = nullptr /* FINISH only */) {
   static_assert(!HITS || LIST, "hit lists are the LIST variant's per-stage lists");
   static_assert(!SORT || (LIST && RANKED && HITS), "the sorting forward is the ranked hit-list forward");
+  static_assert(!FINISH || C == 4, "the finished view is rgb + depth");
   __shared__ __align__(128) FwdSmem<LIST, SORT> sm;
   float4 (&s_rec)[kFwdStages][kStageRecs * 3] = sm.f.rec;
   auto& s_hits = sm.f.hits;
@@ -417,7 +419,17 @@ __device__ __forceinline__ void blend_fwd_body(
     const size_t pix = (size_t)pyi * img_w + pxi;
     final_Ts[pix] = T;
     final_idx[pix] = cur_idx;
-    if (C == 4) {
+    if (FINISH) {
+      // render_finish.cu's finish_fwd_kernel on the pixel in registers, alpha = 1 - T as torch's rsub computes it:
+      // out_img is rgb [3,H,W], the depth channel's background is background[0] (the 4-channel blend's bg[3])
+      const size_t P = (size_t)img_w * img_h;
+      out_img[pix] = acc[0] + T * background[0];
+      out_img[P + pix] = acc[1] + T * background[1];
+      out_img[2 * P + pix] = acc[2] + T * background[2];
+      const float a = 1.f - T;
+      alpha_img[pix] = a;
+      depth_img[pix] = (acc[3] + T * background[0]) / fminf(fmaxf(a, 0.05f), 1.f);
+    } else if (C == 4) {
       reinterpret_cast<float4*>(out_img)[pix] =
           make_float4(acc[0] + T * background[0], acc[1] + T * background[1], acc[2] + T * background[2],
                       acc[3] + T * background[3]);
@@ -441,15 +453,18 @@ __global__ void __launch_bounds__(kFwdThreads) blend_fwd_ilp_kernel(
 }
 
 // The sorting forward.  The sort's 15 keys per thread need more than the 56 registers of four CTAs per SM: three CTAs
-// (72 registers, 864 threads) hold 396 tiles at a time.
-template <int C>
+// (72 registers, 864 threads) hold 396 tiles at a time.  FINISH: the view's rgb [3,H,W], alpha [H,W] and depth [H,W]
+// instead of the 4-channel image (background holds 3 floats).
+template <int C, bool FINISH = false>
 __global__ void __launch_bounds__(kFwdThreads, 3) blend_fwd_sort_kernel(
     int img_w, int img_h, int tbx, const int* order, const int2* __restrict__ tile_bins, const float4* __restrict__ rec,
     const float* __restrict__ background, float* __restrict__ final_Ts, int* __restrict__ final_idx,
     float* __restrict__ out_img, int* __restrict__ hit_list, int* __restrict__ hit_count,
-    const unsigned* __restrict__ depth_keys, int* bucket, int* sorted) {
-  blend_fwd_body<C, true, true, true, true>(img_w, img_h, tbx, order, 0, tile_bins, rec, nullptr, background, final_Ts,
-                                            final_idx, out_img, hit_list, hit_count, depth_keys, bucket, sorted);
+    const unsigned* __restrict__ depth_keys, int* bucket, int* sorted, float* __restrict__ alpha_img = nullptr,
+    float* __restrict__ depth_img = nullptr) {
+  blend_fwd_body<C, true, true, true, true, FINISH>(img_w, img_h, tbx, order, 0, tile_bins, rec, nullptr, background,
+                                                    final_Ts, final_idx, out_img, hit_list, hit_count, depth_keys,
+                                                    bucket, sorted, alpha_img, depth_img);
 }
 
 // ------------------------------------------------------------------ backward
@@ -829,14 +844,19 @@ __global__ void __launch_bounds__(1024) order_items_kernel(int n_items, int* __r
   }
 }
 
-template <int C>
+// FINISH: v_output is the gradient of the finished view's rgb [3,H,W] (may be NULL), g_depth [H,W] (may be NULL) that of
+// its depth, and each pixel's 4-vector is formed in registers with render_finish.cu's finish_bwd_kernel arithmetic
+// (alpha_img: the forward's alpha).  background holds 3 floats, the depth channel's is background[0].
+template <int C, bool FINISH = false>
 __global__ void __launch_bounds__(kListThreads, 6) blend_bwd_lists_kernel(
     int img_w, int img_h, int tbx, int n_items, const int2* __restrict__ tile_bins, const int* __restrict__ hit_list,
     const int* __restrict__ hit_count, int* draw /* hit_count + n_items */,
     const int* __restrict__ ranks, const float4* __restrict__ rec, const float* __restrict__ background,
     const float* __restrict__ final_Ts, const int* __restrict__ final_idx, const float* __restrict__ v_output,
     const float* __restrict__ v_output_alpha, float* __restrict__ v_xy, float* __restrict__ v_conic,
-    float* __restrict__ v_colors, float* __restrict__ v_opacity) {
+    float* __restrict__ v_colors, float* __restrict__ v_opacity, const float* __restrict__ g_depth = nullptr,
+    const float* __restrict__ alpha_img = nullptr) {
+  static_assert(!FINISH || C == 4, "the finished view is rgb + depth");
   __shared__ __align__(16) float4 s_e[kListWarps][2][kChunk * 3];  // entries: the gathered records
   __shared__ __align__(8) int2 s_ig[kListWarps][2][kChunk];        // (sorted index, Gaussian id) of each entry
   __shared__ float2 s_m[kListWarps][kChunk * kMStride];            // (fac, v_sigma) of each (hit, pixel)
@@ -896,24 +916,36 @@ __global__ void __launch_bounds__(kListThreads, 6) blend_bwd_lists_kernel(
       }
       cp_async_commit();
     };
-    load_next(0);
-    gather(0);
-
+    // the pixel loads go out first: their latency hides behind the list -> id -> gather chain of chunk 0
     const float T_final = inside ? final_Ts[pix] : 1.f;
     float T = T_final;
     float bufv = 0.f;  // (colour accumulated behind the current Gaussian) . v_out
     const int bin_final = inside ? final_idx[pix] : -1;
     float vo[4] = {0.f, 0.f, 0.f, 0.f};
-    float voa = 0.f;
+    float voa = 0.f, a_pix = 1.f;
     if (inside) {
+      if (FINISH) {
+        const size_t P = (size_t)img_w * img_h;
+        if (v_output) {
+          vo[0] = v_output[pix];
+          vo[1] = v_output[P + pix];
+          vo[2] = v_output[2 * P + pix];
+        }
+        if (g_depth) vo[3] = g_depth[pix];
+        a_pix = alpha_img[pix];
+      } else {
 #pragma unroll
-      for (int c = 0; c < C; ++c) vo[c] = v_output[pix * C + c];
+        for (int c = 0; c < C; ++c) vo[c] = v_output[pix * C + c];
+      }
       voa = v_output_alpha ? v_output_alpha[pix] : 0.f;  // NULL = no gradient through alpha
     }
+    load_next(0);
+    gather(0);
+    if (FINISH) vo[3] = vo[3] / fminf(fmaxf(a_pix, 0.05f), 1.f);  // 0 without g_depth
     VO[lane] = make_float4(vo[0], vo[1], vo[2], vo[3]);
     float bgdot = 0.f;
 #pragma unroll
-    for (int c = 0; c < C; ++c) bgdot += background[c] * vo[c];
+    for (int c = 0; c < C; ++c) bgdot += background[FINISH && c == 3 ? 0 : c] * vo[c];
     const float tfc = T_final * (voa - bgdot);  // the two T_final * ra terms of v_alpha share it
     if (nchunks > 1) load_next(1);
 
@@ -1538,18 +1570,19 @@ static int launch_fwd_any(int img_h, int img_w, int channels, const int32_t* til
   return 0;
 }
 
-// the sorting forward (SORT): gb_rasterize_ranked_fwd_sort_lists
+// the sorting forward (SORT): gb_rasterize_ranked_fwd_sort_lists, and with alpha_img (4 channels only) the finishing
+// one, gb_rasterize_ranked_fwd_sort_finish
 static int launch_fwd_sort(int img_h, int img_w, int channels, const int32_t* tile_bins, const int32_t* tile_order,
                            const float* depths, int32_t* bucket, int32_t* ranks, const float* records,
                            const float* background, float* out_img, float* final_Ts, int32_t* final_idx,
-                           int32_t* hit_list, int32_t* hit_count, cudaStream_t s) {
+                           int32_t* hit_list, int32_t* hit_count, cudaStream_t s, float* alpha_img = nullptr,
+                           float* depth_img = nullptr) {
   const int tbx = gb::cdiv(img_w, 16), tby = gb::cdiv(img_h, 16);
-#define GB_FWD_SORT(CC)                                                                                                 \
-  blend_fwd_sort_kernel<CC><<<tbx * tby, kFwdThreads, 0, s>>>(img_w, img_h, tbx, tile_order, (const int2*)tile_bins,     \
-                                                            (const float4*)records, background, final_Ts, final_idx,    \
-                                                            out_img, hit_list, hit_count, (const unsigned*)depths,      \
-                                                            bucket, ranks)
-  if (channels == 3) GB_FWD_SORT(3); else GB_FWD_SORT(4);
+#define GB_FWD_SORT(CC, FF)                                                                                             \
+  blend_fwd_sort_kernel<CC, FF><<<tbx * tby, kFwdThreads, 0, s>>>(                                                     \
+      img_w, img_h, tbx, tile_order, (const int2*)tile_bins, (const float4*)records, background, final_Ts, final_idx,  \
+      out_img, hit_list, hit_count, (const unsigned*)depths, bucket, ranks, alpha_img, depth_img)
+  if (alpha_img) GB_FWD_SORT(4, true); else if (channels == 3) GB_FWD_SORT(3, false); else GB_FWD_SORT(4, false);
 #undef GB_FWD_SORT
   gb::count_launches(1);
   GB_CHECK_LAUNCH();
@@ -1591,18 +1624,21 @@ static int launch_bwd_lists(int img_h, int img_w, int channels, const int32_t* r
                             const int32_t* hit_list, int32_t* hit_count, const float* records,
                             const float* background, const float* final_Ts, const int32_t* final_idx,
                             const float* v_output, const float* v_output_alpha, float* v_xy, float* v_conic,
-                            float* v_colors, float* v_opacity, cudaStream_t s) {
+                            float* v_colors, float* v_opacity, cudaStream_t s, bool finish = false,
+                            const float* g_depth = nullptr, const float* alpha_img = nullptr) {
   const int tbx = gb::cdiv(img_w, 16), tby = gb::cdiv(img_h, 16);
   const int n_items = 8 * tbx * tby;
   int dev = 0;
   GB_CUDA(cudaGetDevice(&dev));
   // persistent grid: as many CTAs as fit on the device at once, each warp drawing items until they run out
-  static int resident[64][2] = {};
+  static int resident[64][3] = {};
   int uncached = 0;
-  int& per_sm = (dev >= 0 && dev < 64) ? resident[dev][channels == 4] : uncached;
+  int& per_sm = (dev >= 0 && dev < 64) ? resident[dev][finish ? 2 : channels == 4] : uncached;
   if (per_sm == 0) {
     int n = 0, sms = 0;
-    if (channels == 4)
+    if (finish)
+      GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, blend_bwd_lists_kernel<4, true>, kListThreads, 0));
+    else if (channels == 4)
       GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, blend_bwd_lists_kernel<4>, kListThreads, 0));
     else
       GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, blend_bwd_lists_kernel<3>, kListThreads, 0));
@@ -1611,12 +1647,12 @@ static int launch_bwd_lists(int img_h, int img_w, int channels, const int32_t* r
   }
   const int grid = min(per_sm, gb::cdiv(n_items, kListWarps));
   order_items_kernel<<<1, 1024, 0, s>>>(n_items, hit_count);
-#define GB_BWD_LISTS(CC)                                                                                                \
-  blend_bwd_lists_kernel<CC><<<grid, kListThreads, 0, s>>>(                                                             \
+#define GB_BWD_LISTS(CC, FF)                                                                                            \
+  blend_bwd_lists_kernel<CC, FF><<<grid, kListThreads, 0, s>>>(                                                         \
       img_w, img_h, tbx, n_items, (const int2*)tile_bins, hit_list, hit_count, hit_count + n_items, ranks,              \
       (const float4*)records, background, final_Ts, final_idx, v_output, v_output_alpha, v_xy, v_conic, v_colors,       \
-      v_opacity)
-  if (channels == 3) GB_BWD_LISTS(3); else GB_BWD_LISTS(4);
+      v_opacity, g_depth, alpha_img)
+  if (finish) GB_BWD_LISTS(4, true); else if (channels == 3) GB_BWD_LISTS(3, false); else GB_BWD_LISTS(4, false);
 #undef GB_BWD_LISTS
   gb::count_launches(2);
   GB_CHECK_LAUNCH();
@@ -1691,6 +1727,24 @@ GB_API int gb_rasterize_ranked_fwd_sort_lists(int img_h, int img_w, int channels
   return gbblend::launch_fwd_sort(img_h, img_w, channels, tile_bins, tile_order, depths, bucket, ranks_keys, rec_by_rank,
                                   background, out_img, final_Ts, final_idx, hit_list, hit_count, (cudaStream_t)stream);
 }
+// gb_rasterize_ranked_fwd_sort_lists (4 channels) that writes the finished view instead of the 4-channel image: rgb
+// [3,H,W] = colour + T background, alpha [H,W] = 1 - T and depth [H,W] = (depth channel + T background[0]) /
+// clamp(alpha, 0.05, 1), bit for bit what gb_render_finish_fwd makes of the 4-channel image and 1 - final_Ts.
+// background holds 3 floats.  final_Ts, final_idx, ranks_keys, hit_list and hit_count are those of
+// gb_rasterize_ranked_fwd_sort_lists.
+GB_API int gb_rasterize_ranked_fwd_sort_finish(int img_h, int img_w, const int32_t* tile_bins,
+                                               const int32_t* tile_order, const float* depths, int32_t* bucket,
+                                               int32_t* ranks_keys, const float* rec_by_rank, const float* background,
+                                               float* rgb, float* alpha, float* depth, float* final_Ts,
+                                               int32_t* final_idx, int32_t* hit_list, int32_t* hit_count,
+                                               void* stream) {
+  if (img_h <= 0 || img_w <= 0) return 0;
+  if (!depths || !bucket || !ranks_keys || !hit_list || !hit_count || !rgb || !alpha || !depth)
+    return (int)cudaErrorInvalidValue;
+  return gbblend::launch_fwd_sort(img_h, img_w, 4, tile_bins, tile_order, depths, bucket, ranks_keys, rec_by_rank,
+                                  background, rgb, final_Ts, final_idx, hit_list, hit_count, (cudaStream_t)stream,
+                                  alpha, depth);
+}
 GB_API int gb_rasterize_ranked_bwd_lists(int img_h, int img_w, int channels, const int32_t* ranks_sorted,
                                          const int32_t* tile_bins, const int32_t* hit_list, int32_t* hit_count,
                                          const float* rec_by_rank, const float* background, const float* final_Ts,
@@ -1701,6 +1755,22 @@ GB_API int gb_rasterize_ranked_bwd_lists(int img_h, int img_w, int channels, con
   return gbblend::launch_bwd_lists(img_h, img_w, channels, ranks_sorted, tile_bins, hit_list, hit_count,
                                    rec_by_rank, background, final_Ts, final_idx, v_output, v_output_alpha, v_xy, v_conic,
                                    v_colors, v_opacity, (cudaStream_t)stream);
+}
+// gb_rasterize_ranked_bwd_lists behind gb_rasterize_ranked_fwd_sort_finish: g_rgb [3,H,W] and g_depth [H,W] (either
+// may be NULL) are the gradients of the finished view, alpha [H,W] the forward's alpha (it takes no gradient).  The
+// accumulated gradients are those of gb_render_finish_bwd + gb_rasterize_ranked_bwd_lists, up to the order of the
+// atomic adds.  background holds 3 floats.
+GB_API int gb_rasterize_ranked_bwd_lists_finish(int img_h, int img_w, const int32_t* ranks_sorted,
+                                                const int32_t* tile_bins, const int32_t* hit_list, int32_t* hit_count,
+                                                const float* rec_by_rank, const float* background,
+                                                const float* final_Ts, const int32_t* final_idx, const float* alpha,
+                                                const float* g_rgb, const float* g_depth, float* v_xy, float* v_conic,
+                                                float* v_colors, float* v_opacity, void* stream) {
+  if (img_h <= 0 || img_w <= 0) return 0;
+  if (!ranks_sorted || !hit_list || !hit_count || !alpha) return (int)cudaErrorInvalidValue;
+  return gbblend::launch_bwd_lists(img_h, img_w, 4, ranks_sorted, tile_bins, hit_list, hit_count, rec_by_rank,
+                                   background, final_Ts, final_idx, g_rgb, nullptr, v_xy, v_conic, v_colors, v_opacity,
+                                   (cudaStream_t)stream, true, g_depth, alpha);
 }
 
 // ---------------------------------------------------------------- four lighting conditions per pass (OLAT), C ABI

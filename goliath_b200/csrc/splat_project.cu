@@ -68,7 +68,7 @@ __global__ void __launch_bounds__(kBlock) project_fwd_kernel(
     const float4* __restrict__ quats, const float* __restrict__ viewmat, float fx, float fy, float cx, float cy,
     int img_h, int img_w, int block_width, float clip_thresh, float* __restrict__ cov3d, float2* __restrict__ xys,
     float* __restrict__ depths, int* __restrict__ radii, float* __restrict__ conics,
-    float* __restrict__ compensation, int* __restrict__ num_tiles_hit) {
+    float* __restrict__ compensation, int* __restrict__ num_tiles_hit, float* __restrict__ grad_acc) {
   __shared__ float V[12];
   if (threadIdx.x < 12) V[threadIdx.x] = viewmat[threadIdx.x];
   __syncthreads();
@@ -144,41 +144,39 @@ __global__ void __launch_bounds__(kBlock) project_fwd_kernel(
   conics[3 * i] = o_conic[0]; conics[3 * i + 1] = o_conic[1]; conics[3 * i + 2] = o_conic[2];
 #pragma unroll
   for (int k = 0; k < 6; ++k) cov3d[6 * i + k] = c3[k];
+  if (grad_acc) {  // this Gaussian's row of the blend backward's accumulator (layout: gb_project_gaussians_fwd_acc)
+    reinterpret_cast<float4*>(grad_acc)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    reinterpret_cast<float2*>(grad_acc + 4 * (size_t)G)[i] = make_float2(0.f, 0.f);
+    float* vc = grad_acc + 6 * (size_t)G + 3 * (size_t)i;
+    vc[0] = 0.f; vc[1] = 0.f; vc[2] = 0.f;
+    grad_acc[9 * (size_t)G + i] = 0.f;
+  }
 }
 
-__global__ void __launch_bounds__(kBlock) project_bwd_kernel(
-    int G, const float* __restrict__ means3d, const float* __restrict__ scales, float glob_scale,
-    const float4* __restrict__ quats, const float* __restrict__ viewmat, float fx, float fy,
-    const float* __restrict__ cov3d, const int* __restrict__ radii, const float* __restrict__ conics,
-    const float* __restrict__ compensation, const float2* __restrict__ v_xy, const float* __restrict__ v_depth,
-    const float* __restrict__ v_conic, const float* __restrict__ v_compensation, float* __restrict__ v_cov2d,
-    float* __restrict__ v_cov3d, float* __restrict__ v_mean3d, float* __restrict__ v_scale,
-    float4* __restrict__ v_quat) {
-  __shared__ float V[12];
-  if (threadIdx.x < 12) V[threadIdx.x] = viewmat[threadIdx.x];
-  __syncthreads();
-  const int i = blockIdx.x * kBlock + threadIdx.x;
-  if (i >= G) return;
-  float vm[3] = {0.f, 0.f, 0.f}, vc2[3] = {0.f, 0.f, 0.f}, vsc[3] = {0.f, 0.f, 0.f};
-  float vc3[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  float4 vq = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (radii[i] > 0) {
+// The projection backward of Gaussian i (radii[i] > 0) from the gradients of its xy, depth, conic and compensation, in
+// one fixed order of single IEEE roundings; the outputs are zero-initialised by the caller.
+__device__ __forceinline__ void project_bwd_one(int i, const float* V, const float* __restrict__ means3d,
+                                                const float* __restrict__ scales, float glob_scale,
+                                                const float4* __restrict__ quats, float fx, float fy,
+                                                const float* __restrict__ cov3d, const float* __restrict__ conics,
+                                                const float* __restrict__ compensation, float2 gxy, float vzg,
+                                                const float vcon[3], float vcomp, float vm[3], float vc2[3],
+                                                float vc3[6], float vsc[3], float4& vq) {
+  {
     const float px = means3d[3 * i], py = means3d[3 * i + 1], pz = means3d[3 * i + 2];
     const float vx = V[0] * px + V[1] * py + V[2] * pz + V[3];
     const float vy = V[4] * px + V[5] * py + V[6] * pz + V[7];
     const float vz = V[8] * px + V[9] * py + V[10] * pz + V[11];
     const float rw = 1.f / (vz + 1e-6f);
-    const float2 gxy = v_xy[i];
     const float vpx = fx * gxy.x, vpy = fy * gxy.y;
     const float gvx = vpx * rw, gvy = vpy * rw, gvz = -(vpx * vx + vpy * vy) * rw * rw;
     vm[0] = V[0] * gvx + V[4] * gvy + V[8] * gvz;
     vm[1] = V[1] * gvx + V[5] * gvy + V[9] * gvz;
     vm[2] = V[2] * gvx + V[6] * gvy + V[10] * gvz;
-    const float vzg = v_depth[i];
     vm[0] += V[8] * vzg; vm[1] += V[9] * vzg; vm[2] += V[10] * vzg;
 
     const float X00 = conics[3 * i], X01 = conics[3 * i + 1], X11 = conics[3 * i + 2];
-    const float G00 = v_conic[3 * i], G01 = 0.5f * v_conic[3 * i + 1], G11 = v_conic[3 * i + 2];
+    const float G00 = vcon[0], G01 = 0.5f * vcon[1], G11 = vcon[2];
     const float xg00 = X00 * G00 + X01 * G01, xg01 = X00 * G01 + X01 * G11;
     const float xg10 = X01 * G00 + X11 * G01, xg11 = X01 * G01 + X11 * G11;
     const float s00 = -(xg00 * X00 + xg01 * X01), s01 = -(xg00 * X01 + xg01 * X11);
@@ -188,7 +186,7 @@ __global__ void __launch_bounds__(kBlock) project_bwd_kernel(
       const float comp = compensation[i];
       const float inv_det = X00 * X11 - X01 * X01;
       const float omc = 1.f - comp * comp;
-      const float vsq = v_compensation[i] * 0.5f / (comp + 1e-6f);
+      const float vsq = vcomp * 0.5f / (comp + 1e-6f);
       vc2[0] += vsq * (omc * X00 - 0.3f * inv_det);
       vc2[1] += 2.f * vsq * (omc * X01);
       vc2[2] += vsq * (omc * X11 - 0.3f * inv_det);
@@ -251,10 +249,64 @@ __global__ void __launch_bounds__(kBlock) project_bwd_kernel(
     vq.w = 2.f * (x * (VR(2, 0) + VR(0, 2)) + y * (VR(2, 1) + VR(1, 2)) - 2.f * z * (VR(0, 0) + VR(1, 1)) + w * (VR(1, 0) - VR(0, 1)));
 #undef VR
   }
+}
+
+__global__ void __launch_bounds__(kBlock) project_bwd_kernel(
+    int G, const float* __restrict__ means3d, const float* __restrict__ scales, float glob_scale,
+    const float4* __restrict__ quats, const float* __restrict__ viewmat, float fx, float fy,
+    const float* __restrict__ cov3d, const int* __restrict__ radii, const float* __restrict__ conics,
+    const float* __restrict__ compensation, const float2* __restrict__ v_xy, const float* __restrict__ v_depth,
+    const float* __restrict__ v_conic, const float* __restrict__ v_compensation, float* __restrict__ v_cov2d,
+    float* __restrict__ v_cov3d, float* __restrict__ v_mean3d, float* __restrict__ v_scale,
+    float4* __restrict__ v_quat) {
+  __shared__ float V[12];
+  if (threadIdx.x < 12) V[threadIdx.x] = viewmat[threadIdx.x];
+  __syncthreads();
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  if (i >= G) return;
+  float vm[3] = {0.f, 0.f, 0.f}, vc2[3] = {0.f, 0.f, 0.f}, vsc[3] = {0.f, 0.f, 0.f};
+  float vc3[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  float4 vq = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (radii[i] > 0) {
+    project_bwd_one(i, V, means3d, scales, glob_scale, quats, fx, fy, cov3d, conics, compensation, v_xy[i], v_depth[i],
+                    v_conic + 3 * i, v_compensation[i], vm, vc2, vc3, vsc, vq);
+  }
 #pragma unroll
   for (int k = 0; k < 3; ++k) { v_cov2d[3 * i + k] = vc2[k]; v_mean3d[3 * i + k] = vm[k]; v_scale[3 * i + k] = vsc[k]; }
 #pragma unroll
   for (int k = 0; k < 6; ++k) v_cov3d[6 * i + k] = vc3[k];
+  v_quat[i] = vq;
+}
+
+// The fused render's per-Gaussian backward in one pass: the blend's accumulator row (layout:
+// gb_project_gaussians_fwd_acc) -> the colour and opacity gradients (splat_grad_unpack_kernel's products) and, through
+// project_bwd_one, those of the means, scales and rotations.  v_cov2d / v_cov3d are not written.
+__global__ void __launch_bounds__(kBlock) splat_project_bwd_kernel(
+    int G, const float* __restrict__ means3d, const float* __restrict__ scales, float glob_scale,
+    const float4* __restrict__ quats, const float* __restrict__ viewmat, float fx, float fy,
+    const float* __restrict__ cov3d, const int* __restrict__ radii, const float* __restrict__ conics,
+    const float* __restrict__ compensation, const float* __restrict__ opacity, const float* __restrict__ grad_acc,
+    float* __restrict__ v_colors, float* __restrict__ v_opacity, float* __restrict__ v_mean3d,
+    float* __restrict__ v_scale, float4* __restrict__ v_quat) {
+  __shared__ float V[12];
+  if (threadIdx.x < 12) V[threadIdx.x] = viewmat[threadIdx.x];
+  __syncthreads();
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  if (i >= G) return;
+  const float4 c4 = reinterpret_cast<const float4*>(grad_acc)[i];  // (v_rgb, v_depth)
+  const float e = grad_acc[9 * (size_t)G + i];                     // gradient of opacity * compensation
+  v_colors[3 * i] = c4.x; v_colors[3 * i + 1] = c4.y; v_colors[3 * i + 2] = c4.z;
+  v_opacity[i] = e * compensation[i];
+  float vm[3] = {0.f, 0.f, 0.f}, vc2[3] = {0.f, 0.f, 0.f}, vsc[3] = {0.f, 0.f, 0.f};
+  float vc3[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  float4 vq = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (radii[i] > 0) {
+    project_bwd_one(i, V, means3d, scales, glob_scale, quats, fx, fy, cov3d, conics, compensation,
+                    reinterpret_cast<const float2*>(grad_acc + 4 * (size_t)G)[i], c4.w,
+                    grad_acc + 6 * (size_t)G + 3 * (size_t)i, e * opacity[i], vm, vc2, vc3, vsc, vq);
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) { v_mean3d[3 * i + k] = vm[k]; v_scale[3 * i + k] = vsc[k]; }
   v_quat[i] = vq;
 }
 
@@ -271,7 +323,25 @@ GB_API int gb_project_gaussians_fwd(int G, const float* means3d, const float* sc
   if (block_width < 2 || block_width > 16) return (int)cudaErrorInvalidValue;
   project_fwd_kernel<<<gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream>>>(
       G, means3d, scales, glob_scale, (const float4*)quats, viewmat, fx, fy, cx, cy, img_h, img_w, block_width,
-      clip_thresh, cov3d, (float2*)xys, depths, radii, conics, compensation, num_tiles_hit);
+      clip_thresh, cov3d, (float2*)xys, depths, radii, conics, compensation, num_tiles_hit, nullptr);
+  gb::count_launches(1);
+  GB_CHECK_LAUNCH();
+  return 0;
+}
+
+// gb_project_gaussians_fwd that also zeroes grad_acc [10 G] fp32, the accumulator the fused render's blend backward
+// adds into: v_rgbd [G,4] | v_xy [G,2] | v_conic [G,3] | v_opacity_eff [G], each part aligned for the blend's vector
+// reductions.  gb_splat_project_bwd reads it.
+GB_API int gb_project_gaussians_fwd_acc(int G, const float* means3d, const float* scales, float glob_scale,
+                                        const float* quats, const float* viewmat, float fx, float fy, float cx,
+                                        float cy, int img_h, int img_w, int block_width, float clip_thresh,
+                                        float* cov3d, float* xys, float* depths, int32_t* radii, float* conics,
+                                        float* compensation, int32_t* num_tiles_hit, float* grad_acc, void* stream) {
+  if (G <= 0) return 0;
+  if (block_width < 2 || block_width > 16 || !grad_acc) return (int)cudaErrorInvalidValue;
+  project_fwd_kernel<<<gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream>>>(
+      G, means3d, scales, glob_scale, (const float4*)quats, viewmat, fx, fy, cx, cy, img_h, img_w, block_width,
+      clip_thresh, cov3d, (float2*)xys, depths, radii, conics, compensation, num_tiles_hit, grad_acc);
   gb::count_launches(1);
   GB_CHECK_LAUNCH();
   return 0;
@@ -288,6 +358,23 @@ GB_API int gb_project_gaussians_bwd(int G, const float* means3d, const float* sc
   project_bwd_kernel<<<gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream>>>(
       G, means3d, scales, glob_scale, (const float4*)quats, viewmat, fx, fy, cov3d, radii, conics, compensation,
       (const float2*)v_xy, v_depth, v_conic, v_compensation, v_cov2d, v_cov3d, v_mean3d, v_scale, (float4*)v_quat);
+  gb::count_launches(1);
+  GB_CHECK_LAUNCH();
+  return 0;
+}
+
+// Backward of the fused render per Gaussian, after its blend backward: grad_acc as gb_project_gaussians_fwd_acc left it
+// and the blend filled it, opacity [G] and the projection's saved tensors -> v_colors [G,3], v_opacity [G] and
+// v_mean3d / v_scale / v_quat, bit for bit gb_splat_grad_unpack followed by gb_project_gaussians_bwd.
+GB_API int gb_splat_project_bwd(int G, const float* means3d, const float* scales, float glob_scale, const float* quats,
+                                const float* viewmat, float fx, float fy, const float* cov3d, const int32_t* radii,
+                                const float* conics, const float* compensation, const float* opacity,
+                                const float* grad_acc, float* v_colors, float* v_opacity, float* v_mean3d,
+                                float* v_scale, float* v_quat, void* stream) {
+  if (G <= 0) return 0;
+  splat_project_bwd_kernel<<<gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream>>>(
+      G, means3d, scales, glob_scale, (const float4*)quats, viewmat, fx, fy, cov3d, radii, conics, compensation, opacity,
+      grad_acc, v_colors, v_opacity, v_mean3d, v_scale, (float4*)v_quat);
   gb::count_launches(1);
   GB_CHECK_LAUNCH();
   return 0;

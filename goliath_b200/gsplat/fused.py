@@ -21,16 +21,18 @@ _OVERFLOW = {}
 # binning of the sync-free path: "buckets" (csrc/splat_bin_tiles.cu) or "keysort" (csrc/splat_bin.cu, the gsplat-shaped
 # pipeline: cumsum -> keys -> radix sort -> bin edges -> pack); identical outputs, the switch exists for A/B timing
 BINNING = os.environ.get("GOLIATH_B200_BINNING", "buckets")
-# sync-free path as two autograd nodes (projection | binning + blend), see render_fused_split; "0" keeps the single node
+# sync-free path on the bucket binning: "1" runs it as _RenderBuckets (ranked or packed records, see RANKED; with ranked
+# records render_views has the blend kernels finish the view), "0" as _RenderFused (packed records).  The name is
+# kept from when the first choice was two autograd nodes, projection | binning + blend.
 SPLIT = os.environ.get("GOLIATH_B200_RENDER_SPLIT", "1") != "0"
-# records of the two-node path: "ranked" (default: the blend stages records by Gaussian id from the per-Gaussian table,
+# records of the bucket path: "ranked" (default: the blend stages records by Gaussian id from the per-Gaussian table,
 # G x 48 B, with 16-byte cp.async gathers) or "packed" (sorted 48-byte records materialised by the binning's gather,
 # cap x 48 B).  On an H100 the by-id table (14.4 MB at 300k Gaussians) stays in the 50 MB L2 between the binning and
 # the two blends, the sorted records (52 MB on the bench head scene) do not.  Measured on an H100 SXM at a 700 W power
 # limit (scripts/profile_head_step.py): the ranked blends cost ~2 us (forward) and ~10 us (backward) more than the
 # packed ones, the record gather they make unnecessary cost ~50 us, and the bench head step takes 0.557 instead of
-# 0.592 ms.  The ranked path also holds 4x less memory per view for the backward.  "packed" is kept for A/B timing; the
-# single-node path and OLAT always use packed records.
+# 0.592 ms.  The ranked path also holds 4x less memory per view for the backward.  "packed" is kept for A/B timing;
+# _RenderFused and OLAT always use packed records.
 RANKED = os.environ.get("GOLIATH_B200_RECORDS", "ranked") == "ranked"
 
 
@@ -60,7 +62,7 @@ class _BlendPlan(NamedTuple):
     order_len: int  # int32 entries of the tile order
     fwd: object  # gb_rasterize_{sched,packed}_fwd
     bwd: object  # gb_rasterize_{sched,packed}_bwd
-    ranked: bool  # the two-node path blends id-staged records (gb_rasterize_ranked_*, see RANKED)
+    ranked: bool  # _RenderBuckets blends id-staged records (gb_rasterize_ranked_*, see RANKED)
 
 
 def _blend_plan(T, schedule=True):
@@ -231,52 +233,47 @@ class _RenderFused(Function):
         return (g_mean, g_scale, g_quat, v_opacity, v_colors) + (None,) * 11
 
 
-class _ProjectGeom(Function):
-    """First half of the sync-free fused render: projection only (no dependence on the colours)."""
+def _acc_parts(acc, G):
+    """(v_rgbd [G,4], v_xy [G,2], v_conic [G,3], v_opacity_eff [G]): the blend backward's accumulator as
+    gb_project_gaussians_fwd_acc lays it out and zeroes it, and gb_splat_project_bwd reads it."""
+    return acc[:4 * G].view(G, 4), acc[4 * G:6 * G].view(G, 2), acc[6 * G:9 * G].view(G, 3), acc[9 * G:]
+
+
+class _RenderBuckets(Function):
+    """The sync-free render on the bucket binning (csrc/splat_bin_tiles.cu) as one autograd node: projection ->
+    binning -> blend.  The projection kernel also zeroes the blend backward's accumulator, and the backward turns it
+    into every input gradient with one per-Gaussian kernel (gb_splat_project_bwd).  `colors` may still be in flight on
+    another stream: `colors_event` (torch.cuda.Event recorded after the kernel that writes them) is waited for inside
+    the binning, just before the colours are first read.
+
+    `finish` (ranked records only, see RANKED): the blend kernels also finish the view as render._FinishView does, and
+    the node returns (rgb [3,H,W], alpha [1,H,W] (no gradient), depth [1,H,W], radii); without it (out4 [H,W,4],
+    alpha [H,W], radii)."""
 
     @staticmethod
-    def forward(ctx, means3d, scales, quats, viewmat, glob_scale, fx, fy, cx, cy, img_height, img_width, clip_thresh):
-        ins = [t.contiguous() for t in (means3d, scales, quats, viewmat)]
-        for t, n in zip(ins, ("means3d", "scales", "quats", "viewmat")):
+    def forward(ctx, means3d, scales, quats, opacity, colors, viewmat, background, glob_scale, fx, fy, cx, cy,
+                img_height, img_width, clip_thresh, capacity, colors_event, finish):
+        names = ("means3d", "scales", "quats", "opacity", "colors", "viewmat", "background")
+        ins = [t.contiguous() for t in (means3d, scales, quats, opacity, colors, viewmat, background)]
+        for t, n in zip(ins, names):
             _lib.check_input(t, n)
-        means3d, scales, quats, viewmat = ins
-        xys, depths, radii, conics, comp, _, cov3d = _project_fwd(means3d, scales, quats, viewmat, glob_scale, fx, fy,
-                                                                  cx, cy, img_height, img_width, 16, clip_thresh)
-        ctx.save_for_backward(means3d, scales, quats, viewmat, cov3d, radii, conics, comp)
-        ctx.meta = (float(glob_scale), float(fx), float(fy))
-        ctx.mark_non_differentiable(radii)
-        ctx.set_materialize_grads(False)
-        return xys, depths, conics, comp, radii
-
-    @staticmethod
-    def backward(ctx, v_xy, v_depth, v_conic, v_comp, _v_radii):
-        return _project_bwd(*ctx.saved_tensors, *ctx.meta, v_xy, v_depth, v_conic, v_comp) + (None,) * 9
-
-
-class _BinBlend(Function):
-    """Second half: bucket binning + record packing + the 4-channel blend.  `colors` may still be in flight on another
-    stream: `colors_event` (torch.cuda.Event recorded after the kernel that writes them) is waited for inside
-    gb_bin_tiles_pack_ev just before the record gather, the first reader."""
-
-    @staticmethod
-    def forward(ctx, xys, depths, conics, comp, radii, opacity, colors, background, img_height, img_width, capacity,
-                colors_event):
-        opacity, colors, background = opacity.contiguous(), colors.contiguous(), background.contiguous()
-        for t, n in zip((opacity, colors, background), ("opacity", "colors", "background")):
-            _lib.check_input(t, n)
-        G = xys.size(0)
-        dev = xys.device
+        means3d, scales, quats, opacity, colors, viewmat, background = ins
+        G = means3d.size(0)
+        dev = means3d.device
         L = _lib.lib()
         f32 = dict(device=dev, dtype=torch.float32)
         i32 = dict(device=dev, dtype=torch.int32)
         H, W = int(img_height), int(img_width)
-        out4 = torch.empty(H, W, 4, **f32)
-        final_Ts = torch.empty(H, W, **f32)
-        final_idx = torch.empty(H, W, **i32)
-        bg4 = torch.cat([background, background[:1]])
         tb = _tile_bounds(H, W, 16)
         cap = int(capacity)
         plan = _blend_plan(tb[0] * tb[1])
+        if finish and not plan.ranked:
+            raise ValueError("the blend kernels finish the view only with ranked records (see blend_finishes_view)")
+        acc = torch.empty(10 * G, **f32)
+        xys, depths, radii, conics, comp, _, cov3d = _project_fwd(means3d, scales, quats, viewmat, glob_scale, fx, fy,
+                                                                  cx, cy, H, W, 16, clip_thresh, grad_acc=acc)
+        final_Ts = torch.empty(H, W, **f32)
+        final_idx = torch.empty(H, W, **i32)
         ev = None
         if colors_event is not None:
             ev = colors_event.cuda_event
@@ -297,6 +294,7 @@ class _BinBlend(Function):
         bins, order = _bin_tiles(xys, depths, radii, conics, colors, opacity, comp, H, W, cap, plan, outs,
                                  ranked=plan.ranked, colors_ready=ev)
         hit_list = hit_count = None
+        bg = background if finish else torch.cat([background, background[:1]])
         with torch.cuda.device(dev):
             st = _lib.stream_ptr(dev)
             if plan.ranked:
@@ -305,69 +303,109 @@ class _BinBlend(Function):
                 # walks them instead of culling every tile again
                 hit_list = torch.empty(8 * cap, **i32)
                 hit_count = torch.empty(16 * tb[0] * tb[1] + 2, **i32)
-                _lib.check(L.gb_rasterize_ranked_fwd_sort_lists(
-                    H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(depths), _lib.ptr(bucket), _lib.ptr(ranks),
-                    _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(out4), _lib.ptr(final_Ts), _lib.ptr(final_idx),
-                    _lib.ptr(hit_list), _lib.ptr(hit_count), st), "rasterize_ranked_forward")
+                head = (_lib.ptr(bins), _lib.ptr(order), _lib.ptr(depths), _lib.ptr(bucket), _lib.ptr(ranks),
+                        _lib.ptr(records), _lib.ptr(bg))
+                tail = (_lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(hit_list), _lib.ptr(hit_count), st)
+                if finish:
+                    rgb, a_img, depth = torch.empty(3, H, W, **f32), torch.empty(1, H, W, **f32), torch.empty(1, H, W, **f32)
+                    _lib.check(L.gb_rasterize_ranked_fwd_sort_finish(H, W, *head, _lib.ptr(rgb), _lib.ptr(a_img),
+                                                                     _lib.ptr(depth), *tail), "rasterize_ranked_forward")
+                else:
+                    out4 = torch.empty(H, W, 4, **f32)
+                    _lib.check(L.gb_rasterize_ranked_fwd_sort_lists(H, W, 4, *head, _lib.ptr(out4), *tail),
+                               "rasterize_ranked_forward")
             else:
-                _lib.check(plan.fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4),
+                out4 = torch.empty(H, W, 4, **f32)
+                _lib.check(plan.fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg),
                                     _lib.ptr(out4), _lib.ptr(final_Ts), _lib.ptr(final_idx), st),
                            "rasterize_packed_forward")
-        ctx.save_for_backward(opacity, comp, bg4, gids, bins, order, records, final_Ts, final_idx, ranks, hit_list,
-                              hit_count)
-        ctx.meta = (H, W, plan)
+        alpha = a_img if finish else None
+        ctx.save_for_backward(means3d, scales, quats, opacity, viewmat, bg, cov3d, radii, conics, comp, acc, gids, bins,
+                              order, records, final_Ts, final_idx, ranks, hit_list, hit_count, alpha)
+        ctx.meta = (H, W, float(glob_scale), float(fx), float(fy), plan, finish)
+        ctx.acc_used = False
         ctx.set_materialize_grads(False)
-        return out4, 1 - final_Ts
+        if finish:
+            ctx.mark_non_differentiable(a_img, radii)
+            return rgb, a_img, depth, radii
+        ctx.mark_non_differentiable(radii)
+        return out4, 1 - final_Ts, radii
 
     @staticmethod
-    def backward(ctx, v_out4, v_alpha):
-        (opacity, comp, bg4, gids, bins, order, records, final_Ts, final_idx, ranks, hit_list,
-         hit_count) = ctx.saved_tensors
-        H, W, plan = ctx.meta
-
-        def blend(st, *grads):
-            if plan.ranked:
-                _lib.check(_lib.lib().gb_rasterize_ranked_bwd_lists(
-                    H, W, 4, _lib.ptr(ranks), _lib.ptr(bins), _lib.ptr(hit_list),
-                    _lib.ptr(hit_count), _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(final_Ts), _lib.ptr(final_idx),
-                    *map(_lib.ptr, grads), st), "rasterize_ranked_backward")
+    def backward(ctx, *grads):
+        (means3d, scales, quats, opacity, viewmat, bg, cov3d, radii, conics, comp, acc, gids, bins, order, records,
+         final_Ts, final_idx, ranks, hit_list, hit_count, alpha) = ctx.saved_tensors
+        H, W, glob_scale, fx, fy, plan, finish = ctx.meta
+        G = means3d.size(0)
+        dev = means3d.device
+        L = _lib.lib()
+        f32 = dict(device=dev, dtype=torch.float32)
+        if ctx.acc_used:  # a second backward through this graph (retain_graph): the projection zeroed acc only once
+            acc.zero_()
+        ctx.acc_used = True
+        v_col4, v_xy, v_conic, v_opeff = _acc_parts(acc, G)
+        v_colors, v_opacity = torch.empty(G, 3, **f32), torch.empty(G, 1, **f32)
+        g_mean, g_scale, g_quat = torch.empty(G, 3, **f32), torch.empty(G, 3, **f32), torch.empty(G, 4, **f32)
+        accs = tuple(map(_lib.ptr, (v_xy, v_conic, v_col4, v_opeff)))
+        with torch.cuda.device(dev):
+            st = _lib.stream_ptr(dev)
+            if finish:
+                g_rgb, _, g_depth, _ = (None if g is None else g.contiguous() for g in grads)
+                _lib.check(L.gb_rasterize_ranked_bwd_lists_finish(
+                    H, W, _lib.ptr(ranks), _lib.ptr(bins), _lib.ptr(hit_list), _lib.ptr(hit_count), _lib.ptr(records),
+                    _lib.ptr(bg), _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(alpha), _lib.ptr(g_rgb),
+                    _lib.ptr(g_depth), *accs, st), "rasterize_ranked_backward")
             else:
-                _lib.check(plan.bwd(H, W, 4, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records),
-                                    _lib.ptr(bg4), _lib.ptr(final_Ts), _lib.ptr(final_idx), *map(_lib.ptr, grads), st),
-                           "rasterize_packed_backward")
+                v_out4, v_alpha, _ = grads
+                v_out4 = torch.zeros(H, W, 4, **f32) if v_out4 is None else v_out4.contiguous()
+                v_alpha = None if v_alpha is None else v_alpha.contiguous()  # NULL: no gradient through alpha
+                if plan.ranked:
+                    _lib.check(L.gb_rasterize_ranked_bwd_lists(
+                        H, W, 4, _lib.ptr(ranks), _lib.ptr(bins), _lib.ptr(hit_list), _lib.ptr(hit_count),
+                        _lib.ptr(records), _lib.ptr(bg), _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(v_out4),
+                        _lib.ptr(v_alpha), *accs, st), "rasterize_ranked_backward")
+                else:
+                    _lib.check(plan.bwd(H, W, 4, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records),
+                                        _lib.ptr(bg), _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(v_out4),
+                                        _lib.ptr(v_alpha), *accs, st), "rasterize_packed_backward")
+            _lib.check(L.gb_splat_project_bwd(
+                G, _lib.ptr(means3d), _lib.ptr(scales), glob_scale, _lib.ptr(quats), _lib.ptr(viewmat), fx, fy,
+                _lib.ptr(cov3d), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp), _lib.ptr(opacity), _lib.ptr(acc),
+                _lib.ptr(v_colors), _lib.ptr(v_opacity), _lib.ptr(g_mean), _lib.ptr(g_scale), _lib.ptr(g_quat), st),
+                "splat_project_backward")
+        return (g_mean, g_scale, g_quat, v_opacity, v_colors) + (None,) * 13
 
-        v_xy, v_conic, v_colors, v_opacity, v_comp, v_depth = _blend_grads(H, W, v_out4, v_alpha, opacity, comp, blend)
-        return (v_xy, v_depth, v_conic, v_comp, None, v_opacity, v_colors) + (None,) * 5
+
+def _bucket_path(G, capacity):
+    """render_fused takes the sync-free bucket path (_RenderBuckets)."""
+    return (capacity is not None and SPLIT and BINNING == "buckets" and G > 0
+            and bool(_lib.lib().gb_bin_tiles_supported(G)))
 
 
-def render_fused_split(means3d, scales, glob_scale, quats, viewmat, fx, fy, cx, cy, img_height, img_width, opacity, colors,
-                       background, clip_thresh, capacity, colors_event=None):
-    """render_fused(capacity=N) as TWO autograd nodes — projection | binning + blend — with the same kernels.  What the
-    split buys: the projection, the tile counts, the tile buckets and the per-tile sort do not read the colours, so a
-    caller that runs its shade on a side stream (and passes the event recorded after it) gets them beside the shade
-    forward; in the backward autograd finds the projection backward and the shade backward independent (both only need
-    this node's gradients) and issues them on their own streams.  Requires the bucket binning and G >= 1."""
-    xys, depths, conics, comp, radii = _ProjectGeom.apply(means3d, scales, quats, viewmat, glob_scale, fx, fy, cx, cy,
-                                                          img_height, img_width, clip_thresh)
-    out4, alpha = _BinBlend.apply(xys, depths, conics, comp, radii, opacity, colors, background, img_height, img_width,
-                                  capacity, colors_event)
-    return out4, alpha, radii
+def blend_finishes_view(G, capacity):
+    """True when render_fused(..., finish=True) may be called for G Gaussians: the sync-free bucket path with ranked
+    records, whose blend kernels write the finished view."""
+    return _bucket_path(G, capacity) and _blend_plan(1).ranked
 
 
 def render_fused(means3d, scales, glob_scale, quats, viewmat, fx, fy, cx, cy, img_height, img_width, opacity, colors,
-                 background, clip_thresh=0.01, capacity=None, colors_event=None):
+                 background, clip_thresh=0.01, capacity=None, colors_event=None, finish=False):
     """Returns (out4 [H,W,4] = rgb + depth, alpha [H,W], radii [G] i32).  block_width is 16.
 
     capacity=None keeps the reference's behaviour (one host sync to size the intersection buffers exactly).
     capacity=N runs sync-free: buffers hold N intersections, the count stays on the device, nothing blocks the host, and
     the call can be captured in a CUDA graph; if a view ever needs more than N intersections the excess is dropped and
     `check_overflow()` reports it (results of that call are then incomplete — re-run with a larger capacity).  With
-    zero intersections the sync-free path returns alpha = 0, not the reference's alpha = 1 quirk."""
-    if (capacity is not None and SPLIT and BINNING == "buckets" and means3d.size(0) > 0
-            and _lib.lib().gb_bin_tiles_supported(means3d.size(0))):
-        return render_fused_split(means3d, scales, glob_scale, quats, viewmat, fx, fy, cx, cy, img_height, img_width,
-                                  opacity, colors, background, clip_thresh, capacity, colors_event)
-    if colors_event is not None:  # single-node path: the colours must be complete before the first kernel
+    zero intersections the sync-free path returns alpha = 0, not the reference's alpha = 1 quirk.
+
+    finish=True (only where blend_finishes_view holds) returns the finished view instead, as render._FinishView makes it
+    of out4 and alpha: (rgb [3,H,W], alpha [1,H,W] (no gradient), depth [1,H,W] / clamp(alpha, 0.05, 1), radii)."""
+    if finish and not blend_finishes_view(means3d.size(0), capacity):
+        raise ValueError("render_fused(finish=True) needs the sync-free bucket path with ranked records")
+    if _bucket_path(means3d.size(0), capacity):
+        return _RenderBuckets.apply(means3d, scales, quats, opacity, colors, viewmat, background, glob_scale, fx, fy,
+                                    cx, cy, img_height, img_width, clip_thresh, capacity, colors_event, finish)
+    if colors_event is not None:  # _RenderFused: the colours must be complete before its first kernel
         torch.cuda.current_stream(means3d.device).wait_event(colors_event)
     return _RenderFused.apply(means3d, scales, quats, opacity, colors, viewmat, background, glob_scale, fx, fy, cx, cy,
                               img_height, img_width, clip_thresh, capacity)

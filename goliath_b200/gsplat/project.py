@@ -42,9 +42,10 @@ def project_gaussians(
 
 
 def _project_fwd(means3d, scales, quats, viewmat, glob_scale, fx, fy, cx, cy, img_height, img_width, block_width,
-                 clip_thresh):
+                 clip_thresh, grad_acc=None):
     """The projection kernel on the current stream.  Returns (xys [G,2], depths [G], radii [G] i32, conics [G,3],
-    compensation [G], num_tiles_hit [G] i32, cov3d [G,6])."""
+    compensation [G], num_tiles_hit [G] i32, cov3d [G,6]).  `grad_acc` [10 G], if given, is zeroed by the same kernel
+    for the fused render's blend backward (gb_project_gaussians_fwd_acc)."""
     G = means3d.size(0)
     dev = means3d.device
     f32 = dict(device=dev, dtype=torch.float32)
@@ -52,12 +53,17 @@ def _project_fwd(means3d, scales, quats, viewmat, glob_scale, fx, fy, cx, cy, im
     cov3d, xys, depths = torch.empty(G, 6, **f32), torch.empty(G, 2, **f32), torch.empty(G, **f32)
     radii, conics, comp = torch.empty(G, **i32), torch.empty(G, 3, **f32), torch.empty(G, **f32)
     num_tiles_hit = torch.empty(G, **i32)
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().gb_project_gaussians_fwd(
-            G, _lib.ptr(means3d), _lib.ptr(scales), float(glob_scale), _lib.ptr(quats), _lib.ptr(viewmat), float(fx),
+    L = _lib.lib()
+    args = (G, _lib.ptr(means3d), _lib.ptr(scales), float(glob_scale), _lib.ptr(quats), _lib.ptr(viewmat), float(fx),
             float(fy), float(cx), float(cy), int(img_height), int(img_width), int(block_width), float(clip_thresh),
             _lib.ptr(cov3d), _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp),
-            _lib.ptr(num_tiles_hit), _lib.stream_ptr(dev)), "project_gaussians_forward")
+            _lib.ptr(num_tiles_hit))
+    with torch.cuda.device(dev):
+        if grad_acc is None:
+            _lib.check(L.gb_project_gaussians_fwd(*args, _lib.stream_ptr(dev)), "project_gaussians_forward")
+        else:
+            _lib.check(L.gb_project_gaussians_fwd_acc(*args, _lib.ptr(grad_acc), _lib.stream_ptr(dev)),
+                       "project_gaussians_forward")
     return xys, depths, radii, conics, comp, num_tiles_hit, cov3d
 
 

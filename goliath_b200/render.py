@@ -146,7 +146,9 @@ def _black(dev):
 
 
 class _FinishView(th.autograd.Function):
-    """out4 [H,W,4] + alpha [H,W] -> (rgb [3,H,W], alpha [1,H,W], depth [1,H,W]) in one kernel (csrc/render_finish.cu)."""
+    """out4 [H,W,4] + alpha [H,W] -> (rgb [3,H,W], alpha [1,H,W], depth [1,H,W]) in one kernel (csrc/render_finish.cu),
+    for the renders that produce out4: the sync-free bucket path with packed records and gsplat.fused._RenderFused.
+    With ranked records the blend kernels finish the view themselves (gsplat.fused.blend_finishes_view)."""
 
     @staticmethod
     def forward(ctx, out4, alpha):
@@ -218,18 +220,20 @@ def render_views(width: int, height: int, K: th.Tensor, Rt: th.Tensor, preds, in
     B = Rt.shape[0]
     intrinsics_host = _intrinsics(K, intrinsics_host, B)
     if fused:
-        # per view: one autograd node for project + bin/sort + pack + blend and one for the post-processing
-        from .gsplat.fused import render_fused
+        # per view: one autograd node for project + bin/sort + blend, which also finishes the view where its blend
+        # kernels can (ranked records), else one more for the post-processing
+        from .gsplat.fused import blend_finishes_view, render_fused
         pv = {k: _per_view(preds[k], B, last)
               for k, last in (("primpos", 3), ("primscale", 3), ("primqvec", 4), ("opacity", 1), ("color", 3))}
+        finish = blend_finishes_view(pv["primpos"][0].size(0), capacity)
 
         def render_view(b):
             fx, fy, cx, cy = intrinsics_host[b]
-            out4, alpha, _ = render_fused(
+            outs = render_fused(
                 pv["primpos"][b].contiguous(), pv["primscale"][b].contiguous(), 1.0, pv["primqvec"][b].contiguous(),
                 Rt[b], fx, fy, cx, cy, height, width, pv["opacity"][b].contiguous(), pv["color"][b].contiguous(),
-                _black(Rt.device), 0.1, capacity, colors_event=color_event)
-            return _FinishView.apply(out4, alpha)
+                _black(Rt.device), 0.1, capacity, colors_event=color_event, finish=finish)
+            return outs[:3] if finish else _FinishView.apply(outs[0], outs[1])
 
         rgbs, alphas, depths = zip(*_issue_views(Rt.device, B, capacity, render_view))
         if B == 1:

@@ -59,6 +59,23 @@ int gb_project_gaussians_fwd(int G, const float* means3d, const float* scales, f
                              float* depths, int32_t* radii, float* conics, float* compensation,
                              int32_t* num_tiles_hit, void* stream);
 
+/* gb_project_gaussians_fwd that also zeroes grad_acc [10 G] fp32, the fused render's blend-backward accumulator:
+ * v_rgbd [G,4] | v_xy [G,2] | v_conic [G,3] | v_opacity_eff [G]. */
+int gb_project_gaussians_fwd_acc(int G, const float* means3d, const float* scales, float glob_scale,
+                                 const float* quats, const float* viewmat, float fx, float fy, float cx, float cy,
+                                 int img_h, int img_w, int block_width, float clip_thresh, float* cov3d, float* xys,
+                                 float* depths, int32_t* radii, float* conics, float* compensation,
+                                 int32_t* num_tiles_hit, float* grad_acc, void* stream);
+
+/* The fused render's per-Gaussian backward in one pass: grad_acc (gb_project_gaussians_fwd_acc's layout, filled by the
+ * blend backward), opacity [G] and the projection's saved tensors -> v_colors [G,3], v_opacity [G], v_mean3d,
+ * v_scale, v_quat; the same bits as gb_splat_grad_unpack followed by gb_project_gaussians_bwd. */
+int gb_splat_project_bwd(int G, const float* means3d, const float* scales, float glob_scale, const float* quats,
+                         const float* viewmat, float fx, float fy, const float* cov3d, const int32_t* radii,
+                         const float* conics, const float* compensation, const float* opacity, const float* grad_acc,
+                         float* v_colors, float* v_opacity, float* v_mean3d, float* v_scale, float* v_quat,
+                         void* stream);
+
 /* replaces gsplat._C.project_gaussians_backward.  All five gradient outputs are overwritten. */
 int gb_project_gaussians_bwd(int G, const float* means3d, const float* scales, float glob_scale,
                              const float* quats, const float* viewmat, float fx, float fy, const float* cov3d,
@@ -250,6 +267,21 @@ int gb_rasterize_ranked_fwd_sort_lists(int img_h, int img_w, int channels, const
                                        int32_t* ranks_keys, const float* rec_by_rank, const float* background,
                                        float* out_img, float* final_Ts, int32_t* final_idx, int32_t* hit_list,
                                        int32_t* hit_count, void* stream);
+/* The head view finished inside the blend kernels.  gb_rasterize_ranked_fwd_sort_finish is
+ * gb_rasterize_ranked_fwd_sort_lists (4 channels) writing rgb [3,H,W], alpha [H,W] = 1 - final_Ts and depth [H,W] =
+ * depth channel / clamp(alpha, 0.05, 1) instead of the 4-channel image: gb_render_finish_fwd's results, bit for bit.
+ * gb_rasterize_ranked_bwd_lists_finish is gb_render_finish_bwd + gb_rasterize_ranked_bwd_lists on g_rgb [3,H,W] and
+ * g_depth [H,W] (either may be NULL); alpha takes no gradient.  background holds 3 floats in both. */
+int gb_rasterize_ranked_fwd_sort_finish(int img_h, int img_w, const int32_t* tile_bins, const int32_t* tile_order,
+                                        const float* depths, int32_t* bucket, int32_t* ranks_keys,
+                                        const float* rec_by_rank, const float* background, float* rgb, float* alpha,
+                                        float* depth, float* final_Ts, int32_t* final_idx, int32_t* hit_list,
+                                        int32_t* hit_count, void* stream);
+int gb_rasterize_ranked_bwd_lists_finish(int img_h, int img_w, const int32_t* ranks_sorted, const int32_t* tile_bins,
+                                         const int32_t* hit_list, int32_t* hit_count, const float* rec_by_rank,
+                                         const float* background, const float* final_Ts, const int32_t* final_idx,
+                                         const float* alpha, const float* g_rgb, const float* g_depth, float* v_xy,
+                                         float* v_conic, float* v_colors, float* v_opacity, void* stream);
 
 /* launch order of the tiles, longest list first: order [T] int32 */
 int gb_tile_order(int num_tiles, const int32_t* tile_bins, int32_t* order, void* stream);

@@ -1,4 +1,4 @@
-"""Per-kernel device time of one bench head step (bench.py --config head) for both record modes of the two-node render.
+"""Per-kernel device time of one bench head step (bench.py --config head) for both record modes of the bucket-path render.
 
 Builds the bench scene (bench.packed_scene, HeadWorkload, capacity 8 G), captures one step in a CUDA graph as
 bench.run_ours does, and replays it under torch.profiler (CUDA activities) with the L2 flushed before each replay.
