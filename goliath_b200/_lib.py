@@ -157,6 +157,11 @@ SIGNATURES = {
     "gb_pose_shadow_fwd": (_i, [_i] * 5 + [_vp, _f, _vp, _vp]),
     "gb_pose_shadow_bwd": (_i, [_i] * 5 + [_vp, _f, _vp, _vp, _vp]),
     "gb_head_lights_fwd": (_i, [_i] * 3 + [_vp] * 11 + [_vp]),
+    "gb_hand_valid_gather_fwd": (_i, [_i] * 4 + [_vp] * 5 + [_f] + [_vp] * 4 + [_vp]),
+    "gb_hand_valid_gather_bwd": (_i, [_i] * 4 + [_vp] * 5 + [_f] + [_vp] * 4 + [_vp]),
+    "gb_hand_finish_workspace_bytes": (_sz, [_i] * 3),
+    "gb_hand_finish_fwd": (_i, [_i] * 3 + [_vp] * 7 + [_vp]),
+    "gb_hand_finish_bwd": (_i, [_i] * 3 + [_vp] * 10 + [_vp]),
 }
 
 

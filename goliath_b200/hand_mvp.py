@@ -9,7 +9,10 @@ checkpoints load, plus the two glue stages between those decoders and the raymar
 
 The mesh front end (DESIGN.md row R8') runs on kernels too: `GeomDecoder` poses the mesh with `lbs.LBSModule` and
 builds each primitive's base frame with `prim_base_frames`; `view_cos_uv` gives the RGB decoder's view conditioning
-(hand_mvp.py:230-236), both on csrc/mvp_prims.cu."""
+(hand_mvp.py:230-236), both on csrc/mvp_prims.cu.
+
+`AutoEncoder` (hand_mvp.py:71-266) runs the whole frame on these stages and the MVP raymarcher, with the valid-primitive
+gather before the march and the render finish after it on csrc/hand_frame.cu."""
 from typing import Optional, Tuple
 
 import torch
@@ -330,3 +333,286 @@ class RGBSlabDecoder(nn.Module):
         rgb = self.texdecoder(torch.cat((joint, view_cos_uv, ao_ds), 1))
         rgb = rgb.view(B, self.primsize_z, 3, self.uv_size, self.uv_size)
         return F.relu(25.0 * rgb + 100.0)
+
+
+# ------------------------------------------------------------------------------------------------ the frame
+class _ValidGather(Function):
+    """Raymarcher.forward's primpos / volradius and valid-primitive selection (render_raymarcher.py:36-47) in one
+    launch of csrc/hand_frame.cu; the backward writes the full-size gradients once (zero at invalid primitives)."""
+
+    @staticmethod
+    def forward(ctx, template, primpos, primrot, primscale, slot, n_valid, volradius):
+        template, primpos = template.contiguous(), primpos.contiguous()
+        primrot, primscale = primrot.contiguous(), primscale.contiguous()
+        for t, n in ((template, "primrgba"), (primpos, "primpos"), (primrot, "primrot"), (primscale, "primscale")):
+            _lib.check_input(t, n)
+        _lib.check_input(slot, "slot table", torch.int32)
+        B, K = template.shape[:2]
+        E = template[0, 0].numel()
+        if (primpos.shape != (B, K, 3) or primrot.shape != (B, K, 3, 3) or primscale.shape != (B, K, 3)
+                or slot.shape != (K,)):
+            raise RuntimeError("valid gather: template [B,K,...], primpos / primscale [B,K,3], primrot [B,K,3,3] and "
+                               "a slot table [K] (got K = %d, slot %s)" % (K, tuple(slot.shape)))
+        # torch evaluates `primpos / volradius` as primpos * (1 / volradius) in fp32 (div by a CPU scalar)
+        inv = float(torch.tensor(1.0, dtype=torch.float32) / torch.tensor(float(volradius), dtype=torch.float32))
+        dev = template.device
+        tpl = torch.empty((B, n_valid) + tuple(template.shape[2:]), device=dev)
+        pos, scale = torch.empty(B, n_valid, 3, device=dev), torch.empty(B, n_valid, 3, device=dev)
+        rot = torch.empty(B, n_valid, 3, 3, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().gb_hand_valid_gather_fwd(
+                B, K, n_valid, E, _lib.ptr(slot), _lib.ptr(template), _lib.ptr(primpos), _lib.ptr(primrot),
+                _lib.ptr(primscale), inv, _lib.ptr(tpl), _lib.ptr(pos), _lib.ptr(rot), _lib.ptr(scale),
+                _lib.stream_ptr(dev)), "hand_valid_gather_fwd")
+        ctx.save_for_backward(slot)
+        ctx.meta = (tuple(template.shape), n_valid, inv)
+        return tpl, pos, rot, scale
+
+    @staticmethod
+    def backward(ctx, g_tpl, g_pos, g_rot, g_scale):
+        (slot,) = ctx.saved_tensors
+        shape, n_valid, inv = ctx.meta
+        B, K = shape[:2]
+        g_tpl, g_pos, g_rot, g_scale = (g.contiguous() for g in (g_tpl, g_pos, g_rot, g_scale))
+        dev = g_tpl.device
+        gt = torch.empty(shape, device=dev)
+        gp, gr, gs = torch.empty(B, K, 3, device=dev), torch.empty(B, K, 3, 3, device=dev), torch.empty(B, K, 3,
+                                                                                                      device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().gb_hand_valid_gather_bwd(
+                B, K, n_valid, gt[0, 0].numel(), _lib.ptr(slot), _lib.ptr(g_tpl), _lib.ptr(g_pos), _lib.ptr(g_rot),
+                _lib.ptr(g_scale), inv, _lib.ptr(gt), _lib.ptr(gp), _lib.ptr(gr), _lib.ptr(gs),
+                _lib.stream_ptr(dev)), "hand_valid_gather_bwd")
+        return gt, gp, gr, gs, None, None, None
+
+
+def valid_gather(template, primpos, primrot, primscale, slot, n_valid, volradius):
+    """(template [B,K,TD,TH,TW,4], primpos, primrot, primscale) -> the same tensors at the n_valid primitives with
+    slot[k] >= 0, in slot order, and primpos divided by volradius: the march inputs render_raymarcher.py:36-47 builds.
+    `slot` [K] int32 (rank among the valid primitives, -1 for the others) and n_valid come from the host, so the
+    call issues no host synchronisation."""
+    return _ValidGather.apply(template, primpos, primrot, primscale, slot, int(n_valid), float(volradius))
+
+
+def slot_table(valid_prims):
+    """bool [K] -> (slot [K] int32: rank among the valid entries, -1 elsewhere; the number of valid entries), on
+    valid_prims' device"""
+    v = valid_prims.reshape(-1).to(torch.bool)
+    ranks = torch.cumsum(v.to(torch.int32), 0, dtype=torch.int32) - 1
+    return torch.where(v, ranks, torch.full_like(ranks, -1)), int(v.sum())
+
+
+class _HandFinish(Function):
+    """rayrgba [B,H,W,4] -> calibrated rgb (+ training background) [B,3,H,W], alpha [B,1,H,W] on csrc/hand_frame.cu"""
+
+    @staticmethod
+    def forward(ctx, rayrgba, cal_w, cal_b, grey, bg):
+        rayrgba = rayrgba.contiguous()
+        _lib.check_input(rayrgba, "rayrgba")
+        B, H, W, four = rayrgba.shape
+        if four != 4:
+            raise RuntimeError("hand_finish: rayrgba must be [B,H,W,4]")
+        opt = {}
+        for name, t, shape, dt in (("cal_w", cal_w, (B, 3), torch.float32), ("cal_b", cal_b, (B, 3), torch.float32),
+                                   ("grey", grey, (B,), torch.int32), ("background", bg, (B, 3, H, W), torch.float32)):
+            if t is not None:
+                t = t.contiguous()
+                _lib.check_input(t, name, dt)
+                if tuple(t.shape) != shape:
+                    raise RuntimeError("hand_finish: %s must have shape %s (got %s)" % (name, shape, tuple(t.shape)))
+            opt[name] = t
+        if (opt["cal_w"] is None) != (opt["cal_b"] is None):
+            raise RuntimeError("hand_finish: cal_w and cal_b go together")
+        dev = rayrgba.device
+        rgb, alpha = torch.empty(B, 3, H, W, device=dev), torch.empty(B, 1, H, W, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().gb_hand_finish_fwd(
+                B, H, W, _lib.ptr(rayrgba), _lib.ptr(opt["cal_w"]), _lib.ptr(opt["cal_b"]), _lib.ptr(opt["grey"]),
+                _lib.ptr(opt["background"]), _lib.ptr(rgb), _lib.ptr(alpha), _lib.stream_ptr(dev)), "hand_finish_fwd")
+        ctx.save_for_backward(rayrgba, opt["cal_w"], opt["grey"], opt["background"])
+        ctx.set_materialize_grads(False)
+        return rgb, alpha
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_alpha):
+        rayrgba, cal_w, grey, bg = ctx.saved_tensors
+        B, H, W, _ = rayrgba.shape
+        dev = rayrgba.device
+        if g_rgb is None:
+            g_rgb = torch.zeros(B, 3, H, W, device=dev)
+        g_rgb = g_rgb.contiguous()
+        g_alpha = None if g_alpha is None else g_alpha.contiguous()
+        g_ray = torch.empty_like(rayrgba)
+        g_cw = g_cb = ws = None
+        L = _lib.lib()
+        if cal_w is not None:
+            g_cw, g_cb = torch.empty(B, 3, device=dev), torch.empty(B, 3, device=dev)
+            ws = torch.empty(L.gb_hand_finish_workspace_bytes(B, H, W) // 4, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(L.gb_hand_finish_bwd(
+                B, H, W, _lib.ptr(rayrgba), _lib.ptr(cal_w), _lib.ptr(grey), _lib.ptr(bg), _lib.ptr(g_rgb),
+                _lib.ptr(g_alpha), _lib.ptr(g_ray), _lib.ptr(g_cw), _lib.ptr(g_cb), _lib.ptr(ws),
+                _lib.stream_ptr(dev)), "hand_finish_bwd")
+        return g_ray, g_cw, g_cb, None, None
+
+
+def hand_finish(rayrgba, cal_w=None, cal_b=None, grey=None, background=None):
+    """The raymarcher's channels-last rayrgba [B,H,W,4] -> (rgb [B,3,H,W], alpha [B,1,H,W]) with, in the reference's
+    order (hand_mvp.py:249-255), the calibration rows of `CalV5.rows` (cal_w / cal_b [B,3], grey [B] int32) and the
+    training background [B,3,H,W]: rgb = cal(rayrgb) + (1 - alpha) * background.  Any stage whose tensors are None is
+    skipped.  Gradients: rayrgba (its alpha channel also through the background term), cal_w, cal_b."""
+    return _HandFinish.apply(rayrgba, cal_w, cal_b, grey, background)
+
+
+class Raymarcher(nn.Module):
+    """render_raymarcher.py:17-24: the volume radius and the step size dt / volume_radius (no parameters)"""
+
+    def __init__(self, volradius, dt: float = 1.0):
+        super().__init__()
+        self.volume_radius = volradius
+        self.dt = dt / self.volume_radius
+
+
+class _ImageSize(nn.Module):
+    """the state of pytorch3d's RenderLayer (render_pytorch3d.py:30-31): its persistent `image_size` [2] int32.  The
+    frame never rasterises the mesh, so this holds the checkpoint key only."""
+
+    def __init__(self, h, w):
+        super().__init__()
+        self.register_buffer("image_size", torch.as_tensor([h, w], dtype=torch.int32))
+
+
+class _InpaintedIndexImages:
+    """what `init_primitives` reads of a geometry module: vi, vti, vt and render_index_images(size, impaint=True),
+    whose face and barycentric images come from the assets"""
+
+    def __init__(self, geo_fn, face_index, bary):
+        self.vi, self.vti, self.vt = geo_fn.vi.to(torch.int64), geo_fn.vti.to(torch.int64), geo_fn.vt
+        self.face_index, self.bary = face_index, bary
+
+    def render_index_images(self, uv_size, flip_uv=False, impaint=False):
+        if uv_size != self.face_index.shape[0]:
+            raise ValueError("the assets' inpainted index images are %d x %d, not %d"
+                             % (self.face_index.shape[0], self.face_index.shape[1], uv_size))
+        return None, self.face_index, self.bary
+
+
+HAND_UV_IMAGES = ("face_index_image_impaint", "bary_image_impaint")
+
+
+class AutoEncoder(nn.Module):
+    """hand_mvp.AutoEncoder (ca_code/models/hand_mvp.py:71-266): the hand avatar's frame with the reference's
+    constructor, submodules and state-dict keys (`geomdecoder.{lbs_fn,geo_fn}.*` and `rgbdecoder.geo_fn.*` repeat the
+    shared modules), so `AutoEncoder(**config.model, assets=assets)` builds from hand_mvp_example.yml and a reference
+    checkpoint loads with strict=True.
+
+    `assets` (attributes or dict keys) carries the reference's assets and, because this project does not rasterise UV
+    layouts, the four `geo_fn` images (`mesh_vae._uv_geometry`) plus what `render_index_images(1024, impaint=True)`
+    returns for `init_primitives`: face_index_image_impaint [1024,1024] and bary_image_impaint [1024,1024,3].
+    `renderer` holds only the mesh renderer's `image_size` key: the frame never rasterises the mesh.
+
+    `valid_prims`, its slot table and its count are built once on the host at construction, so forward() (CUDA only)
+    and its backward issue no host synchronisation after the first call.  preds["primrgba"] is the full
+    [B, n_prims, 8, 16, 16, 4] template, as in the reference; the raymarcher receives its valid primitives only."""
+
+    def __init__(self, assets, image_height, image_width, cal=None, n_pose_dims: int = 54, n_embs: int = 64,
+                 volradius: float = 2000.0, primsize: Tuple[int, int, int] = (16, 16, 8), learn_blur: bool = True):
+        super().__init__()
+        import numpy as np
+
+        from .lbs import LBSModule
+        from .mesh_vae import UV_IMAGES, _get, _uv_geometry
+        from .photo_loss import CalV5, LearnableBlur
+
+        missing = [k for k in UV_IMAGES + HAND_UV_IMAGES if _get(assets, k) is None]
+        if missing:
+            raise ValueError("hand_mvp.AutoEncoder: assets must carry the UV images %s at 1024 x 1024; missing: %s"
+                             % (", ".join(UV_IMAGES + HAND_UV_IMAGES), ", ".join(missing)))
+        self.uv_size = 1024
+        self.primsize = tuple(primsize)
+        self.n_prim_x = self.uv_size // self.primsize[0]
+        self.n_prim_y = self.uv_size // self.primsize[1]
+        self.n_prims = self.n_prim_x * self.n_prim_y
+        self.height, self.width = image_height, image_width
+        self.volradius = volradius
+        template = torch.as_tensor(np.asarray(_get(assets, "template_mesh_unscaled")), dtype=torch.float32)
+        self.lbs_fn = LBSModule(_get(assets, "lbs_model_json"), _get(assets, "lbs_config_dict"), template[None],
+                                _get(assets, "skeleton_scales"), global_scaling=[10.0, 10.0, 10.0])
+        self.geo_fn, _ = _uv_geometry(assets)
+        imgs = {k: torch.as_tensor(np.asarray(_get(assets, k))) for k in HAND_UV_IMAGES}
+        if tuple(imgs["face_index_image_impaint"].shape) != (1024, 1024) or \
+                tuple(imgs["bary_image_impaint"].shape) != (1024, 1024, 3):
+            raise ValueError("hand_mvp.AutoEncoder: face_index_image_impaint must be [1024,1024] and "
+                             "bary_image_impaint [1024,1024,3]")
+
+        self.poseencoder = PoseEncoder(n_pose_dims, n_embs, self.n_prim_x)
+        index_images = _InpaintedIndexImages(self.geo_fn, imgs["face_index_image_impaint"].to(torch.int64),
+                                             imgs["bary_image_impaint"].to(torch.float32))
+        self.geomdecoder = GeomDecoder(n_embs, self.primsize[2], self.uv_size, self.n_prims, self.lbs_fn,
+                                       index_images, primposstart=1000)
+        self.geomdecoder.geo_fn = self.geo_fn
+        self.rgbdecoder = RGBSlabDecoder(n_embs + 2, self.primsize[2], self.uv_size, self.geo_fn)
+        self.raymarcher = Raymarcher(volradius=self.volradius, dt=1.0)
+        self.renderer = _ImageSize(image_height, image_width)
+        cameras = _get(assets, "camera_ids")
+        self.learn_blur_enabled = bool(learn_blur)
+        if self.learn_blur_enabled:
+            self.learn_blur = LearnableBlur(cameras)
+        self.cal_enabled = cal is not None
+        if self.cal_enabled:
+            self.cal = CalV5(**cal, cameras=cameras)
+
+        # hand_mvp.py:153-160, once on the host, with the gather's slot table and count
+        valid_mask = F.interpolate(self.geo_fn.valid_mask.float()[None].permute(0, 3, 1, 2),
+                                   (self.n_prim_x, self.n_prim_y), mode="area")
+        valid_prims = (valid_mask != 0).reshape(-1)
+        self.register_buffer("valid_prims", valid_prims, persistent=False)
+        slot, self.n_valid = slot_table(valid_prims)
+        self.register_buffer("valid_slot", slot, persistent=False)
+
+    def forward(self, pose, campos, ambient_occlusion=None, K=None, Rt=None, camera_id=None, frame_id=None,
+                embs=None, encode=True, iteration=None, background=None, **kwargs):
+        from .mvpraymarch import mvpraymarch
+        from .utils import compute_raydirs
+
+        for t, n in ((pose, "pose"), (campos, "campos"), (K, "K"), (Rt, "Rt")):
+            if t is None or not t.is_cuda:
+                raise RuntimeError("hand_mvp.AutoEncoder runs on CUDA only (no CPU fallback): %s is %s"
+                                   % (n, "missing" if t is None else "on %s" % t.device))
+        B = pose.shape[0]
+        joint = self.poseencoder(pose)
+        geo_preds = self.geomdecoder(pose, joint, iteration)
+        gd = self.geomdecoder
+        with torch.no_grad():
+            vc = view_cos_uv(geo_preds["geom_lbs"], self.geo_fn.vi, campos, gd.prim_vidx_img, gd.prim_bary_img)
+        # RGBSlabDecoder.forward (hand_mvp.py:457-474) with the deconv tower's raw output kept: the template takes it
+        # with the activation applied in the slab kernel, so the template's gradient skips the torch activation
+        ao_ds = F.interpolate(ambient_occlusion, (64, 64), mode="bilinear")
+        rd = self.rgbdecoder
+        raw = rd.texdecoder(torch.cat((joint, vc, ao_ds), 1)).view(B, rd.primsize_z, 3, rd.uv_size, rd.uv_size)
+        primrgb = F.relu(25.0 * raw + 100.0)
+        primrgba = slabs_to_primrgba(raw, geo_preds["primalpha"], self.primsize, raw=True)
+        preds = {"primrgb": primrgb, "valid_prims": self.valid_prims, **geo_preds, "primrgba": primrgba}
+
+        # AutoEncoder.render (hand_mvp.py:187-203) and Raymarcher.forward (render_raymarcher.py:36-70)
+        focal = torch.diagonal(K[:, :2, :2], dim1=1, dim2=2).contiguous()
+        princpt = K[:, :2, 2].contiguous()
+        camrot = Rt[:, :3, :3].contiguous()
+        ray_campos = -(camrot.transpose(-2, -1) @ Rt[:, :3, 3:4])[..., 0]
+        raypos, raydir, tminmax = compute_raydirs(ray_campos.contiguous(), camrot, focal, princpt,
+                                                  (self.width, self.height), self.raymarcher.volume_radius)
+        tpl, pos, rot, scale = valid_gather(primrgba, geo_preds["primpos"], geo_preds["primrot"],
+                                            geo_preds["primscale"], self.valid_slot, self.n_valid,
+                                            self.raymarcher.volume_radius)
+        rayrgba = mvpraymarch(raypos, raydir, self.raymarcher.dt, tminmax, (pos, rot, scale), template=tpl, warp=None)
+
+        cal_w = cal_b = grey = None
+        if self.cal_enabled:
+            cal_w, cal_b, grey = self.cal.rows(self.cal.name_to_idx(camera_id))
+        bg = background[:, :3] if self.training and background is not None else None
+        rgb, alpha = hand_finish(rayrgba, cal_w, cal_b, grey, bg)
+        preds.update(rgb=rgb, alpha=alpha)
+        if self.learn_blur_enabled:
+            preds["rgb"] = self.learn_blur(preds["rgb"], camera_id)
+            preds["learn_blur_weights"] = self.learn_blur.reg(camera_id)
+        return preds

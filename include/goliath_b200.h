@@ -909,6 +909,43 @@ int gb_head_lights_fwd(int B, int L, int C, const float* head_pose, const float*
                        float* headrel_campos, float* headrel_light_pos, float* headrel_light_sh, float* lightrot_out,
                        void* stream);
 
+/* ---------------------------------------------------------------- hand frame (row R8'', csrc/hand_frame.cu) */
+
+/* replaces the valid-primitive selection of Raymarcher.forward (ca_code/utils/render_raymarcher.py:36-47):
+ *   primpos / volume_radius, then template / primpos / primrot / primscale [:, valid_prims].contiguous()
+ * with slot [K] int32 = rank of primitive k among the valid ones, -1 when it is not valid (built once on the host,
+ * n_valid = the number of valid primitives).  tpl [B,K,E] (E = tpl_elems floats per primitive, a multiple of 4),
+ * pos / scale [B,K,3], rot [B,K,3,3] -> tpl_out [B,n_valid,E], pos_out = pos * inv_radius, rot_out, scale_out
+ * [B,n_valid,...], each element written once.  One launch, no device-side count. */
+int gb_hand_valid_gather_fwd(int B, int K, int n_valid, int tpl_elems, const int32_t* slot, const float* tpl,
+                             const float* pos, const float* rot, const float* scale, float inv_radius, float* tpl_out,
+                             float* pos_out, float* rot_out, float* scale_out, void* stream);
+/* the transpose of the above (replaces the autograd scatter of the same lines): every element of g_tpl_full [B,K,E],
+ * g_pos_full (= g_pos * inv_radius), g_rot_full and g_scale_full is WRITTEN once, zero at invalid primitives.  No
+ * atomics and no memset: the same bits on every call. */
+int gb_hand_valid_gather_bwd(int B, int K, int n_valid, int tpl_elems, const int32_t* slot, const float* g_tpl,
+                             const float* g_pos, const float* g_rot, const float* g_scale, float inv_radius,
+                             float* g_tpl_full, float* g_pos_full, float* g_rot_full, float* g_scale_full,
+                             void* stream);
+/* bytes of the workspace gb_hand_finish_bwd needs for the calibration gradients (per-CTA partials) */
+size_t gb_hand_finish_workspace_bytes(int B, int H, int W);
+/* replaces the channel split of Raymarcher.forward (render_raymarcher.py:69-70), CalV5.forward
+ * (ca_code/nn/color_cal.py:211-241) and the training background of hand_mvp.AutoEncoder.forward
+ * (ca_code/models/hand_mvp.py:249-255), in that order, in one pass:
+ *   v = rayrgba[..., :3];  v = cal_w * v + cal_b  (grey[b]: every channel = sum_c v_c cal_w_c + sum_c cal_b_c)
+ *   rgb = v + (1 - alpha) * bg,  alpha = rayrgba[..., 3]
+ * rayrgba [B,H,W,4], cal_w / cal_b [B,3] (both NULL: no calibration), grey [B] int32 or NULL, bg [B,3,H,W] or NULL;
+ * rgb [B,3,H,W] and alpha [B,1,H,W] are written once. */
+int gb_hand_finish_fwd(int B, int H, int W, const float* rayrgba, const float* cal_w, const float* cal_b,
+                       const int32_t* grey, const float* bg, float* rgb, float* alpha, void* stream);
+/* the backward of the above: g_rayrgba [B,H,W,4] is WRITTEN, its alpha channel g_alpha - sum_c g_rgb_c bg_c (alpha is
+ * not detached in the reference); g_alpha may be NULL (zero).  With calibration, g_cal_w / g_cal_b [B,3] are WRITTEN
+ * from per-CTA partials in `workspace` (gb_hand_finish_workspace_bytes) reduced per view in a fixed order by a second
+ * launch: the same bits on every call. */
+int gb_hand_finish_bwd(int B, int H, int W, const float* rayrgba, const float* cal_w, const int32_t* grey,
+                       const float* bg, const float* g_rgb, const float* g_alpha, float* g_rayrgba, float* g_cal_w,
+                       float* g_cal_b, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
