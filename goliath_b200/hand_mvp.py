@@ -572,9 +572,6 @@ class AutoEncoder(nn.Module):
 
     def forward(self, pose, campos, ambient_occlusion=None, K=None, Rt=None, camera_id=None, frame_id=None,
                 embs=None, encode=True, iteration=None, background=None, **kwargs):
-        from .mvpraymarch import mvpraymarch
-        from .utils import compute_raydirs
-
         for t, n in ((pose, "pose"), (campos, "campos"), (K, "K"), (Rt, "Rt")):
             if t is None or not t.is_cuda:
                 raise RuntimeError("hand_mvp.AutoEncoder runs on CUDA only (no CPU fallback): %s is %s"
@@ -593,26 +590,52 @@ class AutoEncoder(nn.Module):
         primrgb = F.relu(25.0 * raw + 100.0)
         primrgba = slabs_to_primrgba(raw, geo_preds["primalpha"], self.primsize, raw=True)
         preds = {"primrgb": primrgb, "valid_prims": self.valid_prims, **geo_preds, "primrgba": primrgba}
+        rgb, alpha = self._finish(self._march(K, Rt, preds), camera_id, background)
+        preds.update(rgb=rgb, alpha=alpha)
+        self._blur(preds, camera_id)
+        return preds
 
-        # AutoEncoder.render (hand_mvp.py:187-203) and Raymarcher.forward (render_raymarcher.py:36-70)
+    def _march(self, K, Rt, preds):
+        """AutoEncoder.render (hand_mvp.py:187-203) and Raymarcher.forward (render_raymarcher.py:36-70): the camera
+        of K / Rt, its rays, the valid primitives of preds["primrgba"] and the primitive transforms, and the march ->
+        channels-last rayrgba [B,H,W,4]"""
+        from .mvpraymarch import mvpraymarch  # looked up per call, so a test can wrap the march
+        from .utils import compute_raydirs
+
+        for t, n in ((K, "K"), (Rt, "Rt"), (preds["primrgba"], "primrgba")):
+            if t is None or not t.is_cuda:
+                raise RuntimeError("hand_mvp.AutoEncoder runs on CUDA only (no CPU fallback): %s is %s"
+                                   % (n, "missing" if t is None else "on %s" % t.device))
         focal = torch.diagonal(K[:, :2, :2], dim1=1, dim2=2).contiguous()
         princpt = K[:, :2, 2].contiguous()
         camrot = Rt[:, :3, :3].contiguous()
         ray_campos = -(camrot.transpose(-2, -1) @ Rt[:, :3, 3:4])[..., 0]
         raypos, raydir, tminmax = compute_raydirs(ray_campos.contiguous(), camrot, focal, princpt,
                                                   (self.width, self.height), self.raymarcher.volume_radius)
-        tpl, pos, rot, scale = valid_gather(primrgba, geo_preds["primpos"], geo_preds["primrot"],
-                                            geo_preds["primscale"], self.valid_slot, self.n_valid,
-                                            self.raymarcher.volume_radius)
-        rayrgba = mvpraymarch(raypos, raydir, self.raymarcher.dt, tminmax, (pos, rot, scale), template=tpl, warp=None)
+        tpl, pos, rot, scale = valid_gather(preds["primrgba"], preds["primpos"], preds["primrot"], preds["primscale"],
+                                            self.valid_slot, self.n_valid, self.raymarcher.volume_radius)
+        return mvpraymarch(raypos, raydir, self.raymarcher.dt, tminmax, (pos, rot, scale), template=tpl, warp=None)
 
+    def _finish(self, rayrgba, camera_id, background):
+        """the march's rgb / alpha [B,·,H,W], calibrated and, in training, over the background (hand_mvp.py:249-255)"""
         cal_w = cal_b = grey = None
         if self.cal_enabled:
             cal_w, cal_b, grey = self.cal.rows(self.cal.name_to_idx(camera_id))
         bg = background[:, :3] if self.training and background is not None else None
-        rgb, alpha = hand_finish(rayrgba, cal_w, cal_b, grey, bg)
-        preds.update(rgb=rgb, alpha=alpha)
+        return hand_finish(rayrgba, cal_w, cal_b, grey, bg)
+
+    def _blur(self, preds, camera_id):
         if self.learn_blur_enabled:
             preds["rgb"] = self.learn_blur(preds["rgb"], camera_id)
             preds["learn_blur_weights"] = self.learn_blur.reg(camera_id)
-        return preds
+
+    def render(self, K, Rt, preds, with_shadow: bool = False):
+        """hand_mvp.py:162-205: the template of preds["primrgb"] (activated) and preds["primalpha"], stored as
+        preds["primrgba"] [B, n_prims, 8, 16, 16, 4], marched from the cameras K / Rt -> (rgb [B,3,H,W],
+        alpha [B,1,H,W], None), uncalibrated.  HandMVPSummary draws the teacher's shadow image with it.  No frame
+        marches with `with_shadow=True`, so it raises."""
+        if with_shadow:
+            raise NotImplementedError("hand_mvp.AutoEncoder.render: with_shadow=True is not supported")
+        preds["primrgba"] = slabs_to_primrgba(preds["primrgb"], preds["primalpha"], self.primsize)
+        rgb, alpha = hand_finish(self._march(K, Rt, preds))
+        return rgb, alpha, None

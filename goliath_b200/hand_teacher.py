@@ -17,7 +17,10 @@ the OLAT sum in torch.  Here:
   * OLAT compose forward / backward (`gb_olat_compose_fwd / _bwd`).
 
 The features carry no gradient (the reference builds them under no_grad and marks them as leaves nobody reads), so
-the first convolution computes no input gradient."""
+the first convolution computes no input gradient.
+
+`AutoEncoder` (hand_teacher_mvp.py:49-156) is the teacher's whole frame: `hand_mvp.AutoEncoder` with a second pose
+encoder and this decoder, rendered through the hand frame's gather, march and finish."""
 from typing import Optional
 
 import torch
@@ -25,7 +28,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 from torch.autograd import Function
 
-from . import _lib
+from . import _lib, hand_mvp
+from .envmap import compose_envmap
 from .mvpraymarch import build_accel
 from .nn import Conv2dWNUB, FusedLeakyReLU, glorot
 from .utils import compute_raydirs
@@ -134,6 +138,14 @@ def olat_compose(tex, light_intensity, Z, shadow_feat=None, prev=None, want_texo
     if prev is not None and (prev.shape != (B, Z, 3, U, U) or not prev.is_contiguous()):
         raise RuntimeError("prev must be a contiguous [B, Z, 3, U, U] tensor")
     return _OLATCompose.apply(tex, intensity, shadow_feat, prev, Z, bool(want_texolat))
+
+
+def _colour_intensity(light_intensity):
+    """[B,L,1] intensities (SingleLightCycleDecorator's) broadcast over the three colours, as the reference's product
+    does (hand_teacher_mvp.py:407, 478); any other shape is passed on unchanged"""
+    if light_intensity.dim() == 3 and light_intensity.shape[2] == 1:
+        return light_intensity.expand(-1, -1, 3)
+    return light_intensity
 
 
 def _unet_layer(n_in, n_out, size):
@@ -270,8 +282,9 @@ class OLATRGBDecoder(nn.Module):
     # ------------------------------------------------------------------------------------------------ interface
     def forward_rgb(self, campos, K, Rt, primpos, primrot, primscale, primalpha, valid_prims, joint_feat, light_pos,
                     light_intensity, iteration: Optional[int] = None):
-        """hand_teacher_mvp.py:253-493: one chunk of lights ([B,L,3] positions and intensities).  K and Rt are
-        unused, as in the reference."""
+        """hand_teacher_mvp.py:253-493: one chunk of lights ([B,L,3] positions, [B,L,3] or [B,L,1] intensities).  K and
+        Rt are unused, as in the reference."""
+        light_intensity = _colour_intensity(light_intensity)
         prims = self._prims(primpos, primrot, primscale, primalpha, valid_prims)
         rgb, primshadow, texolat = self._chunk(prims, campos, joint_feat, light_pos, light_intensity, iteration, None,
                                                None, True)
@@ -284,6 +297,7 @@ class OLATRGBDecoder(nn.Module):
                 light_intensity, iteration: Optional[int] = None):
         """hand_teacher_mvp.py:496-554: the lights in chunks of `chunksize`; `primrgb` is the sum over the chunks,
         `primshadow` the sum over the chunks of each chunk's light mean, `texolat` (training) the last chunk's."""
+        light_intensity = _colour_intensity(light_intensity)
         prims = self._prims(primpos, primrot, primscale, primalpha, valid_prims)
         L = light_pos.shape[1]
         n_chunks = (L - 1) // self.chunksize + 1
@@ -297,3 +311,50 @@ class OLATRGBDecoder(nn.Module):
         if self.training:
             output["texolat"] = texolat
         return output
+
+
+# ------------------------------------------------------------------------------------------------ the frame
+class AutoEncoder(hand_mvp.AutoEncoder):
+    """hand_teacher_mvp.AutoEncoder (ca_code/models/hand_teacher_mvp.py:49-156): the hand frame with a second pose
+    encoder and the OLAT decoder in place of the RGB slab decoder.  The constructor and the state-dict keys are the
+    reference's: the hand frame's plus `poseencoder2.*` and `relightdecoder.{enc,dec}_layers.*`, so
+    `AutoEncoder(**config.model, assets=assets)` builds from hand_teacher_mvp_example.yml, a teacher checkpoint loads
+    with strict=True and a hand_mvp checkpoint with strict=False (missing exactly the two new modules).
+
+    As in the reference, the constructor leaves `geomdecoder` in eval mode: until the next .train() / .eval() a fresh
+    model marches its geometry without the training branch and relights in training mode.  The frame is the hand
+    frame's: the relit `primrgb` (already activated) and `primalpha` make the template, the valid-primitive gather and
+    the march run through `hand_mvp.AutoEncoder._march`, calibration and background through `hand_finish`.  With an
+    `envbg` (EnvSpinDecorator) the environment is composited behind the render by `envmap.compose_envmap`.  The
+    decorators' other keys are accepted and ignored.  CUDA only; forward and backward issue no host synchronisation
+    after the first call."""
+
+    def __init__(self, assets, image_height, image_width, cal=None, n_pose_dims: int = 54, n_embs: int = 64,
+                 volradius: float = 2000.0, primsize=(16, 16, 8), learn_blur: bool = True):
+        super().__init__(assets, image_height, image_width, cal, n_pose_dims, n_embs, volradius, primsize, learn_blur)
+        self.poseencoder2 = hand_mvp.PoseEncoder(n_pose_dims, n_embs, self.n_prim_x)
+        self.relightdecoder = OLATRGBDecoder(self.uv_size, self.primsize, self.n_prim_x, self.n_prim_y,
+                                             self.raymarcher, self.volradius)
+        self.geomdecoder.eval()
+
+    def forward(self, pose, campos, K, Rt, light_intensity, light_pos, camera_id=None, frame_id=None, iteration=None,
+                background=None, **kwargs):
+        for t, n in ((pose, "pose"), (campos, "campos"), (K, "K"), (Rt, "Rt"), (light_intensity, "light_intensity"),
+                     (light_pos, "light_pos")):
+            if t is None or not t.is_cuda:
+                raise RuntimeError("hand_teacher.AutoEncoder runs on CUDA only (no CPU fallback): %s is %s"
+                                   % (n, "missing" if t is None else "on %s" % t.device))
+        joint = self.poseencoder(pose)
+        geo_preds = self.geomdecoder(pose, joint, iteration)
+        joint2 = self.poseencoder2(pose)
+        dec_preds = self.relightdecoder(campos, K, Rt, geo_preds["primpos"], geo_preds["primrot"],
+                                        geo_preds["primscale"], geo_preds["primalpha"], self.valid_prims, joint2,
+                                        light_pos, light_intensity, iteration)
+        preds = {"primrgb": dec_preds["primrgb"], "valid_prims": self.valid_prims, **geo_preds, **dec_preds}
+        preds["primrgba"] = hand_mvp.slabs_to_primrgba(preds["primrgb"], preds["primalpha"], self.primsize)
+        rgb, alpha = self._finish(self._march(K, Rt, preds), camera_id, background)
+        if "envbg" in kwargs:
+            rgb = compose_envmap(rgb / 255.0, alpha, kwargs["envbg"], K, Rt)
+        preds.update(rgb=rgb, alpha=alpha, ae=self)
+        self._blur(preds, camera_id)
+        return preds
