@@ -37,9 +37,7 @@ def rotate_envmap_mat(image: torch.Tensor, rot_mat: torch.Tensor) -> torch.Tenso
     if img.shape[1] != 3 or rot.shape != (B, 3, 3) or He < 1 or We < 1:
         raise RuntimeError("rotate_envmap_mat: image must be [B,3,He,We] and rot_mat [B,3,3]")
     out = torch.empty_like(img)
-    with torch.cuda.device(img.device):
-        _lib.check(_lib.lib().gb_envmap_rotate(B, He, We, _lib.ptr(img), _lib.ptr(rot), _lib.ptr(out),
-                                               _lib.stream_ptr(img.device)), "envmap_rotate")
+    _lib.kernels().gb_envmap_rotate(B, He, We, img, rot, out)
     return out if batched else out[0]
 
 
@@ -66,11 +64,9 @@ class _ComposeEnvmap(Function):
             raise RuntimeError("compose_envmap: all tensors must be on one device")
         out = torch.empty_like(render)
         hblur = torch.empty_like(render)
-        with torch.cuda.device(render.device):
-            _lib.check(_lib.lib().gb_envmap_compose_fwd(
-                B, H, W, envbg.shape[2], envbg.shape[3], _lib.ptr(render), _lib.ptr(alpha), _lib.ptr(envbg), _lib.ptr(K),
-                _lib.ptr(Rt), Rt.shape[1], Rt.shape[2], _lib.ptr(hblur), _lib.ptr(out), _lib.stream_ptr(render.device)),
-                "envmap_compose_fwd")
+        _lib.kernels().gb_envmap_compose_fwd(
+            B, H, W, envbg.shape[2], envbg.shape[3], render, alpha, envbg, K, Rt, Rt.shape[1], Rt.shape[2], hblur,
+            out)
         ctx.bhw = (B, H, W)
         return out
 
@@ -79,9 +75,7 @@ class _ComposeEnvmap(Function):
         B, H, W = ctx.bhw
         g_out = g_out.contiguous()
         g_render = torch.empty_like(g_out)
-        with torch.cuda.device(g_out.device):
-            _lib.check(_lib.lib().gb_envmap_compose_bwd(B, H, W, _lib.ptr(g_out), _lib.ptr(g_render),
-                                                        _lib.stream_ptr(g_out.device)), "envmap_compose_bwd")
+        _lib.kernels().gb_envmap_compose_bwd(B, H, W, g_out, g_render)
         return g_render, None, None, None, None
 
 
@@ -134,12 +128,11 @@ def _prefilter_levels(levels, num_samples, seed=None):
     if seed is None:
         seed = int(torch.randint(0, 2 ** 63 - 1, (1,), dtype=torch.int64).item())  # torch's default CPU generator
     ptrs = lambda ts: (ctypes.c_void_p * q)(*[t.data_ptr() for t in ts])
-    dev = vs[0].device
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().gb_envmap_prefilter_sg(
+    # every image reaches the kernel through a host array of device pointers, so no tensor argument names the device
+    with torch.cuda.device(vs[0].device):
+        _lib.kernels().gb_envmap_prefilter_sg(
             B, q, (ctypes.c_int32 * (4 * q))(*[int(x) for x in hw]), (ctypes.c_float * q)(*sig), ptrs(vs), ptrs(envs),
-            ptrs(xis) if with_xi else None, int(num_samples), int(seed) & (2 ** 64 - 1), ptrs(outs),
-            _lib.stream_ptr(dev)), "envmap_prefilter_sg")
+            ptrs(xis) if with_xi else None, int(num_samples), int(seed) & (2 ** 64 - 1), ptrs(outs))
     return outs
 
 

@@ -41,10 +41,8 @@ class _EnvmapSpec(Function):
             raise RuntimeError("envmap_specular: sigma / spec_vis must be [B,G(,1)], lightrot [B,3,3]")
         lv, ptrs, hw = _level_args([t.contiguous() for t in levels], B)
         spec = torch.empty(B, G, 3, device=ref_dirs.device, dtype=torch.float32)
-        with torch.cuda.device(ref_dirs.device):
-            _lib.check(_lib.lib().gb_envmap_spec_fwd(B, G, len(lv), ptrs, hw, _lib.ptr(ref_dirs), _lib.ptr(sigma),
-                                                     _lib.ptr(spec_vis), _lib.ptr(lightrot), float(level_scale),
-                                                     _lib.ptr(spec), _lib.stream_ptr(ref_dirs.device)), "envmap_spec_fwd")
+        _lib.kernels().gb_envmap_spec_fwd(B, G, len(lv), ptrs, hw, ref_dirs, sigma, spec_vis, lightrot,
+                                          float(level_scale), spec)
         ctx.save_for_backward(ref_dirs, sigma, spec_vis, lightrot, *lv)
         ctx.meta = (B, G, float(level_scale), spec_vis.shape)
         return spec
@@ -57,11 +55,8 @@ class _EnvmapSpec(Function):
         g_spec = g_spec.contiguous()
         g_dirs = torch.empty_like(ref_dirs)
         g_vis = torch.empty(vis_shape, device=ref_dirs.device, dtype=torch.float32)
-        with torch.cuda.device(ref_dirs.device):
-            _lib.check(_lib.lib().gb_envmap_spec_bwd(B, G, len(lv), ptrs, hw, _lib.ptr(ref_dirs), _lib.ptr(sigma),
-                                                     _lib.ptr(spec_vis), _lib.ptr(lightrot), level_scale, _lib.ptr(g_spec),
-                                                     _lib.ptr(g_dirs), _lib.ptr(g_vis), _lib.stream_ptr(ref_dirs.device)),
-                       "envmap_spec_bwd")
+        _lib.kernels().gb_envmap_spec_bwd(B, G, len(lv), ptrs, hw, ref_dirs, sigma, spec_vis, lightrot, level_scale,
+                                          g_spec, g_dirs, g_vis)
         return (g_dirs, None, g_vis, None, None) + (None,) * len(lv)
 
 

@@ -42,10 +42,8 @@ def face_tex_tail(x, layer, face_bias):
         _lib.check_input(t, n)
     raw = torch.empty(B, Cout, 2 * Hi, 2 * Wi, device=x.device)
     tex = torch.empty_like(raw)
-    with torch.cuda.device(x.device):
-        _lib.check(_lib.lib().gb_face_tex_tail_fwd(
-            B, Cin, Cout, Hi, Wi, _lib.ptr(x), _lib.ptr(v), _lib.ptr(_wn_scale(v, layer.weight_g)), _lib.ptr(bias),
-            _lib.ptr(fb), _lib.ptr(raw), _lib.ptr(tex), _lib.stream_ptr(x.device)), "face_tex_tail_fwd")
+    _lib.kernels().gb_face_tex_tail_fwd(
+        B, Cin, Cout, Hi, Wi, x, v, _wn_scale(v, layer.weight_g), bias, fb, raw, tex)
     return raw, tex
 
 

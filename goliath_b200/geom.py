@@ -21,9 +21,7 @@ class _VertNormals(Function):
         F = vi.shape[0]
         acc = torch.zeros_like(v)
         vn = torch.empty_like(v)
-        with torch.cuda.device(v.device):
-            _lib.check(_lib.lib().gb_vert_normals_fwd(B, V, F, _lib.ptr(v), _lib.ptr(vi), float(eps), _lib.ptr(acc), _lib.ptr(vn),
-                                                      _lib.stream_ptr(v.device)), "vert_normals_fwd")
+        _lib.kernels().gb_vert_normals_fwd(B, V, F, v, vi, float(eps), acc, vn)
         ctx.save_for_backward(v, vi, acc)
         ctx.eps = float(eps)
         return vn
@@ -34,10 +32,7 @@ class _VertNormals(Function):
         B, V, _ = v.shape
         g_acc = torch.empty_like(v)
         g_v = torch.zeros_like(v)
-        with torch.cuda.device(v.device):
-            _lib.check(_lib.lib().gb_vert_normals_bwd(B, V, vi.shape[0], _lib.ptr(v), _lib.ptr(vi), ctx.eps, _lib.ptr(acc),
-                                                      _lib.ptr(g_vn.contiguous()), _lib.ptr(g_acc), _lib.ptr(g_v),
-                                                      _lib.stream_ptr(v.device)), "vert_normals_bwd")
+        _lib.kernels().gb_vert_normals_bwd(B, V, vi.shape[0], v, vi, ctx.eps, acc, g_vn.contiguous(), g_acc, g_v)
         return g_v, None, None
 
 
@@ -60,9 +55,7 @@ class _ValuesToUV(Function):
         if index.shape[-1] != 3 or bary.shape != index.shape:
             raise RuntimeError("values_to_uv: index_img / bary_img must be [U,U,3]")
         out = torch.empty(B, C, U0, U1, device=values.device, dtype=torch.float32)
-        with torch.cuda.device(values.device):
-            _lib.check(_lib.lib().gb_values_to_uv_fwd(B, V, C, U0 * U1, _lib.ptr(values), _lib.ptr(index), _lib.ptr(bary),
-                                                      _lib.ptr(out), _lib.stream_ptr(values.device)), "values_to_uv_fwd")
+        _lib.kernels().gb_values_to_uv_fwd(B, V, C, U0 * U1, values, index, bary, out)
         ctx.save_for_backward(index, bary)
         ctx.shape = (B, V, C, U0 * U1)
         return out
@@ -72,9 +65,7 @@ class _ValuesToUV(Function):
         index, bary = ctx.saved_tensors
         B, V, C, T = ctx.shape
         g_values = torch.zeros(B, V, C, device=g_out.device, dtype=torch.float32)
-        with torch.cuda.device(g_out.device):
-            _lib.check(_lib.lib().gb_values_to_uv_bwd(B, V, C, T, _lib.ptr(index), _lib.ptr(bary), _lib.ptr(g_out.contiguous()),
-                                                      _lib.ptr(g_values), _lib.stream_ptr(g_out.device)), "values_to_uv_bwd")
+        _lib.kernels().gb_values_to_uv_bwd(B, V, C, T, index, bary, g_out.contiguous(), g_values)
         return g_values, None, None
 
 
@@ -170,7 +161,5 @@ def depth_discontuity_mask(depth: torch.Tensor, threshold: float = 40.0, kscale:
         raise RuntimeError("depth_discontuity_mask: depth must be [B,1,H,W] (got %s)" % (tuple(depth.shape),))
     B, _, H, W = depth.shape
     mask = torch.empty(B, 1, H, W, device=depth.device, dtype=torch.bool)
-    with torch.cuda.device(depth.device):
-        _lib.check(_lib.lib().gb_depth_disc_mask(B, H, W, _lib.ptr(depth), float(threshold), _lib.ptr(mask),
-                                                 _lib.stream_ptr(depth.device)), "depth_disc_mask")
+    _lib.kernels().gb_depth_disc_mask(B, H, W, depth, float(threshold), mask)
     return mask

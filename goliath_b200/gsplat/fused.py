@@ -69,7 +69,7 @@ def _blend_plan(T, schedule=True):
     """How the blend mode (gb_get_blend_mode) maps to a tile order and to the rasterize entry points of a render over T
     tiles.  Blend modes 2 and 4 take an SM-affine schedule; `schedule=False` (the exact path, whose tile order is always
     gb_tile_order) keeps the launch-order tiles in every mode."""
-    L = _lib.lib()
+    L = _lib.kernels()
     mode = L.gb_get_blend_mode()
     sched = 1 if schedule and mode in (2, 4) else 0
     return _BlendPlan(sched, L.gb_tile_schedule_ints(T) if sched else T,
@@ -86,27 +86,25 @@ def _bin_tiles(xys, depths, radii, conics, colors, opacity, comp, H, W, cap, pla
     an event to wait for before the colours are read; either may be None.  Returns (bins [T,2], order)."""
     G = xys.size(0)
     dev = xys.device
-    L = _lib.lib()
+    L = _lib.kernels()
     tb = _tile_bounds(H, W, 16)
     T = tb[0] * tb[1]
     bins = torch.empty(T, 2, device=dev, dtype=torch.int32)
     order = torch.empty(plan.order_len, device=dev, dtype=torch.int32)
     ws = _workspace(dev, L.gb_bin_tiles_workspace_bytes(G, T, cap))
-    with torch.cuda.device(dev):
-        args = (G, _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(colors),
-                _lib.ptr(opacity), _lib.ptr(comp), H, W, 16, cap, _lib.ptr(bins), _lib.ptr(order))
-        tail = (_lib.ptr(n_out), _lib.ptr(_overflow_flag(dev)), _lib.ptr(ws), colors_ready, _lib.stream_ptr(dev))
-        if ranked:  # launch-order tiles (the ranked plan never takes the SM-affine schedule)
-            _lib.check(L.gb_bin_tiles_buckets(*args, *map(_lib.ptr, outs), *tail), "bin_tiles_buckets")
-        else:
-            _lib.check(L.gb_bin_tiles_pack_ev(*args, plan.sched, *map(_lib.ptr, outs), *tail), "bin_tiles_pack")
+    args = (G, xys, depths, radii, conics, colors, opacity, comp, H, W, 16, cap, bins, order)
+    tail = (n_out, _overflow_flag(dev), ws, colors_ready)
+    if ranked:  # launch-order tiles (the ranked plan never takes the SM-affine schedule)
+        L.gb_bin_tiles_buckets(*args, *outs, *tail)
+    else:
+        L.gb_bin_tiles_pack_ev(*args, plan.sched, *outs, *tail)
     return bins, order
 
 
 def _blend_grads(H, W, v_out4, v_alpha, opacity, comp, blend, v_colors=None):
-    """Gradients through a blend.  `blend(st, v_out4, v_alpha, v_xy, v_conic, v_col4, v_opeff)` issues the rasterize
-    backward(s) on stream `st`; they accumulate atomically into the last four arrays, which are zeroed here with one
-    fill.  gb_splat_grad_unpack then turns v_col4 / v_opeff into the gradients of the colours (into `v_colors` when
+    """Gradients through a blend.  `blend(v_out4, v_alpha, v_xy, v_conic, v_col4, v_opeff)` issues the rasterize
+    backward(s) on the current stream; they accumulate atomically into the last four arrays, which are zeroed here with
+    one fill.  gb_splat_grad_unpack then turns v_col4 / v_opeff into the gradients of the colours (into `v_colors` when
     given), opacity, compensation and depth.  Returns (v_xy, v_conic, v_colors, v_opacity, v_comp, v_depth)."""
     G = comp.size(0)
     dev = comp.device
@@ -118,12 +116,8 @@ def _blend_grads(H, W, v_out4, v_alpha, opacity, comp, blend, v_colors=None):
     v_col4, v_opeff = acc[5 * G:9 * G].view(G, 4), acc[9 * G:]
     v_colors = torch.empty(G, 3, **f32) if v_colors is None else v_colors
     v_opacity, v_comp, v_depth = torch.empty(G, 1, **f32), torch.empty(G, **f32), torch.empty(G, **f32)
-    with torch.cuda.device(dev):
-        st = _lib.stream_ptr(dev)
-        blend(st, v_out4, v_alpha, v_xy, v_conic, v_col4, v_opeff)
-        _lib.check(_lib.lib().gb_splat_grad_unpack(G, _lib.ptr(v_col4), _lib.ptr(v_opeff), _lib.ptr(opacity),
-                                                   _lib.ptr(comp), _lib.ptr(v_colors), _lib.ptr(v_opacity),
-                                                   _lib.ptr(v_comp), _lib.ptr(v_depth), st), "splat_grad_unpack")
+    blend(v_out4, v_alpha, v_xy, v_conic, v_col4, v_opeff)
+    _lib.kernels().gb_splat_grad_unpack(G, v_col4, v_opeff, opacity, comp, v_colors, v_opacity, v_comp, v_depth)
     return v_xy, v_conic, v_colors, v_opacity, v_comp, v_depth
 
 
@@ -139,7 +133,7 @@ class _RenderFused(Function):
         if G == 0:
             capacity = None  # nothing to bin: the exact path below returns the background (no device-side count to read)
         dev = means3d.device
-        L = _lib.lib()
+        L = _lib.kernels()
         f32 = dict(device=dev, dtype=torch.float32)
         i32 = dict(device=dev, dtype=torch.int32)
         H, W, BW = int(img_height), int(img_width), 16
@@ -152,62 +146,47 @@ class _RenderFused(Function):
         tb = _tile_bounds(H, W, BW)
         T = tb[0] * tb[1]
         plan = _blend_plan(T, schedule=capacity is not None)
-        with torch.cuda.device(dev):
-            st = _lib.stream_ptr(dev)
-            if capacity is not None:
-                # ---- sync-free path: the count never visits the host; buffers hold `capacity` intersections
-                cap = num_intersects = int(capacity)  # "some": the backward walks the bins, not the count
-                gids = torch.empty(cap, **i32)
-                records = torch.empty(cap, 12, **f32)
-                if BINNING == "buckets" and L.gb_bin_tiles_supported(G):
-                    # per-tile buckets, each sorted by (depth, id) in shared memory (csrc/splat_bin_tiles.cu): same
-                    # bins, ids and records as the key sort below, without sorting the intersection keys globally
-                    bins, order = _bin_tiles(xys, depths, radii, conics, colors, opacity, comp, H, W, cap, plan,
-                                             (gids, records))
-                else:
-                    order = torch.empty(plan.order_len, **i32)
-                    cum = torch.empty_like(num_tiles_hit)
-                    ws = _workspace(dev, max(L.gb_cumsum_workspace_bytes(G), L.gb_sort_workspace_bytes(cap)))
-                    _lib.check(L.gb_cumsum_i32(G, _lib.ptr(num_tiles_hit), _lib.ptr(cum), _lib.ptr(ws), st), "cumsum")
-                    n_dev = cum.data_ptr() + 4 * (G - 1)
-                    isect = torch.empty(cap, device=dev, dtype=torch.int64)
-                    gids_u = torch.empty(cap, **i32)
-                    isect_s = torch.empty(cap, device=dev, dtype=torch.int64)
-                    bins = torch.zeros(T, 2, **i32)
-                    _lib.check(L.gb_map_gaussian_to_intersects_dn(G, _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii),
-                                                                  _lib.ptr(cum), H, W, BW, cap, _lib.ptr(isect),
-                                                                  _lib.ptr(gids_u), st), "map_dn")
-                    _lib.check(L.gb_sort_intersects_dn(cap, n_dev, _lib.ptr(isect), _lib.ptr(gids_u),
-                                                       _lib.ptr(isect_s), _lib.ptr(gids), key_bits(T), _lib.ptr(ws),
-                                                       st), "sort_dn")
-                    _lib.check(L.gb_get_tile_bin_edges_dn(cap, n_dev, _lib.ptr(isect_s), _lib.ptr(bins),
-                                                          _lib.ptr(_overflow_flag(dev)), st), "edges_dn")
-                    _lib.check((L.gb_tile_schedule if plan.sched else L.gb_tile_order)(
-                        T, _lib.ptr(bins), _lib.ptr(order), st), "tile_order")
-                    _lib.check(L.gb_pack_records_fused_dn(cap, n_dev, _lib.ptr(gids), _lib.ptr(xys), _lib.ptr(conics),
-                                                          _lib.ptr(colors), _lib.ptr(depths), _lib.ptr(opacity),
-                                                          _lib.ptr(comp), _lib.ptr(records), st),
-                               "pack_records_fused_dn")
+        if capacity is not None:
+            # ---- sync-free path: the count never visits the host; buffers hold `capacity` intersections
+            cap = num_intersects = int(capacity)  # "some": the backward walks the bins, not the count
+            gids = torch.empty(cap, **i32)
+            records = torch.empty(cap, 12, **f32)
+            if BINNING == "buckets" and L.gb_bin_tiles_supported(G):
+                # per-tile buckets, each sorted by (depth, id) in shared memory (csrc/splat_bin_tiles.cu): same
+                # bins, ids and records as the key sort below, without sorting the intersection keys globally
+                bins, order = _bin_tiles(xys, depths, radii, conics, colors, opacity, comp, H, W, cap, plan,
+                                         (gids, records))
             else:
-                num_intersects, cum = compute_cumulative_intersects(num_tiles_hit)
-                if num_intersects < 1:
-                    # reference behaviour with nothing to draw (gsplat 0.1.11 rasterize.py): background, final_Ts = 0
-                    out4.copy_(bg4.expand(H, W, 4))
-                    final_Ts.zero_()
-                    final_idx.zero_()
-                    gids = bins = order = records = torch.empty(0, **i32)
-                else:
-                    _, _, _, gids, bins = bin_and_sort_gaussians(G, num_intersects, xys, depths, radii, cum, tb, BW)
-                    order = torch.empty(T, **i32)
-                    records = torch.empty(num_intersects, 12, **f32)
-                    _lib.check(L.gb_tile_order(T, _lib.ptr(bins), _lib.ptr(order), st), "tile_order")
-                    _lib.check(L.gb_pack_records_fused(num_intersects, _lib.ptr(gids), _lib.ptr(xys), _lib.ptr(conics),
-                                                       _lib.ptr(colors), _lib.ptr(depths), _lib.ptr(opacity),
-                                                       _lib.ptr(comp), _lib.ptr(records), st), "pack_records_fused")
-            if capacity is not None or num_intersects >= 1:
-                _lib.check(plan.fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4),
-                                    _lib.ptr(out4), _lib.ptr(final_Ts), _lib.ptr(final_idx), st),
-                           "rasterize_packed_forward")
+                order = torch.empty(plan.order_len, **i32)
+                cum = torch.empty_like(num_tiles_hit)
+                ws = _workspace(dev, max(L.gb_cumsum_workspace_bytes(G), L.gb_sort_workspace_bytes(cap)))
+                L.gb_cumsum_i32(G, num_tiles_hit, cum, ws)
+                n_dev = cum.data_ptr() + 4 * (G - 1)
+                isect = torch.empty(cap, device=dev, dtype=torch.int64)
+                gids_u = torch.empty(cap, **i32)
+                isect_s = torch.empty(cap, device=dev, dtype=torch.int64)
+                bins = torch.zeros(T, 2, **i32)
+                L.gb_map_gaussian_to_intersects_dn(G, xys, depths, radii, cum, H, W, BW, cap, isect, gids_u)
+                L.gb_sort_intersects_dn(cap, n_dev, isect, gids_u, isect_s, gids, key_bits(T), ws)
+                L.gb_get_tile_bin_edges_dn(cap, n_dev, isect_s, bins, _overflow_flag(dev))
+                (L.gb_tile_schedule if plan.sched else L.gb_tile_order)(T, bins, order)
+                L.gb_pack_records_fused_dn(cap, n_dev, gids, xys, conics, colors, depths, opacity, comp, records)
+        else:
+            num_intersects, cum = compute_cumulative_intersects(num_tiles_hit)
+            if num_intersects < 1:
+                # reference behaviour with nothing to draw (gsplat 0.1.11 rasterize.py): background, final_Ts = 0
+                out4.copy_(bg4.expand(H, W, 4))
+                final_Ts.zero_()
+                final_idx.zero_()
+                gids = bins = order = records = torch.empty(0, **i32)
+            else:
+                _, _, _, gids, bins = bin_and_sort_gaussians(G, num_intersects, xys, depths, radii, cum, tb, BW)
+                order = torch.empty(T, **i32)
+                records = torch.empty(num_intersects, 12, **f32)
+                L.gb_tile_order(T, bins, order)
+                L.gb_pack_records_fused(num_intersects, gids, xys, conics, colors, depths, opacity, comp, records)
+        if capacity is not None or num_intersects >= 1:
+            plan.fwd(H, W, 4, bins, order, records, bg4, out4, final_Ts, final_idx)
         ctx.save_for_backward(means3d, scales, quats, opacity, viewmat, bg4, cov3d, radii, conics, comp, gids, bins, order,
                               records, final_Ts, final_idx)
         ctx.meta = (H, W, num_intersects, float(glob_scale), float(fx), float(fy), plan)
@@ -221,11 +200,9 @@ class _RenderFused(Function):
          final_idx) = ctx.saved_tensors
         H, W, num_intersects, glob_scale, fx, fy, plan = ctx.meta
 
-        def blend(st, *grads):
+        def blend(*grads):
             if num_intersects >= 1:
-                _lib.check(plan.bwd(H, W, 4, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records),
-                                    _lib.ptr(bg4), _lib.ptr(final_Ts), _lib.ptr(final_idx), *map(_lib.ptr, grads), st),
-                           "rasterize_packed_backward")
+                plan.bwd(H, W, 4, gids, bins, order, records, bg4, final_Ts, final_idx, *grads)
 
         v_xy, v_conic, v_colors, v_opacity, v_comp, v_depth = _blend_grads(H, W, v_out4, v_alpha, opacity, comp, blend)
         g_mean, g_scale, g_quat = _project_bwd(means3d, scales, quats, viewmat, cov3d, radii, conics, comp, glob_scale,
@@ -260,7 +237,7 @@ class _RenderBuckets(Function):
         means3d, scales, quats, opacity, colors, viewmat, background = ins
         G = means3d.size(0)
         dev = means3d.device
-        L = _lib.lib()
+        L = _lib.kernels()
         f32 = dict(device=dev, dtype=torch.float32)
         i32 = dict(device=dev, dtype=torch.int32)
         H, W = int(img_height), int(img_width)
@@ -295,30 +272,23 @@ class _RenderBuckets(Function):
                                  ranked=plan.ranked, colors_ready=ev)
         hit_list = hit_count = None
         bg = background if finish else torch.cat([background, background[:1]])
-        with torch.cuda.device(dev):
-            st = _lib.stream_ptr(dev)
-            if plan.ranked:
-                # each forward CTA sorts its tile's bucket into `ranks` before it blends the tile, and stores each
-                # pixel warp's hits (sorted indices; 8 x cap int32 needs no device-side count) so that the backward
-                # walks them instead of culling every tile again
-                hit_list = torch.empty(8 * cap, **i32)
-                hit_count = torch.empty(16 * tb[0] * tb[1] + 2, **i32)
-                head = (_lib.ptr(bins), _lib.ptr(order), _lib.ptr(depths), _lib.ptr(bucket), _lib.ptr(ranks),
-                        _lib.ptr(records), _lib.ptr(bg))
-                tail = (_lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(hit_list), _lib.ptr(hit_count), st)
-                if finish:
-                    rgb, a_img, depth = torch.empty(3, H, W, **f32), torch.empty(1, H, W, **f32), torch.empty(1, H, W, **f32)
-                    _lib.check(L.gb_rasterize_ranked_fwd_sort_finish(H, W, *head, _lib.ptr(rgb), _lib.ptr(a_img),
-                                                                     _lib.ptr(depth), *tail), "rasterize_ranked_forward")
-                else:
-                    out4 = torch.empty(H, W, 4, **f32)
-                    _lib.check(L.gb_rasterize_ranked_fwd_sort_lists(H, W, 4, *head, _lib.ptr(out4), *tail),
-                               "rasterize_ranked_forward")
+        if plan.ranked:
+            # each forward CTA sorts its tile's bucket into `ranks` before it blends the tile, and stores each
+            # pixel warp's hits (sorted indices; 8 x cap int32 needs no device-side count) so that the backward
+            # walks them instead of culling every tile again
+            hit_list = torch.empty(8 * cap, **i32)
+            hit_count = torch.empty(16 * tb[0] * tb[1] + 2, **i32)
+            head = (bins, order, depths, bucket, ranks, records, bg)
+            tail = (final_Ts, final_idx, hit_list, hit_count)
+            if finish:
+                rgb, a_img, depth = torch.empty(3, H, W, **f32), torch.empty(1, H, W, **f32), torch.empty(1, H, W, **f32)
+                L.gb_rasterize_ranked_fwd_sort_finish(H, W, *head, rgb, a_img, depth, *tail)
             else:
                 out4 = torch.empty(H, W, 4, **f32)
-                _lib.check(plan.fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg),
-                                    _lib.ptr(out4), _lib.ptr(final_Ts), _lib.ptr(final_idx), st),
-                           "rasterize_packed_forward")
+                L.gb_rasterize_ranked_fwd_sort_lists(H, W, 4, *head, out4, *tail)
+        else:
+            out4 = torch.empty(H, W, 4, **f32)
+            plan.fwd(H, W, 4, bins, order, records, bg, out4, final_Ts, final_idx)
         alpha = a_img if finish else None
         ctx.save_for_backward(means3d, scales, quats, opacity, viewmat, bg, cov3d, radii, conics, comp, acc, gids, bins,
                               order, records, final_Ts, final_idx, ranks, hit_list, hit_count, alpha)
@@ -338,7 +308,7 @@ class _RenderBuckets(Function):
         H, W, glob_scale, fx, fy, plan, finish = ctx.meta
         G = means3d.size(0)
         dev = means3d.device
-        L = _lib.lib()
+        L = _lib.kernels()
         f32 = dict(device=dev, dtype=torch.float32)
         if ctx.acc_used:  # a second backward through this graph (retain_graph): the projection zeroed acc only once
             acc.zero_()
@@ -346,40 +316,32 @@ class _RenderBuckets(Function):
         v_col4, v_xy, v_conic, v_opeff = _acc_parts(acc, G)
         v_colors, v_opacity = torch.empty(G, 3, **f32), torch.empty(G, 1, **f32)
         g_mean, g_scale, g_quat = torch.empty(G, 3, **f32), torch.empty(G, 3, **f32), torch.empty(G, 4, **f32)
-        accs = tuple(map(_lib.ptr, (v_xy, v_conic, v_col4, v_opeff)))
-        with torch.cuda.device(dev):
-            st = _lib.stream_ptr(dev)
-            if finish:
-                g_rgb, _, g_depth, _ = (None if g is None else g.contiguous() for g in grads)
-                _lib.check(L.gb_rasterize_ranked_bwd_lists_finish(
-                    H, W, _lib.ptr(ranks), _lib.ptr(bins), _lib.ptr(hit_list), _lib.ptr(hit_count), _lib.ptr(records),
-                    _lib.ptr(bg), _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(alpha), _lib.ptr(g_rgb),
-                    _lib.ptr(g_depth), *accs, st), "rasterize_ranked_backward")
+        accs = (v_xy, v_conic, v_col4, v_opeff)
+        if finish:
+            g_rgb, _, g_depth, _ = (None if g is None else g.contiguous() for g in grads)
+            L.gb_rasterize_ranked_bwd_lists_finish(
+                H, W, ranks, bins, hit_list, hit_count, records, bg, final_Ts, final_idx, alpha, g_rgb, g_depth,
+                *accs)
+        else:
+            v_out4, v_alpha, _ = grads
+            v_out4 = torch.zeros(H, W, 4, **f32) if v_out4 is None else v_out4.contiguous()
+            v_alpha = None if v_alpha is None else v_alpha.contiguous()  # NULL: no gradient through alpha
+            if plan.ranked:
+                L.gb_rasterize_ranked_bwd_lists(
+                    H, W, 4, ranks, bins, hit_list, hit_count, records, bg, final_Ts, final_idx, v_out4, v_alpha,
+                    *accs)
             else:
-                v_out4, v_alpha, _ = grads
-                v_out4 = torch.zeros(H, W, 4, **f32) if v_out4 is None else v_out4.contiguous()
-                v_alpha = None if v_alpha is None else v_alpha.contiguous()  # NULL: no gradient through alpha
-                if plan.ranked:
-                    _lib.check(L.gb_rasterize_ranked_bwd_lists(
-                        H, W, 4, _lib.ptr(ranks), _lib.ptr(bins), _lib.ptr(hit_list), _lib.ptr(hit_count),
-                        _lib.ptr(records), _lib.ptr(bg), _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(v_out4),
-                        _lib.ptr(v_alpha), *accs, st), "rasterize_ranked_backward")
-                else:
-                    _lib.check(plan.bwd(H, W, 4, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records),
-                                        _lib.ptr(bg), _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(v_out4),
-                                        _lib.ptr(v_alpha), *accs, st), "rasterize_packed_backward")
-            _lib.check(L.gb_splat_project_bwd(
-                G, _lib.ptr(means3d), _lib.ptr(scales), glob_scale, _lib.ptr(quats), _lib.ptr(viewmat), fx, fy,
-                _lib.ptr(cov3d), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp), _lib.ptr(opacity), _lib.ptr(acc),
-                _lib.ptr(v_colors), _lib.ptr(v_opacity), _lib.ptr(g_mean), _lib.ptr(g_scale), _lib.ptr(g_quat), st),
-                "splat_project_backward")
+                plan.bwd(H, W, 4, gids, bins, order, records, bg, final_Ts, final_idx, v_out4, v_alpha, *accs)
+        L.gb_splat_project_bwd(
+            G, means3d, scales, glob_scale, quats, viewmat, fx, fy, cov3d, radii, conics, comp, opacity, acc,
+            v_colors, v_opacity, g_mean, g_scale, g_quat)
         return (g_mean, g_scale, g_quat, v_opacity, v_colors) + (None,) * 13
 
 
 def _bucket_path(G, capacity):
     """render_fused takes the sync-free bucket path (_RenderBuckets)."""
     return (capacity is not None and SPLIT and BINNING == "buckets" and G > 0
-            and bool(_lib.lib().gb_bin_tiles_supported(G)))
+            and bool(_lib.kernels().gb_bin_tiles_supported(G)))
 
 
 def blend_finishes_view(G, capacity):

@@ -37,7 +37,7 @@ class _RenderShared(Function):
             raise RuntimeError("render_shared: colors must be [C,G,3]")
         C, G = colors.shape[0], means3d.size(0)
         dev = means3d.device
-        L = _lib.lib()
+        L = _lib.kernels()
         if not L.gb_bin_tiles_supported(G):
             raise RuntimeError("render_shared: %d Gaussians exceed the bucket binning's range (gb_bin_tiles_supported)" % G)
         f32 = dict(device=dev, dtype=torch.float32)
@@ -64,37 +64,29 @@ class _RenderShared(Function):
         n_dev = torch.empty(1, **i32)
         bins, order = _bin_tiles(xys, depths, radii, conics, colors[0], opacity, comp, H, W, cap, plan, (gids, records),
                                  n_out=n_dev)
-        with torch.cuda.device(dev):
-            st = _lib.stream_ptr(dev)
-            _lib.check(plan.fwd(H, W, 4, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4), _lib.ptr(out4),
-                                _lib.ptr(final_Ts), _lib.ptr(final_idx), st), "rasterize_packed_forward")
-            if n_isect == 0:
-                # as render_fused(capacity=None): the reference's final_Ts = 0 when nothing is drawn, so alpha = 1
-                final_Ts.zero_()
-                final_idx.zero_()
-            rgb[0].copy_(out4[..., :3])
-            multi = MODE == "multi" and C > 1
-            wide = None
-            if multi:
-                wide = torch.empty(cap, 20, **f32)
-                _lib.check(L.gb_records_widen(cap, _lib.ptr(n_dev), _lib.ptr(records), _lib.ptr(wide), st), "records_widen")
-                stage = torch.empty(4, H, W, 3, **f32)  # a group's four images (the last group may be partial)
-                for c in range(1, C, 4):
-                    nk = min(4, C - c)
-                    _lib.check(L.gb_records_set_colors4(cap, _lib.ptr(n_dev), _lib.ptr(gids), _lib.ptr(colors[c]), nk, G,
-                                                        _lib.ptr(wide), st), "records_set_colors4")
-                    dst = rgb[c:c + 4] if nk == 4 else stage
-                    _lib.check(L.gb_rasterize_multi_fwd(H, W, _lib.ptr(bins), _lib.ptr(order), plan.sched, _lib.ptr(wide),
-                                                        _lib.ptr(background), _lib.ptr(dst), st), "rasterize_multi_forward")
-                    if nk < 4:
-                        rgb[c:c + nk].copy_(stage[:nk])
-            else:
-                for c in range(1, C):
-                    _lib.check(L.gb_records_set_colors(cap, _lib.ptr(n_dev), _lib.ptr(gids), _lib.ptr(colors[c]), _lib.ptr(depths),
-                                                       _lib.ptr(records), st), "records_set_colors")
-                    _lib.check(plan.fwd(H, W, 3, _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(background),
-                                        _lib.ptr(rgb[c]), _lib.ptr(scratch_T), _lib.ptr(scratch_idx), st),
-                               "rasterize_packed_forward")
+        plan.fwd(H, W, 4, bins, order, records, bg4, out4, final_Ts, final_idx)
+        if n_isect == 0:
+            # as render_fused(capacity=None): the reference's final_Ts = 0 when nothing is drawn, so alpha = 1
+            final_Ts.zero_()
+            final_idx.zero_()
+        rgb[0].copy_(out4[..., :3])
+        multi = MODE == "multi" and C > 1
+        wide = None
+        if multi:
+            wide = torch.empty(cap, 20, **f32)
+            L.gb_records_widen(cap, n_dev, records, wide)
+            stage = torch.empty(4, H, W, 3, **f32)  # a group's four images (the last group may be partial)
+            for c in range(1, C, 4):
+                nk = min(4, C - c)
+                L.gb_records_set_colors4(cap, n_dev, gids, colors[c], nk, G, wide)
+                dst = rgb[c:c + 4] if nk == 4 else stage
+                L.gb_rasterize_multi_fwd(H, W, bins, order, plan.sched, wide, background, dst)
+                if nk < 4:
+                    rgb[c:c + nk].copy_(stage[:nk])
+        else:
+            for c in range(1, C):
+                L.gb_records_set_colors(cap, n_dev, gids, colors[c], depths, records)
+                plan.fwd(H, W, 3, bins, order, records, background, rgb[c], scratch_T, scratch_idx)
         ctx.save_for_backward(means3d, scales, quats, opacity, colors, viewmat, bg4, cov3d, depths, radii, conics, comp, gids,
                               bins, order, records, n_dev, final_Ts, final_idx)
         ctx.wide = wide  # scratch of the multi-condition passes (colour part rewritten per group in the backward)
@@ -109,7 +101,7 @@ class _RenderShared(Function):
          n_dev, final_Ts, final_idx) = ctx.saved_tensors
         C, G, H, W, cap, glob_scale, fx, fy, plan = ctx.meta
         dev = means3d.device
-        L = _lib.lib()
+        L = _lib.kernels()
         f32 = dict(device=dev, dtype=torch.float32)
         v_rgb = torch.zeros(C, H, W, 3, **f32) if v_rgb is None else v_rgb.contiguous()
         v_out4 = torch.empty(H, W, 4, **f32)
@@ -121,7 +113,7 @@ class _RenderShared(Function):
         wide = ctx.wide
         v_colors = (torch.empty if wide is not None else torch.zeros)(C, G, 3, **f32)  # multi: every table is overwritten
 
-        def blend(st, v_out4, v_alpha, v_xy, v_conic, v_col4, v_opeff):
+        def blend(v_out4, v_alpha, v_xy, v_conic, v_col4, v_opeff):
             zero_alpha = None  # the conditions after the first carry no alpha gradient
             bg3 = bg4[:3].contiguous()
             if wide is not None:
@@ -130,33 +122,25 @@ class _RenderShared(Function):
                 stage = torch.zeros(4, H, W, 3, **f32)
                 for c in range(1, C, 4):
                     nk = min(4, C - c)
-                    _lib.check(L.gb_records_set_colors4(cap, _lib.ptr(n_dev), _lib.ptr(gids), _lib.ptr(colors[c]), nk, G,
-                                                        _lib.ptr(wide), st), "records_set_colors4")
+                    L.gb_records_set_colors4(cap, n_dev, gids, colors[c], nk, G, wide)
                     src = v_rgb[c:c + 4]
                     if nk < 4:
                         stage[:nk].copy_(v_rgb[c:c + nk])
                         src = stage
-                    _lib.check(L.gb_rasterize_multi_bwd(H, W, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), plan.sched,
-                                                        _lib.ptr(wide), _lib.ptr(bg3), _lib.ptr(final_Ts), _lib.ptr(final_idx),
-                                                        _lib.ptr(src), _lib.ptr(v_xy), _lib.ptr(v_conic), _lib.ptr(v12),
-                                                        _lib.ptr(v_opeff), st), "rasterize_multi_backward")
-                    _lib.check(L.gb_colors12_unpack(G, nk, _lib.ptr(v12), _lib.ptr(v_colors[c]), st), "colors12_unpack")
+                    L.gb_rasterize_multi_bwd(H, W, gids, bins, order, plan.sched, wide, bg3, final_Ts, final_idx, src,
+                                             v_xy, v_conic, v12, v_opeff)
+                    L.gb_colors12_unpack(G, nk, v12, v_colors[c])
             else:
                 # the records hold the colours of condition C-1 (left by the forward): walk the conditions downwards
                 for c in range(C - 1, 0, -1):
                     if c != C - 1:
-                        _lib.check(L.gb_records_set_colors(cap, _lib.ptr(n_dev), _lib.ptr(gids), _lib.ptr(colors[c]),
-                                                           _lib.ptr(depths), _lib.ptr(records), st), "records_set_colors")
-                    _lib.check(plan.bwd(H, W, 3, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records),
-                                        _lib.ptr(bg3), _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(v_rgb[c]),
-                                        _lib.ptr(zero_alpha), _lib.ptr(v_xy), _lib.ptr(v_conic), _lib.ptr(v_colors[c]),
-                                        _lib.ptr(v_opeff), st), "rasterize_packed_backward")
+                        L.gb_records_set_colors(cap, n_dev, gids, colors[c], depths, records)
+                    plan.bwd(H, W, 3, gids, bins, order, records, bg3, final_Ts, final_idx, v_rgb[c], zero_alpha, v_xy,
+                             v_conic, v_colors[c], v_opeff)
                 if C > 1:
-                    _lib.check(L.gb_records_set_colors(cap, _lib.ptr(n_dev), _lib.ptr(gids), _lib.ptr(colors[0]), _lib.ptr(depths),
-                                                       _lib.ptr(records), st), "records_set_colors")
-            _lib.check(plan.bwd(H, W, 4, _lib.ptr(gids), _lib.ptr(bins), _lib.ptr(order), _lib.ptr(records), _lib.ptr(bg4),
-                                _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(v_out4), _lib.ptr(v_alpha), _lib.ptr(v_xy),
-                                _lib.ptr(v_conic), _lib.ptr(v_col4), _lib.ptr(v_opeff), st), "rasterize_packed_backward")
+                    L.gb_records_set_colors(cap, n_dev, gids, colors[0], depths, records)
+            plan.bwd(H, W, 4, gids, bins, order, records, bg4, final_Ts, final_idx, v_out4, v_alpha, v_xy, v_conic,
+                     v_col4, v_opeff)
 
         v_xy, v_conic, _, v_opacity, v_comp, v_dep = _blend_grads(H, W, v_out4, v_alpha, opacity, comp, blend, v_colors[0])
         g_mean, g_scale, g_quat = _project_bwd(means3d, scales, quats, viewmat, cov3d, radii, conics, comp, glob_scale,

@@ -53,17 +53,14 @@ def _project_fwd(means3d, scales, quats, viewmat, glob_scale, fx, fy, cx, cy, im
     cov3d, xys, depths = torch.empty(G, 6, **f32), torch.empty(G, 2, **f32), torch.empty(G, **f32)
     radii, conics, comp = torch.empty(G, **i32), torch.empty(G, 3, **f32), torch.empty(G, **f32)
     num_tiles_hit = torch.empty(G, **i32)
-    L = _lib.lib()
-    args = (G, _lib.ptr(means3d), _lib.ptr(scales), float(glob_scale), _lib.ptr(quats), _lib.ptr(viewmat), float(fx),
-            float(fy), float(cx), float(cy), int(img_height), int(img_width), int(block_width), float(clip_thresh),
-            _lib.ptr(cov3d), _lib.ptr(xys), _lib.ptr(depths), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp),
-            _lib.ptr(num_tiles_hit))
-    with torch.cuda.device(dev):
-        if grad_acc is None:
-            _lib.check(L.gb_project_gaussians_fwd(*args, _lib.stream_ptr(dev)), "project_gaussians_forward")
-        else:
-            _lib.check(L.gb_project_gaussians_fwd_acc(*args, _lib.ptr(grad_acc), _lib.stream_ptr(dev)),
-                       "project_gaussians_forward")
+    L = _lib.kernels()
+    args = (G, means3d, scales, float(glob_scale), quats, viewmat, float(fx), float(fy), float(cx), float(cy),
+            int(img_height), int(img_width), int(block_width), float(clip_thresh), cov3d, xys, depths, radii, conics,
+            comp, num_tiles_hit)
+    if grad_acc is None:
+        L.gb_project_gaussians_fwd(*args)
+    else:
+        L.gb_project_gaussians_fwd_acc(*args, grad_acc)
     return xys, depths, radii, conics, comp, num_tiles_hit, cov3d
 
 
@@ -81,12 +78,9 @@ def _project_bwd(means3d, scales, quats, viewmat, cov3d, radii, conics, comp, gl
     v_xy, v_depth, v_conic, v_comp = z(v_xy, (G, 2)), z(v_depth, (G,)), z(v_conic, (G, 3)), z(v_comp, (G,))
     g_cov2d, g_cov3d = torch.empty(G, 3, **f32), torch.empty(G, 6, **f32)
     g_mean, g_scale, g_quat = torch.empty(G, 3, **f32), torch.empty(G, 3, **f32), torch.empty(G, 4, **f32)
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().gb_project_gaussians_bwd(
-            G, _lib.ptr(means3d), _lib.ptr(scales), float(glob_scale), _lib.ptr(quats), _lib.ptr(viewmat), float(fx),
-            float(fy), _lib.ptr(cov3d), _lib.ptr(radii), _lib.ptr(conics), _lib.ptr(comp), _lib.ptr(v_xy),
-            _lib.ptr(v_depth), _lib.ptr(v_conic), _lib.ptr(v_comp), _lib.ptr(g_cov2d), _lib.ptr(g_cov3d),
-            _lib.ptr(g_mean), _lib.ptr(g_scale), _lib.ptr(g_quat), _lib.stream_ptr(dev)), "project_gaussians_backward")
+    _lib.kernels().gb_project_gaussians_bwd(
+        G, means3d, scales, float(glob_scale), quats, viewmat, float(fx), float(fy), cov3d, radii, conics, comp,
+        v_xy, v_depth, v_conic, v_comp, g_cov2d, g_cov3d, g_mean, g_scale, g_quat)
     return g_mean, g_scale, g_quat
 
 

@@ -48,9 +48,7 @@ def _bin_cached(xys, depths, radii, num_tiles_hit, img_height, img_width, block_
         if block_width == 16:
             T = tile_bounds[0] * tile_bounds[1]
             tile_order = torch.empty(T, dtype=torch.int32, device=dev)
-            with torch.cuda.device(dev):
-                _lib.check(_lib.lib().gb_tile_order(T, _lib.ptr(tile_bins), _lib.ptr(tile_order),
-                                                    _lib.stream_ptr(dev)), "tile_order")
+            _lib.kernels().gb_tile_order(T, tile_bins, tile_order)
         res = (num_intersects, gaussian_ids_sorted, tile_bins, tile_order)
     if key is not None:
         # the strong references keep the storages (and the token) alive, so equal pointers / ids are the same objects
@@ -109,7 +107,7 @@ class _RasterizeGaussians(Function):
         _lib.check_input(num_tiles_hit, "num_tiles_hit", torch.int32)
         C = colors.shape[-1]
         dev = xys.device
-        L = _lib.lib()
+        L = _lib.kernels()
         num_intersects, gaussian_ids_sorted, tile_bins, tile_order = _bin_cached(
             xys, depths, radii, num_tiles_hit, img_height, img_width, block_width)
         records = None
@@ -123,22 +121,15 @@ class _RasterizeGaussians(Function):
             out_img = torch.empty(img_height, img_width, C, device=dev, dtype=torch.float32)
             final_Ts = torch.empty(img_height, img_width, device=dev, dtype=torch.float32)
             final_idx = torch.empty(img_height, img_width, device=dev, dtype=torch.int32)
-            with torch.cuda.device(dev):
-                st = _lib.stream_ptr(dev)
-                if block_width == 16:
-                    records = torch.empty(num_intersects, 12, device=dev, dtype=torch.float32)
-                    _lib.check(L.gb_pack_records(num_intersects, C, _lib.ptr(gaussian_ids_sorted), _lib.ptr(xys),
-                                                 _lib.ptr(conics), _lib.ptr(colors), _lib.ptr(opacity),
-                                                 _lib.ptr(records), st), "pack_records")
-                    _lib.check(L.gb_rasterize_packed_fwd(img_height, img_width, C, _lib.ptr(tile_bins),
-                                                         _lib.ptr(tile_order), _lib.ptr(records), _lib.ptr(background),
-                                                         _lib.ptr(out_img), _lib.ptr(final_Ts), _lib.ptr(final_idx),
-                                                         st), "rasterize_packed_forward")
-                else:
-                    _lib.check(L.gb_rasterize_fwd(
-                        img_height, img_width, block_width, C, _lib.ptr(gaussian_ids_sorted), _lib.ptr(tile_bins),
-                        _lib.ptr(xys), _lib.ptr(conics), _lib.ptr(colors), _lib.ptr(opacity), _lib.ptr(background),
-                        _lib.ptr(out_img), _lib.ptr(final_Ts), _lib.ptr(final_idx), st), "rasterize_forward")
+            if block_width == 16:
+                records = torch.empty(num_intersects, 12, device=dev, dtype=torch.float32)
+                L.gb_pack_records(num_intersects, C, gaussian_ids_sorted, xys, conics, colors, opacity, records)
+                L.gb_rasterize_packed_fwd(img_height, img_width, C, tile_bins, tile_order, records, background,
+                                          out_img, final_Ts, final_idx)
+            else:
+                L.gb_rasterize_fwd(
+                    img_height, img_width, block_width, C, gaussian_ids_sorted, tile_bins, xys, conics, colors,
+                    opacity, background, out_img, final_Ts, final_idx)
 
         ctx.img_width, ctx.img_height = img_width, img_height
         ctx.num_intersects, ctx.block_width = num_intersects, block_width
@@ -158,30 +149,23 @@ class _RasterizeGaussians(Function):
         (gaussian_ids_sorted, tile_bins, xys, conics, colors, opacity, background, final_Ts, final_idx) = saved[:9]
         if v_out_alpha is None:
             v_out_alpha = torch.zeros_like(v_out_img[..., 0])
-        dev = xys.device
         C = colors.shape[-1]
         v_xy = torch.zeros_like(xys)
         v_conic = torch.zeros_like(conics)
         v_colors = torch.zeros_like(colors)
         v_opacity = torch.zeros_like(opacity)
         if ctx.num_intersects >= 1:
-            L = _lib.lib()
+            L = _lib.kernels()
             v_out_img = v_out_img.contiguous()
             v_out_alpha = v_out_alpha.contiguous()
-            with torch.cuda.device(dev):
-                st = _lib.stream_ptr(dev)
-                if ctx.packed:
-                    records, tile_order = saved[9], saved[10]
-                    _lib.check(L.gb_rasterize_packed_bwd(
-                        ctx.img_height, ctx.img_width, C, _lib.ptr(gaussian_ids_sorted), _lib.ptr(tile_bins),
-                        _lib.ptr(tile_order), _lib.ptr(records), _lib.ptr(background), _lib.ptr(final_Ts),
-                        _lib.ptr(final_idx), _lib.ptr(v_out_img), _lib.ptr(v_out_alpha), _lib.ptr(v_xy),
-                        _lib.ptr(v_conic), _lib.ptr(v_colors), _lib.ptr(v_opacity), st), "rasterize_packed_backward")
-                else:
-                    _lib.check(L.gb_rasterize_bwd(
-                        ctx.img_height, ctx.img_width, ctx.block_width, C, _lib.ptr(gaussian_ids_sorted),
-                        _lib.ptr(tile_bins), _lib.ptr(xys), _lib.ptr(conics), _lib.ptr(colors), _lib.ptr(opacity),
-                        _lib.ptr(background), _lib.ptr(final_Ts), _lib.ptr(final_idx), _lib.ptr(v_out_img),
-                        _lib.ptr(v_out_alpha), _lib.ptr(v_xy), _lib.ptr(v_conic), _lib.ptr(v_colors),
-                        _lib.ptr(v_opacity), st), "rasterize_backward")
+            if ctx.packed:
+                records, tile_order = saved[9], saved[10]
+                L.gb_rasterize_packed_bwd(
+                    ctx.img_height, ctx.img_width, C, gaussian_ids_sorted, tile_bins, tile_order, records,
+                    background, final_Ts, final_idx, v_out_img, v_out_alpha, v_xy, v_conic, v_colors, v_opacity)
+            else:
+                L.gb_rasterize_bwd(
+                    ctx.img_height, ctx.img_width, ctx.block_width, C, gaussian_ids_sorted, tile_bins, xys, conics,
+                    colors, opacity, background, final_Ts, final_idx, v_out_img, v_out_alpha, v_xy, v_conic,
+                    v_colors, v_opacity)
         return (v_xy, None, None, v_conic, None, v_colors, v_opacity, None, None, None, None, None)

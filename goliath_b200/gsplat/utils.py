@@ -42,10 +42,8 @@ def compute_cumulative_intersects(num_tiles_hit: Tensor) -> Tuple[int, Tensor]:
     if n == 0:
         return 0, cum
     dev = num_tiles_hit.device
-    ws = _workspace(dev, _lib.lib().gb_cumsum_workspace_bytes(n))
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().gb_cumsum_i32(n, _lib.ptr(num_tiles_hit), _lib.ptr(cum), _lib.ptr(ws),
-                                            _lib.stream_ptr(dev)), "cumsum")
+    ws = _workspace(dev, _lib.kernels().gb_cumsum_workspace_bytes(n))
+    _lib.kernels().gb_cumsum_i32(n, num_tiles_hit, cum, ws)
     num_intersects = int(cum[-1].item())  # same host sync as the reference (gsplat utils: cum_tiles_hit[-1].item())
     return num_intersects, cum
 
@@ -56,11 +54,9 @@ def map_gaussian_to_intersects(num_points: int, num_intersects: int, xys: Tensor
     isect_ids = torch.empty(num_intersects, dtype=torch.int64, device=dev)
     gaussian_ids = torch.empty(num_intersects, dtype=torch.int32, device=dev)
     img_w, img_h = tile_bounds[0] * block_width, tile_bounds[1] * block_width
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().gb_map_gaussian_to_intersects(
-            num_points, _lib.ptr(xys.contiguous()), _lib.ptr(depths.contiguous()), _lib.ptr(radii.contiguous()),
-            _lib.ptr(cum_tiles_hit.contiguous()), img_h, img_w, block_width, _lib.ptr(isect_ids),
-            _lib.ptr(gaussian_ids), _lib.stream_ptr(dev)), "map_gaussian_to_intersects")
+    _lib.kernels().gb_map_gaussian_to_intersects(
+        num_points, xys.contiguous(), depths.contiguous(), radii.contiguous(), cum_tiles_hit.contiguous(), img_h,
+        img_w, block_width, isect_ids, gaussian_ids)
     return isect_ids, gaussian_ids
 
 
@@ -71,20 +67,16 @@ def sort_intersects(isect_ids: Tensor, gaussian_ids: Tensor, num_tiles: int) -> 
     gids_sorted = torch.empty_like(gaussian_ids)
     if n == 0:
         return isect_sorted, gids_sorted
-    ws = _workspace(dev, _lib.lib().gb_sort_workspace_bytes(n))
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().gb_sort_intersects(n, _lib.ptr(isect_ids), _lib.ptr(gaussian_ids),
-                                                 _lib.ptr(isect_sorted), _lib.ptr(gids_sorted), key_bits(num_tiles),
-                                                 _lib.ptr(ws), _lib.stream_ptr(dev)), "sort_intersects")
+    ws = _workspace(dev, _lib.kernels().gb_sort_workspace_bytes(n))
+    _lib.kernels().gb_sort_intersects(n, isect_ids, gaussian_ids, isect_sorted, gids_sorted, key_bits(num_tiles),
+                                      ws)
     return isect_sorted, gids_sorted
 
 
 def get_tile_bin_edges(num_intersects: int, isect_ids_sorted: Tensor, tile_bounds) -> Tensor:
     dev = isect_ids_sorted.device
     tile_bins = torch.zeros(tile_bounds[0] * tile_bounds[1], 2, dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().gb_get_tile_bin_edges(num_intersects, _lib.ptr(isect_ids_sorted), _lib.ptr(tile_bins),
-                                                    _lib.stream_ptr(dev)), "get_tile_bin_edges")
+    _lib.kernels().gb_get_tile_bin_edges(num_intersects, isect_ids_sorted, tile_bins)
     return tile_bins
 
 

@@ -110,10 +110,8 @@ class _PrimTransforms(Function):
         primpos = torch.empty(B, K, 3, device=dev)
         primrot = torch.empty(B, K, 3, 3, device=dev)
         primscale = torch.empty(B, K, 3, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_mvp_prim_transform_fwd(
-                B, K, _lib.ptr(dec), _lib.ptr(posbase), _lib.ptr(rotbase), float(prim_scale), int(zero_delta),
-                _lib.ptr(primpos), _lib.ptr(primrot), _lib.ptr(primscale), _lib.stream_ptr(dev)), "mvp_prim_transform_fwd")
+        _lib.kernels().gb_mvp_prim_transform_fwd(
+            B, K, dec, posbase, rotbase, float(prim_scale), int(zero_delta), primpos, primrot, primscale)
         ctx.save_for_backward(dec, posbase, rotbase)
         ctx.meta = (B, K, float(prim_scale), int(zero_delta))
         ctx.set_materialize_grads(False)
@@ -125,10 +123,8 @@ class _PrimTransforms(Function):
         B, K, prim_scale, zero_delta = ctx.meta
         g_pos, g_rot, g_scale = (None if g is None else g.contiguous() for g in (g_pos, g_rot, g_scale))
         g_dec = torch.empty_like(dec)
-        with torch.cuda.device(dec.device):
-            _lib.check(_lib.lib().gb_mvp_prim_transform_bwd(
-                B, K, _lib.ptr(dec), _lib.ptr(posbase), _lib.ptr(rotbase), prim_scale, zero_delta, _lib.ptr(g_pos),
-                _lib.ptr(g_rot), _lib.ptr(g_scale), _lib.ptr(g_dec), _lib.stream_ptr(dec.device)), "mvp_prim_transform_bwd")
+        _lib.kernels().gb_mvp_prim_transform_bwd(
+            B, K, dec, posbase, rotbase, prim_scale, zero_delta, g_pos, g_rot, g_scale, g_dec)
         return g_dec, None, None, None, None
 
 
@@ -150,10 +146,8 @@ class _SlabsToPrims(Function):
             raise RuntimeError("primrgb must be [B,PZ,3,U,U] and primalpha [B,PZ,1,U,U] with PZ = primsize[2]")
         PSX, PSY = int(primsize[0]), int(primsize[1])
         tpl = torch.empty(B, n_out, PZ, PSY, PSX, 4, device=rgb.device)
-        with torch.cuda.device(rgb.device):
-            _lib.check(_lib.lib().gb_mvp_slab_to_prims_fwd(
-                B, PZ, U, PSX, PSY, n_out, _lib.ptr(rgb), _lib.ptr(alpha), _lib.ptr(prim_slot), float(rgb_mul),
-                float(rgb_add), int(relu), _lib.ptr(tpl), _lib.stream_ptr(rgb.device)), "mvp_slab_to_prims_fwd")
+        _lib.kernels().gb_mvp_slab_to_prims_fwd(
+            B, PZ, U, PSX, PSY, n_out, rgb, alpha, prim_slot, float(rgb_mul), float(rgb_add), int(relu), tpl)
         ctx.save_for_backward(rgb, alpha, prim_slot)
         ctx.meta = (B, PZ, U, PSX, PSY, n_out, float(rgb_mul), float(rgb_add), int(relu))
         return tpl
@@ -164,10 +158,8 @@ class _SlabsToPrims(Function):
         B, PZ, U, PSX, PSY, n_out, rgb_mul, rgb_add, relu = ctx.meta
         g_tpl = g_tpl.contiguous()
         g_rgb, g_alpha = torch.empty_like(rgb), torch.empty_like(alpha)
-        with torch.cuda.device(rgb.device):
-            _lib.check(_lib.lib().gb_mvp_slab_to_prims_bwd(
-                B, PZ, U, PSX, PSY, n_out, _lib.ptr(rgb), _lib.ptr(alpha), _lib.ptr(prim_slot), rgb_mul, rgb_add, relu,
-                _lib.ptr(g_tpl), _lib.ptr(g_rgb), _lib.ptr(g_alpha), _lib.stream_ptr(rgb.device)), "mvp_slab_to_prims_bwd")
+        _lib.kernels().gb_mvp_slab_to_prims_bwd(
+            B, PZ, U, PSX, PSY, n_out, rgb, alpha, prim_slot, rgb_mul, rgb_add, relu, g_tpl, g_rgb, g_alpha)
         return g_rgb, g_alpha, None, None, None, None, None, None
 
 
@@ -248,10 +240,8 @@ def prim_base_frames(geom_lbs, vt, prim_vidx_img, prim_vtidx_img, prim_bary_img)
         raise RuntimeError("index / barycentric images must be [S,S,3] and vt [NT,2]")
     posbase = torch.empty(B, T, 3, device=geom.device)
     rotbase = torch.empty(B, T, 3, 3, device=geom.device)
-    with torch.cuda.device(geom.device):
-        _lib.check(_lib.lib().gb_mvp_prim_frames_fwd(
-            B, V, vt.shape[0], T, _lib.ptr(geom), _lib.ptr(vidx), _lib.ptr(vtidx), _lib.ptr(bary), _lib.ptr(vt), None,
-            None, _lib.ptr(posbase), _lib.ptr(rotbase), None, _lib.stream_ptr(geom.device)), "mvp_prim_frames_fwd")
+    _lib.kernels().gb_mvp_prim_frames_fwd(
+        B, V, vt.shape[0], T, geom, vidx, vtidx, bary, vt, None, None, posbase, rotbase, None)
     return posbase, rotbase
 
 
@@ -272,10 +262,8 @@ def view_cos_uv(geom_lbs, vi, campos, prim_vidx_img, prim_bary_img):
         raise RuntimeError("prim_vidx_img / prim_bary_img must be [S,S,3] and campos [B,3]")
     vn = vert_normals(geom, vi)
     out = torch.empty(B, 1, S0, S1, device=geom.device)
-    with torch.cuda.device(geom.device):
-        _lib.check(_lib.lib().gb_mvp_prim_frames_fwd(
-            B, V, 0, S0 * S1, _lib.ptr(geom), _lib.ptr(vidx), None, _lib.ptr(bary), None, _lib.ptr(vn),
-            _lib.ptr(campos), None, None, _lib.ptr(out), _lib.stream_ptr(geom.device)), "mvp_prim_frames_fwd")
+    _lib.kernels().gb_mvp_prim_frames_fwd(
+        B, V, 0, S0 * S1, geom, vidx, None, bary, None, vn, campos, None, None, out)
     return out
 
 
@@ -359,11 +347,8 @@ class _ValidGather(Function):
         tpl = torch.empty((B, n_valid) + tuple(template.shape[2:]), device=dev)
         pos, scale = torch.empty(B, n_valid, 3, device=dev), torch.empty(B, n_valid, 3, device=dev)
         rot = torch.empty(B, n_valid, 3, 3, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_hand_valid_gather_fwd(
-                B, K, n_valid, E, _lib.ptr(slot), _lib.ptr(template), _lib.ptr(primpos), _lib.ptr(primrot),
-                _lib.ptr(primscale), inv, _lib.ptr(tpl), _lib.ptr(pos), _lib.ptr(rot), _lib.ptr(scale),
-                _lib.stream_ptr(dev)), "hand_valid_gather_fwd")
+        _lib.kernels().gb_hand_valid_gather_fwd(
+            B, K, n_valid, E, slot, template, primpos, primrot, primscale, inv, tpl, pos, rot, scale)
         ctx.save_for_backward(slot)
         ctx.meta = (tuple(template.shape), n_valid, inv)
         return tpl, pos, rot, scale
@@ -378,11 +363,8 @@ class _ValidGather(Function):
         gt = torch.empty(shape, device=dev)
         gp, gr, gs = torch.empty(B, K, 3, device=dev), torch.empty(B, K, 3, 3, device=dev), torch.empty(B, K, 3,
                                                                                                       device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_hand_valid_gather_bwd(
-                B, K, n_valid, gt[0, 0].numel(), _lib.ptr(slot), _lib.ptr(g_tpl), _lib.ptr(g_pos), _lib.ptr(g_rot),
-                _lib.ptr(g_scale), inv, _lib.ptr(gt), _lib.ptr(gp), _lib.ptr(gr), _lib.ptr(gs),
-                _lib.stream_ptr(dev)), "hand_valid_gather_bwd")
+        _lib.kernels().gb_hand_valid_gather_bwd(
+            B, K, n_valid, gt[0, 0].numel(), slot, g_tpl, g_pos, g_rot, g_scale, inv, gt, gp, gr, gs)
         return gt, gp, gr, gs, None, None, None
 
 
@@ -425,10 +407,8 @@ class _HandFinish(Function):
             raise RuntimeError("hand_finish: cal_w and cal_b go together")
         dev = rayrgba.device
         rgb, alpha = torch.empty(B, 3, H, W, device=dev), torch.empty(B, 1, H, W, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_hand_finish_fwd(
-                B, H, W, _lib.ptr(rayrgba), _lib.ptr(opt["cal_w"]), _lib.ptr(opt["cal_b"]), _lib.ptr(opt["grey"]),
-                _lib.ptr(opt["background"]), _lib.ptr(rgb), _lib.ptr(alpha), _lib.stream_ptr(dev)), "hand_finish_fwd")
+        _lib.kernels().gb_hand_finish_fwd(
+            B, H, W, rayrgba, opt["cal_w"], opt["cal_b"], opt["grey"], opt["background"], rgb, alpha)
         ctx.save_for_backward(rayrgba, opt["cal_w"], opt["grey"], opt["background"])
         ctx.set_materialize_grads(False)
         return rgb, alpha
@@ -444,15 +424,11 @@ class _HandFinish(Function):
         g_alpha = None if g_alpha is None else g_alpha.contiguous()
         g_ray = torch.empty_like(rayrgba)
         g_cw = g_cb = ws = None
-        L = _lib.lib()
+        L = _lib.kernels()
         if cal_w is not None:
             g_cw, g_cb = torch.empty(B, 3, device=dev), torch.empty(B, 3, device=dev)
             ws = torch.empty(L.gb_hand_finish_workspace_bytes(B, H, W) // 4, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(L.gb_hand_finish_bwd(
-                B, H, W, _lib.ptr(rayrgba), _lib.ptr(cal_w), _lib.ptr(grey), _lib.ptr(bg), _lib.ptr(g_rgb),
-                _lib.ptr(g_alpha), _lib.ptr(g_ray), _lib.ptr(g_cw), _lib.ptr(g_cb), _lib.ptr(ws),
-                _lib.stream_ptr(dev)), "hand_finish_bwd")
+        L.gb_hand_finish_bwd(B, H, W, rayrgba, cal_w, grey, bg, g_rgb, g_alpha, g_ray, g_cw, g_cb, ws)
         return g_ray, g_cw, g_cb, None, None
 
 

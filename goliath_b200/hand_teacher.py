@@ -91,10 +91,8 @@ class _OLATCompose(Function):
         B, L = intensity.shape[:2]
         rgb = prev if prev is not None else torch.empty(B, Z, 3, U, U, device=tex.device)
         texolat = torch.empty(B, L, Z, 3, U, U, device=tex.device) if want_texolat else None
-        with torch.cuda.device(tex.device):
-            _lib.check(_lib.lib().gb_olat_compose_fwd(
-                B, L, Z, U, _lib.ptr(tex), _lib.ptr(intensity), _lib.ptr(shadow_feat), _lib.ptr(rgb),
-                int(prev is not None), _lib.ptr(texolat), _lib.stream_ptr(tex.device)), "olat_compose_fwd")
+        _lib.kernels().gb_olat_compose_fwd(
+            B, L, Z, U, tex, intensity, shadow_feat, rgb, int(prev is not None), texolat)
         if prev is not None:
             ctx.mark_dirty(prev)
         ctx.save_for_backward(tex, intensity, shadow_feat)
@@ -111,10 +109,7 @@ class _OLATCompose(Function):
             g_rgb = torch.zeros(B, Z, 3, U, U, device=tex.device) if g_rgb is None else g_rgb.contiguous()
             g_texolat = None if g_texolat is None else g_texolat.contiguous()
             g_tex = torch.empty_like(tex)
-            with torch.cuda.device(tex.device):
-                _lib.check(_lib.lib().gb_olat_compose_bwd(
-                    B, L, Z, U, _lib.ptr(tex), _lib.ptr(intensity), _lib.ptr(shadow_feat), _lib.ptr(g_rgb),
-                    _lib.ptr(g_texolat), _lib.ptr(g_tex), _lib.stream_ptr(tex.device)), "olat_compose_bwd")
+            _lib.kernels().gb_olat_compose_bwd(B, L, Z, U, tex, intensity, shadow_feat, g_rgb, g_texolat, g_tex)
         return g_tex, None, None, g_rgb if has_prev else None, None, None
 
 
@@ -215,12 +210,9 @@ class OLATRGBDecoder(nn.Module):
         raypos, raydir, tminmax = compute_raydirs(lpos, lrot, focal, princpt, pix, self.volradius)
         TD, TH, TW = self.primsize[2], self.primsize[1], self.primsize[0]
         shadow = torch.zeros(B * L, K, TD, TH, TW, 2, device=pp.device)
-        with torch.cuda.device(pp.device):
-            _lib.check(_lib.lib().gb_mvp_shadow_march(
-                B * L, L, S0, S1, K, _lib.ptr(raypos), _lib.ptr(raydir), float(self.raymarcher.dt), _lib.ptr(tminmax),
-                _lib.ptr(nodeaabb), _lib.ptr(pp_n), _lib.ptr(pr), _lib.ptr(ps), TD, TH, TW, self.uv_size,
-                _lib.ptr(alpha), _lib.ptr(valid), _lib.ptr(shadow), 8.0, 8.0, 8, 16, _lib.stream_ptr(pp.device)),
-                "mvp_shadow_march")
+        _lib.kernels().gb_mvp_shadow_march(
+            B * L, L, S0, S1, K, raypos, raydir, float(self.raymarcher.dt), tminmax, nodeaabb, pp_n, pr, ps, TD, TH,
+            TW, self.uv_size, alpha, valid, shadow, 8.0, 8.0, 8, 16)
         return shadow
 
     def features(self, prims, campos, light_pos, shadow, primshadow=None, want_shadow_feat=False):
@@ -241,11 +233,9 @@ class OLATRGBDecoder(nn.Module):
         if primshadow is None:
             primshadow = torch.empty(B, TD, 3, U, U, device=pp.device)
         sf = torch.empty(B * L, TD, U, U, device=pp.device) if want_shadow_feat else None
-        with torch.cuda.device(pp.device):
-            _lib.check(_lib.lib().gb_olat_features(
-                B, L, K, TD, TH, TW, U, float(self.volradius), _lib.ptr(pp), _lib.ptr(pr), _lib.ptr(ps), _lib.ptr(valid),
-                _lib.ptr(lp), _lib.ptr(cp), _lib.ptr(shadow), _lib.ptr(feat), _lib.ptr(primshadow), int(accumulate),
-                _lib.ptr(sf), _lib.stream_ptr(pp.device)), "olat_features")
+        _lib.kernels().gb_olat_features(
+            B, L, K, TD, TH, TW, U, float(self.volradius), pp, pr, ps, valid, lp, cp, shadow, feat, primshadow,
+            int(accumulate), sf)
         return feat, primshadow, sf
 
     def unet(self, x, joint_feat, L):

@@ -107,10 +107,7 @@ class _Skin(Function):
         if verts.shape[2:] != (3,) or vb not in (1, B) or skin_idx.shape != (V, N_SLOTS):
             raise RuntimeError("verts_unposed must be [1 or B, V, 3] with V = the skinned mesh's vertex count")
         out = torch.empty(B, V, 3, device=verts.device)
-        with torch.cuda.device(verts.device):
-            _lib.check(_lib.lib().gb_lbs_skin_fwd(
-                B, V, J, vb, _lib.ptr(mats), _lib.ptr(verts), _lib.ptr(templ), _lib.ptr(skin_idx), _lib.ptr(skin_w),
-                _lib.ptr(gscale), _lib.ptr(out), _lib.stream_ptr(verts.device)), "lbs_skin_fwd")
+        _lib.kernels().gb_lbs_skin_fwd(B, V, J, vb, mats, verts, templ, skin_idx, skin_w, gscale, out)
         ctx.save_for_backward(mats, skin_idx, skin_w, gscale)
         ctx.vb = vb
         return out
@@ -122,10 +119,7 @@ class _Skin(Function):
         V = skin_idx.shape[0]
         g_out = g_out.contiguous()
         g_v = torch.empty(ctx.vb, V, 3, device=g_out.device)
-        with torch.cuda.device(g_out.device):
-            _lib.check(_lib.lib().gb_lbs_skin_bwd(
-                B, V, J, ctx.vb, _lib.ptr(mats), _lib.ptr(skin_idx), _lib.ptr(skin_w), _lib.ptr(gscale),
-                _lib.ptr(g_out), _lib.ptr(g_v), _lib.stream_ptr(g_out.device)), "lbs_skin_bwd")
+        _lib.kernels().gb_lbs_skin_bwd(B, V, J, ctx.vb, mats, skin_idx, skin_w, gscale, g_out, g_v)
         return g_v, None, None, None, None, None
 
 
@@ -252,13 +246,10 @@ class LinearBlendSkinning(nn.Module):
         stride = scales.stride(0) if scales.shape[0] == B else 0  # 0: one row for every item (lbs_scale.expand)
         mats = torch.empty(B, J, 3, 4, device=poses.device)
         states = torch.empty(B, J, 8, device=poses.device) if return_states else None
-        with torch.cuda.device(poses.device):
-            _lib.check(_lib.lib().gb_lbs_skeleton_fwd(
-                B, J, P, S, _lib.ptr(poses), _lib.ptr(scales), stride, _lib.ptr(tabs["transform"]),
-                _lib.ptr(tabs["offsets"]), _lib.ptr(tabs["joint_offset"]), _lib.ptr(tabs["joint_rotation"]),
-                _lib.ptr(tabs["parents"]), _lib.ptr(tabs["order"]), _lib.ptr(tabs["level_start"]), tabs["n_levels"],
-                _lib.ptr(tabs["bind"]), _lib.ptr(mats), _lib.ptr(states), _lib.stream_ptr(poses.device)),
-                "lbs_skeleton_fwd")
+        _lib.kernels().gb_lbs_skeleton_fwd(
+            B, J, P, S, poses, scales, stride, tabs["transform"], tabs["offsets"], tabs["joint_offset"],
+            tabs["joint_rotation"], tabs["parents"], tabs["order"], tabs["level_start"], tabs["n_levels"],
+            tabs["bind"], mats, states)
         return (mats, states) if return_states else mats
 
     def skin(self, mats, verts, template=None, global_scaling=None):
@@ -281,11 +272,8 @@ class LinearBlendSkinning(nn.Module):
         if verts.shape[2:] != (3,) or vb not in (1, B) or tabs["skin_idx"].shape != (V, N_SLOTS):
             raise RuntimeError("verts must be [1 or B, V, 3] with V = the skinned mesh's vertex count")
         out = torch.empty(B, V, 3, device=verts.device)
-        with torch.cuda.device(verts.device):
-            _lib.check(_lib.lib().gb_lbs_unskin_fwd(
-                B, V, J, vb, _lib.ptr(mats), _lib.ptr(verts), _lib.ptr(template), _lib.ptr(tabs["skin_idx"]),
-                _lib.ptr(tabs["skin_w"]), _lib.ptr(global_scaling), _lib.ptr(out), _lib.stream_ptr(verts.device)),
-                "lbs_unskin_fwd")
+        _lib.kernels().gb_lbs_unskin_fwd(
+            B, V, J, vb, mats, verts, template, tabs["skin_idx"], tabs["skin_w"], global_scaling, out)
         return out
 
     def unpose(self, poses: torch.Tensor, scales: torch.Tensor, verts: torch.Tensor):

@@ -123,11 +123,9 @@ class EnvSpinDecorator(th.nn.Module):
         light_intensity = th.empty(B, 512, 3, **f32)
         norm_scale = th.empty(B, **f32)
         angles = (ctypes.c_float * B)(*[2.0 * np.pi * float(index[i]) / self.cycle for i in range(B)])
-        with th.cuda.device(img.device):
-            _lib.check(_lib.lib().gb_envmap_spin_table(
-                B, He, We, angles, _lib.ptr(img), self.perc90, float(self.env_scale), _lib.ptr(lightrot),
-                _lib.ptr(envbg), _lib.ptr(hpass), _lib.ptr(envmap), _lib.ptr(light_intensity), _lib.ptr(norm_scale),
-                _lib.stream_ptr(img.device)), "envmap_spin_table")
+        _lib.kernels().gb_envmap_spin_table(
+            B, He, We, angles, img, self.perc90, float(self.env_scale), lightrot, envbg, hpass, envmap,
+            light_intensity, norm_scale)
         return lightrot, envbg, envmap, light_intensity, norm_scale
 
     def forward(self, **data):

@@ -56,8 +56,7 @@ class _MeshRender(Function):
         C, Ht, Wt = tex.shape[1:]
         H, W = layer.h, layer.w
         dev = v_pix.device
-        L = _lib.lib()
-        st = _lib.stream_ptr(dev)
+        L = _lib.kernels()
         index_img = torch.empty(B, H, W, device=dev, dtype=torch.int32)
         depth = torch.empty(B, H, W, device=dev)
         bary = torch.empty(B, 3, H, W, device=dev)
@@ -65,13 +64,9 @@ class _MeshRender(Function):
         mask = torch.empty(B, 1, H, W, device=dev)
         render = torch.empty(B, C, H, W, device=dev)
         ws = torch.empty(L.gb_mesh_raster_workspace_bytes(B, F, H, W), device=dev, dtype=torch.uint8)
-        with torch.cuda.device(dev):
-            _lib.check(L.gb_mesh_raster(B, V, F, H, W, _lib.ptr(v_pix), _lib.ptr(vi), _lib.ptr(index_img),
-                                        _lib.ptr(ws), st), "mesh_raster")
-            _lib.check(L.gb_mesh_render_fwd(B, V, F, H, W, C, Ht, Wt, _lib.ptr(v_pix), _lib.ptr(vi), _lib.ptr(vti),
-                                            _lib.ptr(vt), _lib.ptr(tex), _lib.ptr(index_img), _lib.ptr(depth),
-                                            _lib.ptr(bary), _lib.ptr(vt_img), _lib.ptr(mask), _lib.ptr(render), st),
-                       "mesh_render_fwd")
+        L.gb_mesh_raster(B, V, F, H, W, v_pix, vi, index_img, ws)
+        L.gb_mesh_render_fwd(B, V, F, H, W, C, Ht, Wt, v_pix, vi, vti, vt, tex, index_img, depth, bary, vt_img,
+                             mask, render)
         ctx.mark_non_differentiable(depth, bary, vt_img, index_img, mask)
         ctx.save_for_backward(v_pix, tex, index_img, vt_img, render)
         ctx.tables, ctx.edge_grad = (vi, vti, vt, inc), bool(edge_grad)
@@ -89,17 +84,14 @@ class _MeshRender(Function):
         g_render = g_render.contiguous()
         g_v = torch.empty_like(v_pix)
         g_tex = torch.empty_like(tex)
-        L = _lib.lib()
+        L = _lib.kernels()
         ws = torch.empty(L.gb_mesh_render_bwd_workspace_bytes(B, F, H, W, Ht, Wt), device=dev, dtype=torch.uint8)
         inc_ptr = inc.ptr
         if inc_ptr.numel() < V + 1:  # vertices no face uses: empty lists
             inc_ptr = torch.cat([inc_ptr, inc_ptr[-1:].expand(V + 1 - inc_ptr.numel())]).contiguous()
-        with torch.cuda.device(dev):
-            _lib.check(L.gb_mesh_render_bwd(
-                B, V, F, H, W, C, Ht, Wt, _lib.ptr(v_pix), _lib.ptr(vi), _lib.ptr(vti), _lib.ptr(vt), _lib.ptr(tex),
-                _lib.ptr(index_img), _lib.ptr(vt_img), _lib.ptr(render), _lib.ptr(g_render), int(ctx.edge_grad),
-                _lib.ptr(inc_ptr), _lib.ptr(inc.inc), _lib.ptr(g_v), _lib.ptr(g_tex), _lib.ptr(ws),
-                _lib.stream_ptr(dev)), "mesh_render_bwd")
+        L.gb_mesh_render_bwd(
+            B, V, F, H, W, C, Ht, Wt, v_pix, vi, vti, vt, tex, index_img, vt_img, render, g_render,
+            int(ctx.edge_grad), inc_ptr, inc.inc, g_v, g_tex, ws)
         return g_v, g_tex, None, None
 
 

@@ -43,14 +43,12 @@ class _ConvSlices(Function):
         if C2 != 2 * c or vb.shape != va.shape or va.shape[2:] != (3, 3):
             raise RuntimeError("the final convolutions need a [B, %d, H, W] map" % (2 * va.shape[1]))
         outs = []
-        with torch.cuda.device(x.device):
-            for i, (v, g, b) in enumerate(((va, ga, ba), (vb, gb, bb))):
-                out = torch.empty(B, Cout, H, W, device=x.device)
-                _lib.check(_lib.lib().gb_conv2d_wnub_fwd(
-                    B, c, Cout, H, W, 3, x.data_ptr() + 4 * i * c * H * W, C2 * H * W, _lib.ptr(v.contiguous()),
-                    _lib.ptr(_wn_scale(v, g)), _lib.ptr(b.contiguous()), 2, 1.0, 0, _lib.ptr(out),
-                    _lib.stream_ptr(x.device)), "conv2d_wnub_fwd")
-                outs.append(out)
+        for i, (v, g, b) in enumerate(((va, ga, ba), (vb, gb, bb))):
+            out = torch.empty(B, Cout, H, W, device=x.device)
+            _lib.kernels().gb_conv2d_wnub_fwd(
+                B, c, Cout, H, W, 3, x.data_ptr() + 4 * i * c * H * W, C2 * H * W, v.contiguous(), _wn_scale(v, g),
+                b.contiguous(), 2, 1.0, 0, out)
+            outs.append(out)
         ctx.save_for_backward(x, va, ga, vb, gb)
         return tuple(outs)
 
@@ -61,18 +59,16 @@ class _ConvSlices(Function):
         c, Cout = va.shape[1], va.shape[0]
         gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
         grads = []
-        L = _lib.lib()
+        L = _lib.kernels()
         ws = torch.empty(L.gb_conv2d_wnub_bwd_workspace_bytes(B, c, Cout, H, W, 3) // 4, device=x.device)
-        with torch.cuda.device(x.device):
-            for i, (v, g, go) in enumerate(((va, ga, g_a), (vb, gb, g_b))):
-                gbias = torch.empty(Cout, H, W, device=x.device)
-                gw = torch.empty_like(v)
-                _lib.check(L.gb_conv2d_wnub_bwd(
-                    B, c, Cout, H, W, 3, x.data_ptr() + 4 * i * c * H * W, C2 * H * W, _lib.ptr(v.contiguous()),
-                    _lib.ptr(_wn_scale(v, g)), None, _lib.ptr(go.contiguous()), 1.0, 0, 2, None, _lib.ptr(gbias),
-                    None if gx is None else gx.data_ptr() + 4 * i * c * H * W, _lib.ptr(gw), _lib.ptr(ws),
-                    _lib.stream_ptr(x.device)), "conv2d_wnub_bwd")
-                grads += list(_wn_chain(v, g, gw)) + [gbias]
+        for i, (v, g, go) in enumerate(((va, ga, g_a), (vb, gb, g_b))):
+            gbias = torch.empty(Cout, H, W, device=x.device)
+            gw = torch.empty_like(v)
+            L.gb_conv2d_wnub_bwd(
+                B, c, Cout, H, W, 3, x.data_ptr() + 4 * i * c * H * W, C2 * H * W, v.contiguous(), _wn_scale(v, g),
+                None, go.contiguous(), 1.0, 0, 2, None, gbias,
+                None if gx is None else gx.data_ptr() + 4 * i * c * H * W, gw, ws)
+            grads += list(_wn_chain(v, g, gw)) + [gbias]
         return (gx, *grads)
 
 
@@ -219,10 +215,7 @@ class _TexCompose(Function):
             raise RuntimeError("texture composite: shapes do not match T1 %s" % (tuple(t1.shape),))
         scale = _wn_scale(v, g)
         out = torch.empty(B, 3, 2 * H, 2 * W, device=t1.device)
-        with torch.cuda.device(t1.device):
-            _lib.check(_lib.lib().gb_body_tex_compose_fwd(
-                B, H, W, _lib.ptr(t1), _lib.ptr(h), _lib.ptr(v2), _lib.ptr(scale), _lib.ptr(bias), float(tex_std),
-                _lib.ptr(tex_mean), _lib.ptr(s3), _lib.ptr(out), _lib.stream_ptr(t1.device)), "body_tex_compose_fwd")
+        _lib.kernels().gb_body_tex_compose_fwd(B, H, W, t1, h, v2, scale, bias, float(tex_std), tex_mean, s3, out)
         ctx.save_for_backward(t1, h, v, g, bias, tex_mean, s3)
         ctx.tex_std = float(tex_std)
         return out
@@ -237,14 +230,11 @@ class _TexCompose(Function):
         g_t1, g_h, g_s3 = torch.empty_like(t1), torch.empty_like(h), torch.empty_like(s3)
         g_bias = torch.empty_like(bias)
         g_w = torch.zeros_like(v)
-        L = _lib.lib()
+        L = _lib.kernels()
         ws = torch.empty(L.gb_body_tex_compose_workspace_bytes(H, W) // 4, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(L.gb_body_tex_compose_bwd(
-                B, H, W, _lib.ptr(t1), _lib.ptr(h), _lib.ptr(v.reshape(v.shape[0], -1).contiguous()),
-                _lib.ptr(scale), _lib.ptr(bias), ctx.tex_std, _lib.ptr(tex_mean), _lib.ptr(s3), _lib.ptr(g_out),
-                _lib.ptr(g_t1), _lib.ptr(g_h), _lib.ptr(g_bias), _lib.ptr(g_w), _lib.ptr(g_s3), _lib.ptr(ws),
-                _lib.stream_ptr(dev)), "body_tex_compose_bwd")
+        L.gb_body_tex_compose_bwd(
+            B, H, W, t1, h, v.reshape(v.shape[0], -1).contiguous(), scale, bias, ctx.tex_std, tex_mean, s3, g_out,
+            g_t1, g_h, g_bias, g_w, g_s3, ws)
         gv, gg = _wn_chain(v, g, g_w)
         return g_t1, g_h, gv, gg, g_bias, None, g_s3, None
 
@@ -392,9 +382,7 @@ class _PixelBias(Function):
                                % (tuple(bias.shape), tuple(idx.shape)))
         out = torch.empty_like(rgb)
         n, _, Hb, Wb = bias.shape
-        with torch.cuda.device(rgb.device):
-            _lib.check(_lib.lib().gb_pixel_bias_fwd(B, C, H, W, n, Hb, Wb, _lib.ptr(rgb), _lib.ptr(bias), _lib.ptr(idx),
-                                                    _lib.ptr(out), _lib.stream_ptr(rgb.device)), "pixel_bias_fwd")
+        _lib.kernels().gb_pixel_bias_fwd(B, C, H, W, n, Hb, Wb, rgb, bias, idx, out)
         ctx.save_for_backward(idx)
         ctx.shapes = (tuple(rgb.shape), tuple(bias.shape))
         return out
@@ -407,10 +395,7 @@ class _PixelBias(Function):
         if ctx.needs_input_grad[1]:
             g_out = g_out.contiguous()
             g_bias = torch.empty(n, 1, Hb, Wb, device=g_out.device)
-            with torch.cuda.device(g_out.device):
-                _lib.check(_lib.lib().gb_pixel_bias_bwd(B, C, H, W, n, Hb, Wb, _lib.ptr(idx), _lib.ptr(g_out),
-                                                        _lib.ptr(g_bias), _lib.stream_ptr(g_out.device)),
-                           "pixel_bias_bwd")
+            _lib.kernels().gb_pixel_bias_bwd(B, C, H, W, n, Hb, Wb, idx, g_out, g_bias)
         return g_out if ctx.needs_input_grad[0] else None, g_bias, None
 
 

@@ -58,10 +58,7 @@ def face_tex_cond(face_tex, mask):
     if mask.numel() != H * W:
         raise RuntimeError("tex_cond_mask must hold one [H, W] plane")
     out = torch.empty(B, C, H, W, device=face_tex.device)
-    with torch.cuda.device(face_tex.device):
-        _lib.check(_lib.lib().gb_face_tex_cond_fwd(B, C, Hs, Ws, H, W, _lib.ptr(face_tex), _lib.ptr(mask),
-                                                   _lib.ptr(out), _lib.stream_ptr(face_tex.device)),
-                   "face_tex_cond_fwd")
+    _lib.kernels().gb_face_tex_cond_fwd(B, C, Hs, Ws, H, W, face_tex, mask, out)
     return out
 
 

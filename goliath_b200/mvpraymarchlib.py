@@ -58,12 +58,9 @@ def compute_aabb(primpos, primrot, primscale, sortedobjid, nodechildren, nodepar
         _chk(t, n, torch.int32)
     N, K = primpos.size(0), primpos.size(1)
     dev = primpos.device
-    L = _lib.lib()
+    L = _lib.kernels()
     ws = _workspace(dev, L.gb_mvp_aabb_workspace_bytes(N, K))
-    with torch.cuda.device(dev):
-        _lib.check(L.gb_mvp_compute_aabb(N, K, _lib.ptr(primpos), _lib.ptr(primrot), _lib.ptr(primscale),
-                                         _lib.ptr(sortedobjid), _lib.ptr(nodechildren), _lib.ptr(nodeparent),
-                                         _lib.ptr(nodeaabb), _lib.ptr(ws), _lib.stream_ptr(dev)), "compute_aabb")
+    L.gb_mvp_compute_aabb(N, K, primpos, primrot, primscale, sortedobjid, nodechildren, nodeparent, nodeaabb, ws)
     return []
 
 
@@ -90,13 +87,10 @@ def raymarch_forward(rayposim, raydirim, stepsize, tminmaxim, sortedobjid, nodec
         raise RuntimeError("usebvh=False / missing primitive transform is not a functional path of the reference")
     N, H, W, K, TD, TH, TW, WD, WH, WW = _dims(rayposim, primposim, tplateim, warpim, chlast)
     algo = int(algorithm)
-    dev = rayposim.device
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().gb_mvp_raymarch_fwd(
-            N, H, W, K, _lib.ptr(rayposim), _lib.ptr(raydirim), float(stepsize), _lib.ptr(tminmaxim), _lib.ptr(nodeaabb),
-            _lib.ptr(primposim), _lib.ptr(primrotim), _lib.ptr(primscaleim), TD, TH, TW, _lib.ptr(tplateim), WD, WH, WW,
-            _lib.ptr(warpim) if algo == 1 else None, _lib.ptr(rayrgbaim), _lib.ptr(raysatim), _lib.ptr(shadow), algo,
-            float(fadescale), float(fadeexp), int(blocksizex), int(blocksizey), _lib.stream_ptr(dev)), "raymarch_forward")
+    _lib.kernels().gb_mvp_raymarch_fwd(
+        N, H, W, K, rayposim, raydirim, float(stepsize), tminmaxim, nodeaabb, primposim, primrotim, primscaleim, TD,
+        TH, TW, tplateim, WD, WH, WW, warpim if algo == 1 else None, rayrgbaim, raysatim, shadow, algo,
+        float(fadescale), float(fadeexp), int(blocksizex), int(blocksizey))
     return []
 
 
@@ -113,13 +107,9 @@ def raymarch_backward(rayposim, raydirim, stepsize, tminmaxim, sortedobjid, node
         _chk(t, n)
     N, H, W, K, TD, TH, TW, WD, WH, WW = _dims(rayposim, primposim, tplateim, warpim, chlast)
     algo = int(algorithm)
-    dev = rayposim.device
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().gb_mvp_raymarch_bwd(
-            N, H, W, K, _lib.ptr(rayposim), _lib.ptr(raydirim), float(stepsize), _lib.ptr(tminmaxim), _lib.ptr(nodeaabb),
-            _lib.ptr(primposim), _lib.ptr(primrotim), _lib.ptr(primscaleim), TD, TH, TW, _lib.ptr(tplateim), WD, WH, WW,
-            _lib.ptr(warpim) if algo == 1 else None, _lib.ptr(raysatim), _lib.ptr(grad_rayrgba), _lib.ptr(grad_primposim),
-            _lib.ptr(grad_primrotim), _lib.ptr(grad_primscaleim), _lib.ptr(grad_tplateim),
-            _lib.ptr(grad_warpim) if algo == 1 else None, algo, float(fadescale), float(fadeexp), int(blocksizex),
-            int(blocksizey), _lib.stream_ptr(dev)), "raymarch_backward")
+    _lib.kernels().gb_mvp_raymarch_bwd(
+        N, H, W, K, rayposim, raydirim, float(stepsize), tminmaxim, nodeaabb, primposim, primrotim, primscaleim, TD,
+        TH, TW, tplateim, WD, WH, WW, warpim if algo == 1 else None, raysatim, grad_rayrgba, grad_primposim,
+        grad_primrotim, grad_primscaleim, grad_tplateim, grad_warpim if algo == 1 else None, algo, float(fadescale),
+        float(fadeexp), int(blocksizex), int(blocksizey))
     return []

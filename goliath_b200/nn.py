@@ -38,11 +38,9 @@ class _Deconv4x4s2WNUB(Function):
         if b is not None and b.shape != (Cout, 2 * Hi, 2 * Wi):
             raise RuntimeError("untied bias must be [Cout, 2*Hi, 2*Wi]")
         out = torch.empty(B, Cout, 2 * Hi, 2 * Wi, device=x.device, dtype=torch.float32)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().gb_deconv4x4s2_wnub_fwd(
-                B, Cin, Cout, Hi, Wi, _lib.ptr(x), _lib.ptr(weight_v), _lib.ptr(scale), _lib.ptr(b),
-                float(slope if slope is not None else 1.0), int(slope is not None), _lib.ptr(out),
-                _lib.stream_ptr(x.device)), "deconv4x4s2_wnub_fwd")
+        _lib.kernels().gb_deconv4x4s2_wnub_fwd(
+            B, Cin, Cout, Hi, Wi, x, weight_v, scale, b, float(slope if slope is not None else 1.0),
+            int(slope is not None), out)
         ctx.save_for_backward(x, weight_v, weight_g, out)
         ctx.slope = slope
         ctx.has_bias = bias is not None
@@ -64,13 +62,11 @@ class _Deconv4x4s2WNUB(Function):
             gb = torch.empty(Cout, 2 * Hi, 2 * Wi, device=dev, dtype=torch.float32)
         gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
         gw = torch.empty_like(v)
-        L = _lib.lib()
+        L = _lib.kernels()
         ws = torch.empty(L.gb_deconv4x4s2_wnub_bwd_workspace_bytes(B, Cin, Cout, Hi, Wi) // 4, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(L.gb_deconv4x4s2_wnub_bwd(
-                B, Cin, Cout, Hi, Wi, _lib.ptr(x), _lib.ptr(v), _lib.ptr(_wn_scale(v, g)), _lib.ptr(out), _lib.ptr(gout),
-                float(ctx.slope if ctx.slope is not None else 1.0), int(ctx.slope is not None), _lib.ptr(gz), _lib.ptr(gb),
-                _lib.ptr(gx), _lib.ptr(gw), _lib.ptr(ws), _lib.stream_ptr(dev)), "deconv4x4s2_wnub_bwd")
+        L.gb_deconv4x4s2_wnub_bwd(
+            B, Cin, Cout, Hi, Wi, x, v, _wn_scale(v, g), out, gout,
+            float(ctx.slope if ctx.slope is not None else 1.0), int(ctx.slope is not None), gz, gb, gx, gw, ws)
         if alias_bias:
             gb = gz.view(Cout, 2 * Hi, 2 * Wi)
         return (gx, *_wn_chain(v, g, gw), gb, None)
@@ -125,11 +121,9 @@ class _ConvS1WN(Function):
             else:
                 raise RuntimeError("bias must be [Cout] or [Cout, H, W]")
         out = torch.empty(B, Cout, H, W, device=x.device, dtype=torch.float32)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().gb_conv2d_wnub_fwd(
-                B, Cin, Cout, H, W, K, _lib.ptr(x), Cin * H * W, _lib.ptr(weight_v),
-                _lib.ptr(_wn_scale(weight_v, weight_g)), _lib.ptr(b), mode, float(slope if slope is not None else 1.0),
-                int(slope is not None), _lib.ptr(out), _lib.stream_ptr(x.device)), "conv2d_wnub_fwd")
+        _lib.kernels().gb_conv2d_wnub_fwd(
+            B, Cin, Cout, H, W, K, x, Cin * H * W, weight_v, _wn_scale(weight_v, weight_g), b, mode,
+            float(slope if slope is not None else 1.0), int(slope is not None), out)
         ctx.save_for_backward(x, weight_v, weight_g, out)
         ctx.slope, ctx.mode = slope, mode
         return out
@@ -149,14 +143,12 @@ class _ConvS1WN(Function):
             gb = torch.empty(Cout, H, W, device=dev, dtype=torch.float32)
         gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
         gw = torch.empty_like(v)
-        L = _lib.lib()
+        L = _lib.kernels()
         ws = torch.empty(L.gb_conv2d_wnub_bwd_workspace_bytes(B, Cin, Cout, H, W, K) // 4, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(L.gb_conv2d_wnub_bwd(
-                B, Cin, Cout, H, W, K, _lib.ptr(x), Cin * H * W, _lib.ptr(v), _lib.ptr(_wn_scale(v, g)), _lib.ptr(out),
-                _lib.ptr(gout), float(ctx.slope if ctx.slope is not None else 1.0), int(ctx.slope is not None),
-                ctx.mode, _lib.ptr(gz), _lib.ptr(gb), _lib.ptr(gx), _lib.ptr(gw), _lib.ptr(ws), _lib.stream_ptr(dev)),
-                "conv2d_wnub_bwd")
+        L.gb_conv2d_wnub_bwd(
+            B, Cin, Cout, H, W, K, x, Cin * H * W, v, _wn_scale(v, g), out, gout,
+            float(ctx.slope if ctx.slope is not None else 1.0), int(ctx.slope is not None), ctx.mode, gz, gb, gx,
+            gw, ws)
         return (gx, *_wn_chain(v, g, gw), gb, None)
 
 
@@ -180,11 +172,9 @@ class _Conv4x4s2WN(Function):
             raise RuntimeError("untied bias must be [Cout, H/2, W/2]")
         scale = _wn_scale(weight_v, weight_g)
         out = torch.empty(B, Cout, Ho, Wo, device=x.device, dtype=torch.float32)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().gb_conv4x4s2_wnub_fwd(
-                B, Cin, Cout, Ho, Wo, _lib.ptr(x), _lib.ptr(weight_v), _lib.ptr(scale), _lib.ptr(b),
-                float(slope if slope is not None else 1.0), int(slope is not None), _lib.ptr(out),
-                _lib.stream_ptr(x.device)), "conv4x4s2_wnub_fwd")
+        _lib.kernels().gb_conv4x4s2_wnub_fwd(
+            B, Cin, Cout, Ho, Wo, x, weight_v, scale, b, float(slope if slope is not None else 1.0),
+            int(slope is not None), out)
         ctx.save_for_backward(x, weight_v, weight_g, out)
         ctx.slope = slope
         ctx.has_bias = bias is not None
@@ -206,13 +196,11 @@ class _Conv4x4s2WN(Function):
             gb = torch.empty(Cout, Ho, Wo, device=dev, dtype=torch.float32)
         gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
         gw = torch.empty_like(v)
-        L = _lib.lib()
+        L = _lib.kernels()
         ws = torch.empty(L.gb_conv4x4s2_wnub_bwd_workspace_bytes(B, Cin, Cout, Ho, Wo) // 4, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(L.gb_conv4x4s2_wnub_bwd(
-                B, Cin, Cout, Ho, Wo, _lib.ptr(x), _lib.ptr(v), _lib.ptr(_wn_scale(v, g)), _lib.ptr(out), _lib.ptr(gout),
-                float(ctx.slope if ctx.slope is not None else 1.0), int(ctx.slope is not None), _lib.ptr(gz), _lib.ptr(gb),
-                _lib.ptr(gx), _lib.ptr(gw), _lib.ptr(ws), _lib.stream_ptr(dev)), "conv4x4s2_wnub_bwd")
+        L.gb_conv4x4s2_wnub_bwd(
+            B, Cin, Cout, Ho, Wo, x, v, _wn_scale(v, g), out, gout,
+            float(ctx.slope if ctx.slope is not None else 1.0), int(ctx.slope is not None), gz, gb, gx, gw, ws)
         if alias_bias:
             gb = gz.view(Cout, Ho, Wo)
         return (gx, *_wn_chain(v, g, gw), gb, None)
@@ -332,62 +320,57 @@ def tower_forward_tc(tower: nn.Sequential, x: torch.Tensor) -> torch.Tensor:
     with Cout > 256 would fall back to the SIMT kernel.
     No autograd: use the module's normal forward for training."""
     assert not torch.is_grad_enabled(), "tower_forward_tc is the inference path"
-    L = _lib.lib()
+    L = _lib.kernels()
     dev = x.device
     layers = [m for m in tower if isinstance(m, ConvTranspose2dWNUB)]
     cur_nchw, cur_hi, cur_lo, cur_c = x.contiguous(), None, None, x.shape[1]
     B, _, H, W = x.shape
-    with torch.cuda.device(dev):
-        st = _lib.stream_ptr(dev)
-        for i, layer in enumerate(layers):
-            Cin, Cout = layer.in_channels, layer.out_channels
-            # with Cin = 16 the layer is pure output/bias bandwidth and the per-pixel NCHW epilogue of the tensor-core
-            # kernel loses to the SIMT kernel (bench.py decoder object, 16 -> 125 @ 1024^2 on an H100 SXM at 400 W:
-            # 0.92 ms SIMT, 1.05 ms tensor cores), so it stays SIMT
-            tc_ok = _tc_layer_ok(Cin, Cout)
-            nxt = layers[i + 1] if i + 1 < len(layers) else None
-            nxt_tc = nxt is not None and _tc_layer_ok(nxt.in_channels, nxt.out_channels)
-            bias = None if layer.bias is None else layer.bias.contiguous()
-            slope = layer.fused_slope
-            # frozen-parameter cache: weight-norm scale and the prepared tensor-core weight matrices are functions of
-            # (weight_v, weight_g) only; they are rebuilt when either tensor is modified in place or replaced
-            key = (layer.weight_v.data_ptr(), layer.weight_v._version, layer.weight_g.data_ptr(), layer.weight_g._version)
-            cache = getattr(layer, "_tc_cache", None)
-            fresh = cache is None or cache[0] != key
-            if fresh:
-                scale = _wn_scale(layer.weight_v, layer.weight_g)
-                ws = torch.empty(L.gb_deconv_tc_weight_bytes(_pad32(Cin), Cout) // 4, device=dev) if tc_ok else None
-                layer._tc_cache = (key, scale, ws)
-            else:
-                _, scale, ws = cache
-            if tc_ok:
-                cpad = _pad32(Cin)
-                if cur_hi is None:  # enter the NHWC hi/lo format
-                    cur_hi = torch.empty(B, H, W, cpad, device=dev)
-                    cur_lo = torch.empty(B, H, W, cpad, device=dev)
-                    _lib.check(L.gb_nchw_to_nhwc_split(B, Cin, cpad, H, W, _lib.ptr(cur_nchw), _lib.ptr(cur_hi),
-                                                       _lib.ptr(cur_lo), st), "nchw_to_nhwc_split")
-                    cur_c = cpad
-                assert cur_c == cpad, "channel padding mismatch between consecutive tensor-core layers"
-                ldc = _pad32(Cout)
-                # padded output channels must be zero for the next layer's K loop
-                o_hi = (torch.zeros if ldc != Cout else torch.empty)(B, 2 * H, 2 * W, ldc, device=dev) if nxt_tc else None
-                o_lo = (torch.zeros if ldc != Cout else torch.empty)(B, 2 * H, 2 * W, ldc, device=dev) if nxt_tc else None
-                o_nchw = None if nxt_tc else torch.empty(B, Cout, 2 * H, 2 * W, device=dev)
-                _lib.check(L.gb_deconv4x4s2_tc_fwd(
-                    B, Cin, cpad, Cout, H, W, _lib.ptr(cur_hi), _lib.ptr(cur_lo),
-                    _lib.ptr(layer.weight_v.contiguous()) if fresh else None, _lib.ptr(ws), _lib.ptr(scale), _lib.ptr(bias), float(slope if slope is not None else 1.0),
-                    int(slope is not None), _lib.ptr(o_hi), _lib.ptr(o_lo), ldc, _lib.ptr(o_nchw), st), "deconv4x4s2_tc_fwd")
-                cur_hi, cur_lo, cur_c, cur_nchw = o_hi, o_lo, ldc, o_nchw
-            else:
-                assert cur_nchw is not None
-                out = torch.empty(B, Cout, 2 * H, 2 * W, device=dev)
-                _lib.check(L.gb_deconv4x4s2_wnub_fwd(
-                    B, Cin, Cout, H, W, _lib.ptr(cur_nchw), _lib.ptr(layer.weight_v.contiguous()), _lib.ptr(scale),
-                    _lib.ptr(bias), float(slope if slope is not None else 1.0), int(slope is not None), _lib.ptr(out), st),
-                    "deconv4x4s2_wnub_fwd")
-                cur_nchw, cur_hi, cur_lo = out, None, None
-            H, W = 2 * H, 2 * W
+    for i, layer in enumerate(layers):
+        Cin, Cout = layer.in_channels, layer.out_channels
+        # with Cin = 16 the layer is pure output/bias bandwidth and the per-pixel NCHW epilogue of the tensor-core
+        # kernel loses to the SIMT kernel (bench.py decoder object, 16 -> 125 @ 1024^2 on an H100 SXM at 400 W:
+        # 0.92 ms SIMT, 1.05 ms tensor cores), so it stays SIMT
+        tc_ok = _tc_layer_ok(Cin, Cout)
+        nxt = layers[i + 1] if i + 1 < len(layers) else None
+        nxt_tc = nxt is not None and _tc_layer_ok(nxt.in_channels, nxt.out_channels)
+        bias = None if layer.bias is None else layer.bias.contiguous()
+        slope = layer.fused_slope
+        # frozen-parameter cache: weight-norm scale and the prepared tensor-core weight matrices are functions of
+        # (weight_v, weight_g) only; they are rebuilt when either tensor is modified in place or replaced
+        key = (layer.weight_v.data_ptr(), layer.weight_v._version, layer.weight_g.data_ptr(), layer.weight_g._version)
+        cache = getattr(layer, "_tc_cache", None)
+        fresh = cache is None or cache[0] != key
+        if fresh:
+            scale = _wn_scale(layer.weight_v, layer.weight_g)
+            ws = torch.empty(L.gb_deconv_tc_weight_bytes(_pad32(Cin), Cout) // 4, device=dev) if tc_ok else None
+            layer._tc_cache = (key, scale, ws)
+        else:
+            _, scale, ws = cache
+        if tc_ok:
+            cpad = _pad32(Cin)
+            if cur_hi is None:  # enter the NHWC hi/lo format
+                cur_hi = torch.empty(B, H, W, cpad, device=dev)
+                cur_lo = torch.empty(B, H, W, cpad, device=dev)
+                L.gb_nchw_to_nhwc_split(B, Cin, cpad, H, W, cur_nchw, cur_hi, cur_lo)
+                cur_c = cpad
+            assert cur_c == cpad, "channel padding mismatch between consecutive tensor-core layers"
+            ldc = _pad32(Cout)
+            # padded output channels must be zero for the next layer's K loop
+            o_hi = (torch.zeros if ldc != Cout else torch.empty)(B, 2 * H, 2 * W, ldc, device=dev) if nxt_tc else None
+            o_lo = (torch.zeros if ldc != Cout else torch.empty)(B, 2 * H, 2 * W, ldc, device=dev) if nxt_tc else None
+            o_nchw = None if nxt_tc else torch.empty(B, Cout, 2 * H, 2 * W, device=dev)
+            L.gb_deconv4x4s2_tc_fwd(
+                B, Cin, cpad, Cout, H, W, cur_hi, cur_lo, layer.weight_v.contiguous() if fresh else None, ws, scale,
+                bias, float(slope if slope is not None else 1.0), int(slope is not None), o_hi, o_lo, ldc, o_nchw)
+            cur_hi, cur_lo, cur_c, cur_nchw = o_hi, o_lo, ldc, o_nchw
+        else:
+            assert cur_nchw is not None
+            out = torch.empty(B, Cout, 2 * H, 2 * W, device=dev)
+            L.gb_deconv4x4s2_wnub_fwd(
+                B, Cin, Cout, H, W, cur_nchw, layer.weight_v.contiguous(), scale, bias,
+                float(slope if slope is not None else 1.0), int(slope is not None), out)
+            cur_nchw, cur_hi, cur_lo = out, None, None
+        H, W = 2 * H, 2 * W
     assert cur_nchw is not None, "a tower must end with a layer that produces NCHW output"
     return cur_nchw
 
@@ -478,11 +461,8 @@ class _UpConvBlock(Function):
         out = torch.empty(B, Cout, H, W, device=dev)
         train = any(ctx.needs_input_grad)
         mask = torch.empty(B, Cout, H, W, device=dev, dtype=torch.uint8) if train else None
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_upconv_block_fwd(
-                B, Cin, Cout, groups, Hi, Wi, _lib.ptr(x), _lib.ptr(v1), _lib.ptr(s1), _lib.ptr(b1), _lib.ptr(v2),
-                _lib.ptr(s2), _lib.ptr(b2), _lib.ptr(vr), _lib.ptr(sr), _lib.ptr(br), float(slope), _lib.ptr(h1),
-                _lib.ptr(out), _lib.ptr(mask), _lib.stream_ptr(dev)), "upconv_block_fwd")
+        _lib.kernels().gb_upconv_block_fwd(
+            B, Cin, Cout, groups, Hi, Wi, x, v1, s1, b1, v2, s2, b2, vr, sr, br, float(slope), h1, out, mask)
         if train:
             ctx.save_for_backward(x, v1, g1, v2, g2, vr, gr, h1, mask)
         ctx.slope, ctx.groups = float(slope), groups
@@ -506,14 +486,11 @@ class _UpConvBlock(Function):
         gb2 = torch.empty(Cout, H, W, device=dev)
         gbr = torch.empty(Cout, device=dev)
         gw1, gw2, gwr = torch.empty_like(v1), torch.empty_like(v2), torch.empty_like(vr)
-        L = _lib.lib()
+        L = _lib.kernels()
         ws = torch.empty(L.gb_upconv_block_bwd_workspace_bytes(B, Cin, Cout, ctx.groups, Hi, Wi) // 4, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(L.gb_upconv_block_bwd(
-                B, Cin, Cout, ctx.groups, Hi, Wi, _lib.ptr(x), _lib.ptr(v1), _lib.ptr(s1), _lib.ptr(v2), _lib.ptr(s2),
-                _lib.ptr(vr), _lib.ptr(sr), _lib.ptr(h1), _lib.ptr(mask), _lib.ptr(gout), ctx.slope, _lib.ptr(gz2),
-                _lib.ptr(gz1), _lib.ptr(gu), _lib.ptr(gb1), _lib.ptr(gb2), _lib.ptr(gbr), _lib.ptr(gw1), _lib.ptr(gw2),
-                _lib.ptr(gwr), _lib.ptr(gx), _lib.ptr(ws), _lib.stream_ptr(dev)), "upconv_block_bwd")
+        L.gb_upconv_block_bwd(
+            B, Cin, Cout, ctx.groups, Hi, Wi, x, v1, s1, v2, s2, vr, sr, h1, mask, gout, ctx.slope, gz2, gz1, gu,
+            gb1, gb2, gbr, gw1, gw2, gwr, gx, ws)
         gv1, gg1 = _wn_chain(v1, g1, gw1)
         gv2, gg2 = _wn_chain(v2, g2, gw2)
         gvr, ggr = _wn_chain(vr, gr, gwr)
@@ -594,11 +571,9 @@ class _DownConvBlock(Function):
         ctx.xargs = (B, Cin, Cout, groups, H, W)
         ctx.cond = (x.stride(0), x.stride(1), x.stride(2), Hs, Ws)
         ctx.cond_scale = float(cond_scale)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_downconv_block_fwd(
-                *ctx.xargs, _lib.ptr(x), *ctx.cond, _lib.ptr(cond_mask), ctx.cond_scale, _lib.ptr(v1), _lib.ptr(s1),
-                _lib.ptr(b1), _lib.ptr(v2), _lib.ptr(s2), _lib.ptr(b2), _lib.ptr(vr), _lib.ptr(sr), _lib.ptr(br),
-                float(slope), _lib.ptr(h1), _lib.ptr(out), _lib.ptr(mask), _lib.stream_ptr(dev)), "downconv_block_fwd")
+        _lib.kernels().gb_downconv_block_fwd(
+            *ctx.xargs, x, *ctx.cond, cond_mask, ctx.cond_scale, v1, s1, b1, v2, s2, b2, vr, sr, br, float(slope),
+            h1, out, mask)
         if train:
             ctx.save_for_backward(x, v1, g1, v2, g2, vr, gr, h1, mask, cond_mask)
         ctx.slope = float(slope)
@@ -614,7 +589,7 @@ class _DownConvBlock(Function):
         need_gx = ctx.needs_input_grad[0]
         if need_gx and cond_mask is not None:
             raise RuntimeError("ConvDownBlock: the fused resize + mask of the input has no backward")
-        L = _lib.lib()
+        L = _lib.kernels()
         gz2 = torch.empty(B, Cout, H // 2, W // 2, device=dev)
         gz1 = torch.empty(B, Cin, H, W, device=dev)
         gx = torch.empty(B, Cin, H, W, device=dev) if need_gx else None
@@ -623,12 +598,9 @@ class _DownConvBlock(Function):
         gbr = torch.empty(Cout, device=dev)
         gw1, gw2, gwr = torch.empty_like(v1), torch.empty_like(v2), torch.empty_like(vr)
         ws = torch.empty(L.gb_downconv_block_bwd_workspace_bytes(*ctx.xargs) // 4, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(L.gb_downconv_block_bwd(
-                *ctx.xargs, _lib.ptr(x), *ctx.cond, _lib.ptr(cond_mask), ctx.cond_scale, _lib.ptr(v1), _lib.ptr(s1),
-                _lib.ptr(v2), _lib.ptr(s2), _lib.ptr(vr), _lib.ptr(sr), _lib.ptr(h1), _lib.ptr(mask), _lib.ptr(gout),
-                ctx.slope, _lib.ptr(gz2), _lib.ptr(gz1), _lib.ptr(gb1), _lib.ptr(gb2), _lib.ptr(gbr), _lib.ptr(gw1),
-                _lib.ptr(gw2), _lib.ptr(gwr), _lib.ptr(gx), _lib.ptr(ws), _lib.stream_ptr(dev)), "downconv_block_bwd")
+        L.gb_downconv_block_bwd(
+            *ctx.xargs, x, *ctx.cond, cond_mask, ctx.cond_scale, v1, s1, v2, s2, vr, sr, h1, mask, gout, ctx.slope,
+            gz2, gz1, gb1, gb2, gbr, gw1, gw2, gwr, gx, ws)
         gv1, gg1 = _wn_chain(v1, g1, gw1)
         gv2, gg2 = _wn_chain(v2, g2, gw2)
         gvr, ggr = _wn_chain(vr, gr, gwr)

@@ -37,7 +37,7 @@ class FusedAdam(torch.optim.Optimizer):
 
     # ---- device table of {p, g, m, v, numel, lr, wd} rows + chunk map, rebuilt when a pointer or a rate changes
     def _build(self):
-        L = _lib.lib()
+        L = _lib.kernels()
         chunk = L.gb_optim_chunk_elems()
         assert L.gb_optim_row_bytes() == 56
         rows, chunks, key = [], [], []
@@ -84,7 +84,7 @@ class FusedAdam(torch.optim.Optimizer):
         dev = self._build()
         if dev is None or self._n_chunks == 0:
             return loss
-        L = _lib.lib()
+        L = _lib.kernels()
         self._steps += 1
         for group in self.param_groups:
             for p in group["params"]:
@@ -92,17 +92,13 @@ class FusedAdam(torch.optim.Optimizer):
                     self.state[p]["step"] += 1
         b1, b2 = self.param_groups[0]["betas"]
         t = self._steps
-        with torch.cuda.device(dev):
-            stream = _lib.stream_ptr(dev)
-            clip = self.max_grad_norm is not None and self.max_grad_norm > 0
-            if self.sanitize or clip:
-                self._sqnorm.zero_()
-                _lib.check(L.gb_grad_sanitize_sqnorm(_lib.ptr(self._table), _lib.ptr(self._chunks), self._n_chunks,
-                                                     _lib.ptr(self._sqnorm), stream), "grad_sanitize_sqnorm")
-            _lib.check(L.gb_adam_step(_lib.ptr(self._table), _lib.ptr(self._chunks), self._n_chunks,
-                                      _lib.ptr(self._sqnorm) if clip else None, float(self.max_grad_norm or 0.0), float(b1), float(b2),
-                                      float(self.param_groups[0]["eps"]), int(t), int(self.adamw),
-                                      int(self.write_clipped_grads), stream), "adam_step")
+        clip = self.max_grad_norm is not None and self.max_grad_norm > 0
+        if self.sanitize or clip:
+            self._sqnorm.zero_()
+            L.gb_grad_sanitize_sqnorm(self._table, self._chunks, self._n_chunks, self._sqnorm)
+        L.gb_adam_step(self._table, self._chunks, self._n_chunks, self._sqnorm if clip else None,
+                       float(self.max_grad_norm or 0.0), float(b1), float(b2), float(self.param_groups[0]["eps"]),
+                       int(t), int(self.adamw), int(self.write_clipped_grads))
         return loss
 
     def grad_norm(self) -> torch.Tensor:

@@ -39,11 +39,9 @@ class _PostRender(Function):
         if opt["background"] is not None and opt["alpha"] is None:
             raise RuntimeError("post_render: the background composite needs alpha")
         pred = torch.empty_like(rgb)
-        with torch.cuda.device(rgb.device):
-            _lib.check(_lib.lib().gb_post_render_fwd(
-                B, H, W, _lib.ptr(rgb), _lib.ptr(opt["alpha"]), _lib.ptr(opt["background"]), _lib.ptr(opt["cal_w"]),
-                _lib.ptr(opt["cal_b"]), _lib.ptr(opt["grey"]), _lib.ptr(opt["blur_w"]), _lib.ptr(pred),
-                _lib.stream_ptr(rgb.device)), "post_render_fwd")
+        _lib.kernels().gb_post_render_fwd(
+            B, H, W, rgb, opt["alpha"], opt["background"], opt["cal_w"], opt["cal_b"], opt["grey"], opt["blur_w"],
+            pred)
         ctx.save_for_backward(rgb, *[opt[k] for k in ("alpha", "background", "cal_w", "cal_b", "grey", "blur_w")])
         return pred
 
@@ -55,11 +53,8 @@ class _PostRender(Function):
         g_rgb = torch.empty_like(rgb)
         z = lambda t: None if t is None else torch.zeros_like(t)
         g_cw, g_cb, g_bw = z(cal_w), z(cal_b), z(blur_w)
-        with torch.cuda.device(rgb.device):
-            _lib.check(_lib.lib().gb_post_render_bwd(
-                B, H, W, _lib.ptr(rgb), _lib.ptr(alpha), _lib.ptr(background), _lib.ptr(cal_w), _lib.ptr(cal_b), _lib.ptr(grey),
-                _lib.ptr(blur_w), _lib.ptr(g_pred), _lib.ptr(g_rgb), _lib.ptr(g_cw), _lib.ptr(g_cb), _lib.ptr(g_bw),
-                _lib.stream_ptr(rgb.device)), "post_render_bwd")
+        _lib.kernels().gb_post_render_bwd(
+            B, H, W, rgb, alpha, background, cal_w, cal_b, grey, blur_w, g_pred, g_rgb, g_cw, g_cb, g_bw)
         return g_rgb, None, None, g_cw, g_cb, None, g_bw
 
 
@@ -86,10 +81,7 @@ class _SsimL1(Function):
         dev = pred.device
         d_mu, d_pp, d_tp = torch.empty_like(pred), torch.empty_like(pred), torch.empty_like(pred)
         sums = torch.zeros(3, dtype=torch.float64, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_ssim_l1_fwd(B, H, W, _lib.ptr(pred), _lib.ptr(target), _lib.ptr(mask), _lib.ptr(d_mu),
-                                                 _lib.ptr(d_pp), _lib.ptr(d_tp), _lib.ptr(sums), _lib.stream_ptr(dev)),
-                       "ssim_l1_fwd")
+        _lib.kernels().gb_ssim_l1_fwd(B, H, W, pred, target, mask, d_mu, d_pp, d_tp, sums)
         l1 = (sums[0] / float(B * 3 * H * W)).float()
         ssim = (sums[1] / sums[2].clamp(min=1.0)).float()
         loss = l1_weight * l1 + ssim_weight * (1.0 - ssim)
@@ -104,10 +96,8 @@ class _SsimL1(Function):
         B, _, H, W = pred.shape
         g_pred = torch.empty_like(pred)
         g_loss = g_loss.contiguous().float()
-        with torch.cuda.device(pred.device):
-            _lib.check(_lib.lib().gb_ssim_l1_bwd(B, H, W, _lib.ptr(pred), _lib.ptr(target), _lib.ptr(mask), _lib.ptr(d_mu),
-                                                 _lib.ptr(d_pp), _lib.ptr(d_tp), _lib.ptr(sums), _lib.ptr(g_loss), ctx.w[0],
-                                                 ctx.w[1], _lib.ptr(g_pred), _lib.stream_ptr(pred.device)), "ssim_l1_bwd")
+        _lib.kernels().gb_ssim_l1_bwd(B, H, W, pred, target, mask, d_mu, d_pp, d_tp, sums, g_loss, ctx.w[0],
+                                      ctx.w[1], g_pred)
         return g_pred, None, None, None, None
 
 

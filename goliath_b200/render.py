@@ -159,9 +159,7 @@ class _FinishView(th.autograd.Function):
         dev = out4.device
         rgb = th.empty(3, H, W, device=dev)
         a_img, depth = th.empty(1, H, W, device=dev), th.empty(1, H, W, device=dev)
-        with th.cuda.device(dev):
-            _lib.check(_lib.lib().gb_render_finish_fwd(H, W, _lib.ptr(out4), _lib.ptr(alpha), _lib.ptr(rgb), _lib.ptr(a_img),
-                                                       _lib.ptr(depth), _lib.stream_ptr(dev)), "render_finish_fwd")
+        _lib.kernels().gb_render_finish_fwd(H, W, out4, alpha, rgb, a_img, depth)
         ctx.save_for_backward(alpha)
         ctx.hw = (H, W)
         ctx.mark_non_differentiable(a_img)
@@ -176,9 +174,7 @@ class _FinishView(th.autograd.Function):
         g_out4 = th.empty(H, W, 4, device=alpha.device)
         g_rgb = None if g_rgb is None else g_rgb.contiguous()
         g_depth = None if g_depth is None else g_depth.contiguous()
-        with th.cuda.device(alpha.device):
-            _lib.check(_lib.lib().gb_render_finish_bwd(H, W, _lib.ptr(alpha), _lib.ptr(g_rgb), _lib.ptr(g_depth),
-                                                       _lib.ptr(g_out4), _lib.stream_ptr(alpha.device)), "render_finish_bwd")
+        _lib.kernels().gb_render_finish_bwd(H, W, alpha, g_rgb, g_depth, g_out4)
         return g_out4, None
 
 

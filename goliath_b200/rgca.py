@@ -207,12 +207,10 @@ def head_lights(head_pose: th.Tensor, campos: th.Tensor, Rt: th.Tensor, light_po
     out = {"headrel_Rt": th.empty(B, 3, 4, **f32), "headrel_campos": th.empty(B, 3, **f32),
            "headrel_light_pos": th.empty(B, L, 3, **f32), "headrel_light_sh": th.empty(B, 3, 81, **f32),
            "lightrot": th.empty(B, 3, 3, **f32) if lightrot is not None else None}
-    with th.cuda.device(dev):
-        _lib.check(_lib.lib().gb_head_lights_fwd(
-            B, L, C, _lib.ptr(args["head_pose"]), _lib.ptr(args["campos"]), _lib.ptr(args["Rt"]),
-            _lib.ptr(args["light_pos"]), _lib.ptr(args["light_intensity"]), _lib.ptr(args.get("lightrot")),
-            _lib.ptr(out["headrel_Rt"]), _lib.ptr(out["headrel_campos"]), _lib.ptr(out["headrel_light_pos"]),
-            _lib.ptr(out["headrel_light_sh"]), _lib.ptr(out["lightrot"]), _lib.stream_ptr(dev)), "head_lights_fwd")
+    _lib.kernels().gb_head_lights_fwd(
+        B, L, C, args["head_pose"], args["campos"], args["Rt"], args["light_pos"], args["light_intensity"],
+        args.get("lightrot"), out["headrel_Rt"], out["headrel_campos"], out["headrel_light_pos"],
+        out["headrel_light_sh"], out["lightrot"])
     return out
 
 

@@ -43,11 +43,8 @@ class _GaussianHeads(Function):
             if light_sh2.shape != light_sh.shape:
                 raise RuntimeError("light_sh2 must have the shape of light_sh [B,3,81]")
             shsum2 = e(B, G, 3)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_rgca_heads_fwd(
-                B, G, *[_lib.ptr(t) for t in ins], float(scale_lo), float(scale_hi),
-                *[_lib.ptr(outs[k]) for k in _OUT], _lib.ptr(shsum), _lib.ptr(light_sh2), _lib.ptr(shsum2),
-                _lib.stream_ptr(dev)), "rgca_heads_fwd")
+        _lib.kernels().gb_rgca_heads_fwd(B, G, *ins, float(scale_lo), float(scale_hi), *[outs[k] for k in _OUT], shsum,
+                                         light_sh2, shsum2)
         ctx.save_for_backward(*ins, shsum)
         ctx.light_sh2 = light_sh2  # constant (no gradient): built under no_grad upstream
         ctx.scale = (float(scale_lo), float(scale_hi))
@@ -69,14 +66,10 @@ class _GaussianHeads(Function):
         g_pt = torch.empty_like(postex)
         g_tn = torch.empty_like(tn)
         g_al = torch.empty(B, G, 3, device=dev, dtype=torch.float32)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_rgca_heads_bwd(
-                B, G, _lib.ptr(f_vnocond), _lib.ptr(f_vcond), _lib.ptr(postex), _lib.ptr(tn), _lib.ptr(albedo),
-                _lib.ptr(light_sh), _lib.ptr(campos), ctx.scale[0], ctx.scale[1], _lib.ptr(shsum),
-                *[_lib.ptr(g) for g in gouts], _lib.ptr(g_fn), _lib.ptr(g_fv), _lib.ptr(g_pt), _lib.ptr(g_tn),
-                _lib.ptr(g_al), _lib.ptr(ctx.light_sh2 if g_shsum2 is not None else None),
-                _lib.ptr(None if g_shsum2 is None or ctx.light_sh2 is None else g_shsum2.contiguous()),
-                _lib.stream_ptr(dev)), "rgca_heads_bwd")
+        _lib.kernels().gb_rgca_heads_bwd(
+            B, G, f_vnocond, f_vcond, postex, tn, albedo, light_sh, campos, ctx.scale[0], ctx.scale[1], shsum,
+            *gouts, g_fn, g_fv, g_pt, g_tn, g_al, ctx.light_sh2 if g_shsum2 is not None else None,
+            None if g_shsum2 is None or ctx.light_sh2 is None else g_shsum2.contiguous())
         g_albedo = g_al.sum(0, keepdim=True).view_as(albedo) if ctx.needs_input_grad[4] else None
         return g_fn, g_fv, g_pt, g_tn, g_albedo, None, None, None, None, None
 
@@ -113,11 +106,9 @@ class _ShadeCompose(Function):
         dev = ref_dirs.device
         color = torch.empty(N, D, 3, device=dev, dtype=torch.float32)
         spec = torch.empty(N, D, 3, device=dev, dtype=torch.float32) if want_spec else None
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_sg_shade_compose_fwd(
-                _lib.ptr(ref_dirs), _lib.ptr(sigma), _lib.ptr(light_values), _lib.ptr(light_pts), _lib.ptr(prim_pts),
-                _lib.ptr(n_lights), _lib.ptr(diff_color), _lib.ptr(spec_vis), _lib.ptr(color), _lib.ptr(spec), N, D, L,
-                int(w_type), _lib.stream_ptr(dev)), "sg_shade_compose_fwd")
+        _lib.kernels().gb_sg_shade_compose_fwd(
+            ref_dirs, sigma, light_values, light_pts, prim_pts, n_lights, diff_color, spec_vis, color, spec, N, D,
+            L, int(w_type))
         ctx.save_for_backward(ref_dirs, sigma, light_values, light_pts, prim_pts, n_lights, diff_color, spec_vis, color)
         ctx.meta = (N, D, L, int(w_type), sigma.shape, spec_vis.shape)
         ctx.set_materialize_grads(False)
@@ -136,12 +127,9 @@ class _ShadeCompose(Function):
         g_dirs, g_sig = torch.empty(N, D, 3, **f32), torch.empty(sig_shape, **f32)
         g_diff, g_vis = torch.empty(N, D, 3, **f32), torch.empty(vis_shape, **f32)
         g_light = torch.zeros_like(light_values) if ctx.needs_input_grad[2] else None
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().gb_sg_shade_compose_bwd(
-                _lib.ptr(ref_dirs), _lib.ptr(sigma), _lib.ptr(light_values), _lib.ptr(light_pts), _lib.ptr(prim_pts),
-                _lib.ptr(n_lights), _lib.ptr(diff_color), _lib.ptr(spec_vis), _lib.ptr(color), _lib.ptr(g_color),
-                _lib.ptr(g_spec), _lib.ptr(g_dirs), _lib.ptr(g_sig), _lib.ptr(g_diff), _lib.ptr(g_vis), _lib.ptr(g_light),
-                N, D, L, w_type, _lib.stream_ptr(dev)), "sg_shade_compose_bwd")
+        _lib.kernels().gb_sg_shade_compose_bwd(
+            ref_dirs, sigma, light_values, light_pts, prim_pts, n_lights, diff_color, spec_vis, color, g_color,
+            g_spec, g_dirs, g_sig, g_diff, g_vis, g_light, N, D, L, w_type)
         return g_dirs, g_sig, g_light, None, None, None, g_diff, g_vis, None, None
 
 

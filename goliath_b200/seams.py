@@ -35,10 +35,7 @@ class GatherTable:
 
 
 def _apply(B, C, n_rows, ptr, col, coef, src, in_strides, out, out_strides):
-    with torch.cuda.device(src.device):
-        _lib.check(_lib.lib().gb_sparse_rows_apply(
-            B, C, n_rows, _lib.ptr(ptr), _lib.ptr(col), _lib.ptr(coef), _lib.ptr(src), *in_strides, _lib.ptr(out),
-            *out_strides, _lib.stream_ptr(src.device)), "sparse_rows_apply")
+    _lib.kernels().gb_sparse_rows_apply(B, C, n_rows, ptr, col, coef, src, *in_strides, out, *out_strides)
 
 
 class _Gather(Function):

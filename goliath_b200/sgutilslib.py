@@ -24,11 +24,8 @@ def evaluate_gaussian_fwd(lobe_dirs, lobe_sigmas, light_values, light_pts, prim_
                  (prim_pts, "prim_pts"), (integral, "integral")):
         if t.size(0) != N:
             raise RuntimeError("Batch dim mismatch for %s." % n)
-    with torch.cuda.device(lobe_dirs.device):
-        _lib.check(_lib.lib().gb_sg_evaluate_fwd(
-            _lib.ptr(lobe_dirs), _lib.ptr(lobe_sigmas), _lib.ptr(light_values), _lib.ptr(light_pts),
-            _lib.ptr(prim_pts), _lib.ptr(n_lights), _lib.ptr(integral), N, D, L, int(w_type),
-            _lib.stream_ptr(lobe_dirs.device)), "evaluate_gaussian_fwd")
+    _lib.kernels().gb_sg_evaluate_fwd(
+        lobe_dirs, lobe_sigmas, light_values, light_pts, prim_pts, n_lights, integral, N, D, L, int(w_type))
     return []
 
 
@@ -43,10 +40,7 @@ def evaluate_gaussian_bwd(lobe_dirs, lobe_sigmas, light_values, light_pts, prim_
     if grad_light_values is not None:
         _lib.check_input(grad_light_values, "grad_light_values")
     N, D, L = _dims(lobe_dirs, light_values)
-    with torch.cuda.device(lobe_dirs.device):
-        _lib.check(_lib.lib().gb_sg_evaluate_bwd(
-            _lib.ptr(lobe_dirs), _lib.ptr(lobe_sigmas), _lib.ptr(light_values), _lib.ptr(light_pts),
-            _lib.ptr(prim_pts), _lib.ptr(n_lights), _lib.ptr(grad_integral), _lib.ptr(grad_dirs),
-            _lib.ptr(grad_lobe_sigmas), _lib.ptr(grad_light_values), N, D, L, int(w_type),
-            _lib.stream_ptr(lobe_dirs.device)), "evaluate_gaussian_bwd")
+    _lib.kernels().gb_sg_evaluate_bwd(
+        lobe_dirs, lobe_sigmas, light_values, light_pts, prim_pts, n_lights, grad_integral, grad_dirs,
+        grad_lobe_sigmas, grad_light_values, N, D, L, int(w_type))
     return []

@@ -92,9 +92,7 @@ class _PoseShadow(Function):
         _lib.check_input(x, "input")
         B, C, h, w = x.shape
         out = torch.empty(B, C, size, size, device=x.device)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().gb_pose_shadow_fwd(B * C, h, w, size, size, _lib.ptr(x), float(beta), _lib.ptr(out),
-                                                     _lib.stream_ptr(x.device)), "pose_shadow_fwd")
+        _lib.kernels().gb_pose_shadow_fwd(B * C, h, w, size, size, x, float(beta), out)
         ctx.save_for_backward(x)
         ctx.beta = float(beta)
         return out
@@ -105,10 +103,7 @@ class _PoseShadow(Function):
         B, C, h, w = x.shape
         g_out = g_out.contiguous()
         g_x = torch.empty_like(x)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().gb_pose_shadow_bwd(B * C, h, w, g_out.shape[2], g_out.shape[3], _lib.ptr(x),
-                                                     ctx.beta, _lib.ptr(g_out), _lib.ptr(g_x),
-                                                     _lib.stream_ptr(x.device)), "pose_shadow_bwd")
+        _lib.kernels().gb_pose_shadow_bwd(B * C, h, w, g_out.shape[2], g_out.shape[3], x, ctx.beta, g_out, g_x)
         return g_x, None, None
 
 

@@ -1,8 +1,6 @@
 """Drop-in for the reference's pybind module `utilslib` (extensions/utils/utils.cpp:134-137): same function names,
 positional arguments and in-place output convention; the kernel is csrc/raydirs.cu on the caller's current stream
 (the reference launches on stream 0 with no device guard, utils.cpp:79)."""
-import torch
-
 from . import _lib
 
 
@@ -17,17 +15,14 @@ def compute_raydirs_forward(viewposim, viewrotim, focalim, princptim, pixelcoord
         if pixelcoordsim.size(1) != H or pixelcoordsim.size(2) != W:
             raise RuntimeError("pixelcoordsim must be [N, H, W, 2]")
     N = viewposim.size(0)
-    dev = viewposim.device
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().gb_compute_raydirs_fwd(
-            N, int(H), int(W), _lib.ptr(viewposim), _lib.ptr(viewrotim), _lib.ptr(focalim), _lib.ptr(princptim),
-            _lib.ptr(pixelcoordsim), float(volradius), _lib.ptr(rayposim), _lib.ptr(raydirim), _lib.ptr(tminmaxim),
-            _lib.stream_ptr(dev)), "compute_raydirs_forward")
+    _lib.kernels().gb_compute_raydirs_fwd(
+        N, int(H), int(W), viewposim, viewrotim, focalim, princptim, pixelcoordsim, float(volradius), rayposim,
+        raydirim, tminmaxim)
     return []
 
 
 def compute_raydirs_backward(viewposim, viewrotim, focalim, princptim, pixelcoordsim, W, H, volradius, rayposim,
                              raydirim, tminmaxim, grad_viewpos, grad_viewrot, grad_focal, grad_princpt):
     """utils.cpp:84-132: the reference kernel (utils_kernel.cu:53-94) is an empty stub; nothing is written."""
-    _lib.check(_lib.lib().gb_compute_raydirs_bwd(), "compute_raydirs_backward")
+    _lib.kernels().gb_compute_raydirs_bwd()
     return []

@@ -104,12 +104,45 @@ def _vs_oracle(ours, ref, inputs, outs, ref_inputs=None):
     _check_grads(_grads(ours, inputs, outs, torch.float32), r64, r32)
 
 
+class _LeakyReLUBranch(torch.nn.Module):
+    """LeakyReLU that takes the branch `pos` gives at every element (z itself only decides the value)."""
+
+    def __init__(self, pos, slope):
+        super().__init__()
+        self.pos, self.slope = pos, slope
+
+    def forward(self, z):
+        return torch.where(self.pos, z, self.slope * z)
+
+
 def test_unet_vs_oracle(cuda):
     from goliath_b200.unet import UNetWB
 
     ref = bt.seeded_fill(bt.UNetWB(4, 3, 1024), 11).to(cuda)
     x = torch.randn(2, 4, 1024, 1024, device=cuda, generator=torch.Generator(device=cuda).manual_seed(1))
-    _vs_oracle(UNetWB(4, 3, 1024).to(cuda), ref, [x], ["out"])
+    ours = UNetWB(4, 3, 1024).to(cuda)
+    ours.load_state_dict(ref.state_dict(), strict=True)
+    # At 1024^2 a few pre-activations lie within fp32 rounding of the LeakyReLU kink, so an fp32 run (ours or cuDNN's)
+    # may take the other branch there than fp64 does, and one such element moves a layer's gradient by ~3e-4.  The
+    # references take our branch at those elements and only there: anywhere else the branches must agree.
+    acts = [n for n, m in ref.named_children() if isinstance(m, bt.Act)]
+    pos, z64 = {}, {}
+    hooks = [getattr(ours, n).register_forward_hook(lambda m, i, o, n=n: pos.__setitem__(n, o > 0)) for n in acts]
+    hooks += [getattr(ref, n)[0].register_forward_hook(lambda m, i, o, n=n: z64.__setitem__(n, o)) for n in acts]
+    with torch.no_grad():
+        ours(x)
+        ref.double()(x.double())
+    for h in hooks:
+        h.remove()
+    for n in acts:
+        z = z64[n]
+        ties = z.abs() <= 1e-6 * z.std()
+        assert torch.equal((z > 0) | ties, pos[n] | ties), n
+        getattr(ref, n)[1] = _LeakyReLUBranch(pos[n], getattr(ref, n)[1].negative_slope)
+    with _no_tf32():
+        r64 = _grads(ref, [x], ["out"], torch.float64)
+        r32 = _grads(ref, [x], ["out"], torch.float32)
+    _check_grads(_grads(ours, [x], ["out"], torch.float32), r64, r32)
 
 
 @pytest.mark.parametrize("biases", [False, True])
