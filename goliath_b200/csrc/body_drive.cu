@@ -141,7 +141,8 @@ GB_API int gb_face_tex_tail_fwd(int B, int Cin, int Cout, int Hi, int Wi, const 
   const dim3 grid(gb::cdiv(2 * Wi, TT_X), gb::cdiv(2 * Hi, TT_Y), B), block(TT_X, TT_Y);
   cudaStream_t s = (cudaStream_t)stream;
 #define GB_TAIL(C)                                                                                                     \
-  face_tex_tail_kernel<C><<<grid, block, 0, s>>>(Cin, Hi, Wi, x, weight_v, scale, bias, face_bias, tex_raw, tex)
+  GB_CUDA(gb::launch<face_tex_tail_kernel<C>>(grid, block, 0, s, Cin, Hi, Wi, x, weight_v, scale, bias, face_bias,     \
+                                              tex_raw, tex))
   switch (Cout) {
     case 1: GB_TAIL(1); break;
     case 2: GB_TAIL(2); break;
@@ -149,8 +150,6 @@ GB_API int gb_face_tex_tail_fwd(int B, int Cin, int Cout, int Hi, int Wi, const 
     default: GB_TAIL(4); break;
   }
 #undef GB_TAIL
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
   return 0;
 }
 
@@ -159,10 +158,7 @@ GB_API int gb_face_tex_cond_fwd(int B, int C, int Hs, int Ws, int H, int W, cons
   if (B <= 0 || C <= 0 || H <= 0 || W <= 0) return 0;
   if (Hs <= 0 || Ws <= 0) return 1;
   const dim3 grid(gb::cdiv(W, 256), H, B);
-  face_tex_cond_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(C, Hs, Ws, H, W, x, mask, out);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<face_tex_cond_kernel>(grid, 256, 0, (cudaStream_t)stream, C, Hs, Ws, H, W, x, mask, out);
 }
 
 GB_API int gb_pose_shadow_fwd(int N, int h, int w, int H, int W, const float* x, float beta, float* out,
@@ -170,10 +166,7 @@ GB_API int gb_pose_shadow_fwd(int N, int h, int w, int H, int W, const float* x,
   if (N <= 0 || H <= 0 || W <= 0) return 0;
   if (h <= 0 || w <= 0) return 1;
   const dim3 grid(gb::cdiv(W, 256), H, N);
-  pose_shadow_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(h, w, H, W, x, beta, out);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<pose_shadow_fwd_kernel>(grid, 256, 0, (cudaStream_t)stream, h, w, H, W, x, beta, out);
 }
 
 GB_API int gb_pose_shadow_bwd(int N, int h, int w, int H, int W, const float* x, float beta, const float* g_out,
@@ -181,8 +174,6 @@ GB_API int gb_pose_shadow_bwd(int N, int h, int w, int H, int W, const float* x,
   if (N <= 0 || h <= 0 || w <= 0) return 0;
   if (H <= 0 || W <= 0) return 1;
   const int n = N * h * w;
-  pose_shadow_bwd_kernel<<<gb::cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(N, h, w, H, W, x, beta, g_out, g_x);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<pose_shadow_bwd_kernel>(gb::cdiv(n, 256), 256, 0, (cudaStream_t)stream, N, h, w, H, W, x, beta,
+                                            g_out, g_x);
 }

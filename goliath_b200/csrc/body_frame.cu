@@ -116,10 +116,8 @@ GB_API int gb_depth_disc_mask(int B, int H, int W, const float* depth, float thr
                               void* stream) {
   if (B <= 0 || H <= 0 || W <= 0) return 0;
   const dim3 grid(gb::cdiv(W, DD_TX), gb::cdiv(H, DD_TY), B);
-  depth_disc_kernel<<<grid, dim3(DD_TX, DD_TY), 0, (cudaStream_t)stream>>>(H, W, depth, (double)threshold, mask);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<depth_disc_kernel>(grid, dim3(DD_TX, DD_TY), 0, (cudaStream_t)stream, H, W, depth,
+                                       (double)threshold, mask);
 }
 
 GB_API int gb_pixel_bias_fwd(int B, int C, int H, int W, int n_cams, int Hb, int Wb, const float* rgb,
@@ -127,10 +125,8 @@ GB_API int gb_pixel_bias_fwd(int B, int C, int H, int W, int n_cams, int Hb, int
   if (B <= 0 || C <= 0 || H <= 0 || W <= 0) return 0;
   if (n_cams <= 0 || Hb <= 0 || Wb <= 0) return 1;
   const dim3 grid(gb::cdiv(W, 256), H, B);
-  pixel_bias_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(B, C, H, W, n_cams, Hb, Wb, rgb, bias, idx, out);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<pixel_bias_fwd_kernel>(grid, 256, 0, (cudaStream_t)stream, B, C, H, W, n_cams, Hb, Wb, rgb, bias,
+                                           idx, out);
 }
 
 GB_API int gb_pixel_bias_bwd(int B, int C, int H, int W, int n_cams, int Hb, int Wb, const long long* idx,
@@ -138,9 +134,6 @@ GB_API int gb_pixel_bias_bwd(int B, int C, int H, int W, int n_cams, int Hb, int
   if (n_cams <= 0 || Hb <= 0 || Wb <= 0) return 0;
   if (H <= 0 || W <= 0) return 1;
   const int n = n_cams * Hb * Wb;
-  pixel_bias_bwd_kernel<<<gb::cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(B, C, H, W, n_cams, Hb, Wb, idx, g_out,
-                                                                           g_bias);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<pixel_bias_bwd_kernel>(gb::cdiv(n, 256), 256, 0, (cudaStream_t)stream, B, C, H, W, n_cams, Hb, Wb,
+                                           idx, g_out, g_bias);
 }

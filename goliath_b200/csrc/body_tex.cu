@@ -280,11 +280,8 @@ GB_API int gb_body_tex_compose_fwd(int B, int H, int W, const float* t1, const f
                                    const float* scale, const float* bias, float tex_std, const float* tex_mean,
                                    const float* s3, float* out, void* stream) {
   if (B <= 0 || H <= 0 || W <= 0) return 0;
-  body_tex_compose_fwd_kernel<<<grid_of(H, W), dim3(TX, TY), 0, (cudaStream_t)stream>>>(
+  return gb::launch<body_tex_compose_fwd_kernel>(grid_of(H, W), dim3(TX, TY), 0, (cudaStream_t)stream,
       B, H, W, t1, h, v, scale, bias, tex_std, tex_mean, s3, out);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 GB_API int gb_body_tex_compose_bwd(int B, int H, int W, const float* t1, const float* h, const float* v,
@@ -294,11 +291,9 @@ GB_API int gb_body_tex_compose_bwd(int B, int H, int W, const float* t1, const f
   if (B <= 0 || H <= 0 || W <= 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
   const dim3 g = grid_of(H, W);
-  body_tex_compose_bwd_kernel<<<g, dim3(TX, TY), 0, s>>>(B, H, W, t1, h, v, scale, bias, tex_std, tex_mean, s3, g_out,
-                                                         g_t1, g_h, g_bias, g_s3, workspace);
+  GB_CUDA(gb::launch<body_tex_compose_bwd_kernel>(g, dim3(TX, TY), 0, s, B, H, W, t1, h, v, scale, bias, tex_std,
+                                                  tex_mean, s3, g_out, g_t1, g_h, g_bias, g_s3, workspace));
   constexpr int warps = NO * NK / 4;  // 4 CTAs of 12 warps
-  body_tex_gw_reduce_kernel<<<gb::cdiv(NO * NK, warps), warps * 32, 0, s>>>((int)(g.x * g.y), workspace, g_w);
-  gb::count_launches(2);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<body_tex_gw_reduce_kernel>(gb::cdiv(NO * NK, warps), warps * 32, 0, s, (int)(g.x * g.y), workspace,
+                                               g_w);
 }

@@ -3,28 +3,55 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
+#include <mutex>
+#include <utility>
+
 #define GB_API extern "C" __attribute__((visibility("default")))
 
-// Every C-ABI entry point returns 0 or a cudaError_t value (never throws, never allocates).
-#define GB_CHECK_LAUNCH()                          \
+// Every C-ABI entry point returns 0 or a cudaError_t value (never throws, never allocates).  Variadic so that a
+// template argument list with commas passes through: GB_CUDA(gb::launch<k<4, false>>(...)).
+#define GB_CUDA(...)                               \
   do {                                             \
-    cudaError_t e__ = cudaGetLastError();          \
-    if (e__ != cudaSuccess) return (int)e__;       \
-  } while (0)
-
-#define GB_CUDA(x)                                 \
-  do {                                             \
-    cudaError_t e__ = (x);                         \
-    if (e__ != cudaSuccess) return (int)e__;       \
+    const int e__ = (int)(__VA_ARGS__);            \
+    if (e__ != 0) return e__;                      \
   } while (0)
 
 namespace gb {
 
 // number of kernel launches issued by this library (bench.py reports it as gpu_launches)
 extern unsigned long long g_launch_count;
-inline void count_launches(int n) { __atomic_fetch_add(&g_launch_count, (unsigned long long)n, __ATOMIC_RELAXED); }
 
 constexpr int kNumSMs = 132;  // H100 SXM
+constexpr int kMaxDevices = 64;
+
+// Every kernel of the library is launched through here: Kernel<<<grid, block, smem, stream>>>(args...).
+// Without an opt-in a kernel's dynamic shared memory is limited to 48 KB less its static shared memory.  The opt-in
+// applies to the current device: it is made once per (kernel, device) for any dynamic shared memory and raised when a
+// later call asks for more.  Returns cudaGetLastError(); only a launch that succeeded is counted in g_launch_count.
+template <auto Kernel, class... Args>
+[[nodiscard]] cudaError_t launch(dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
+  if (smem > 0) {
+    static std::atomic<size_t> granted[kMaxDevices];
+    static std::mutex mu;
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    if (dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
+    if (granted[dev].load(std::memory_order_acquire) < smem) {
+      std::lock_guard<std::mutex> lock(mu);
+      if (granted[dev].load(std::memory_order_relaxed) < smem) {
+        e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        granted[dev].store(smem, std::memory_order_release);
+      }
+    }
+  }
+  Kernel<<<grid, block, smem, stream>>>(std::forward<Args>(args)...);
+  const cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) __atomic_fetch_add(&g_launch_count, 1ull, __ATOMIC_RELAXED);
+  return e;
+}
 
 __host__ __device__ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }

@@ -20,18 +20,18 @@ namespace {
 int co_tile(int n) { return n <= 4 ? 4 : 8; }
 
 template <int CO_T, int K>
-void launch_fwd(int B, int Cin, int Cout, const InMap& x, const float* v, const float* scale, const float* bias,
-                int bias_mode, float slope, int apply_act, float* out, cudaStream_t s) {
+[[nodiscard]] int launch_fwd(int B, int Cin, int Cout, const InMap& x, const float* v, const float* scale, const float* bias,
+                             int bias_mode, float slope, int apply_act, float* out, cudaStream_t s) {
   dim3 grid(gb::cdiv(x.H, TP) * gb::cdiv(x.W, TP), gb::cdiv(Cout, CO_T), B);
-  wn_conv_fwd_kernel<CO_T, K, 1, false, 0, IN_PLAIN><<<grid, TP * TP, 0, s>>>(
+  return gb::launch<wn_conv_fwd_kernel<CO_T, K, 1, false, 0, IN_PLAIN>>(grid, TP * TP, 0, s,
       Cin, Cout, 1, x, x.H, x.W, v, scale, bias, bias_mode, apply_act, slope, x, nullptr, nullptr, nullptr, out, nullptr);
 }
 
 template <int CO_T, int K>
-void launch_dgrad(int B, int Cin, int Cout, int H, int W, const float* gz, const float* v, const float* scale,
-                  float* gx, long long x_bs, cudaStream_t s) {
+[[nodiscard]] int launch_dgrad(int B, int Cin, int Cout, int H, int W, const float* gz, const float* v,
+                               const float* scale, float* gx, long long x_bs, cudaStream_t s) {
   dim3 grid(gb::cdiv(H, TP) * gb::cdiv(W, TP), gb::cdiv(Cin, CO_T), B);
-  wn_conv_dgrad_kernel<CO_T, K, 1, false, 0><<<grid, TP * TP, 0, s>>>(
+  return gb::launch<wn_conv_dgrad_kernel<CO_T, K, 1, false, 0>>(grid, TP * TP, 0, s,
       Cin, Cout, 1, H, W, gz, v, scale, nullptr, 1.f, 0, nullptr, nullptr, nullptr, gx, x_bs);
 }
 
@@ -56,15 +56,11 @@ GB_API int gb_conv2d_wnub_fwd(int B, int Cin, int Cout, int H, int W, int K, con
   cudaStream_t s = (cudaStream_t)stream;
   const InMap xm = plain_map(x, x_bs, H, W);
   if (co_tile(Cout) == 8) {
-    if (K == 1) launch_fwd<8, 1>(B, Cin, Cout, xm, v, scale, bias, bias_mode, slope, apply_act, out, s);
-    else launch_fwd<8, 3>(B, Cin, Cout, xm, v, scale, bias, bias_mode, slope, apply_act, out, s);
-  } else {
-    if (K == 1) launch_fwd<4, 1>(B, Cin, Cout, xm, v, scale, bias, bias_mode, slope, apply_act, out, s);
-    else launch_fwd<4, 3>(B, Cin, Cout, xm, v, scale, bias, bias_mode, slope, apply_act, out, s);
+    if (K == 1) return launch_fwd<8, 1>(B, Cin, Cout, xm, v, scale, bias, bias_mode, slope, apply_act, out, s);
+    return launch_fwd<8, 3>(B, Cin, Cout, xm, v, scale, bias, bias_mode, slope, apply_act, out, s);
   }
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  if (K == 1) return launch_fwd<4, 1>(B, Cin, Cout, xm, v, scale, bias, bias_mode, slope, apply_act, out, s);
+  return launch_fwd<4, 3>(B, Cin, Cout, xm, v, scale, bias, bias_mode, slope, apply_act, out, s);
 }
 
 GB_API size_t gb_conv2d_wnub_bwd_workspace_bytes(int B, int Cin, int Cout, int H, int W, int K) {
@@ -85,35 +81,26 @@ GB_API int gb_conv2d_wnub_bwd(int B, int Cin, int Cout, int H, int W, int K, con
   cudaStream_t s = (cudaStream_t)stream;
   const long long per_item = (long long)Cout * H * W;
   const unsigned grid = (unsigned)gb::cdiv64(per_item, 256);
-  int n = 0;
   const float* g = gout;
   if (apply_act) {
-    act_bwd_kernel<<<grid, 256, 0, s>>>(B, per_item, gout, nullptr, out, slope, gz, bias_mode == 2 ? g_bias : nullptr);
+    GB_CUDA(gb::launch<act_bwd_kernel>(grid, 256, 0, s, B, per_item, gout, nullptr, out, slope, gz,
+                                       bias_mode == 2 ? g_bias : nullptr));
     g = gz;
-    ++n;
   } else if (bias_mode == 2 && g_bias) {
-    batch_sum_kernel<<<grid, 256, 0, s>>>(B, per_item, gout, g_bias);
-    ++n;
+    GB_CUDA(gb::launch<batch_sum_kernel>(grid, 256, 0, s, B, per_item, gout, g_bias));
   }
-  if (bias_mode == 1 && g_bias) {
-    chan_sum_kernel<<<Cout, 256, 0, s>>>(B, Cout, H * W, g, g_bias);
-    ++n;
-  }
+  if (bias_mode == 1 && g_bias) GB_CUDA(gb::launch<chan_sum_kernel>(Cout, 256, 0, s, B, Cout, H * W, g, g_bias));
   if (gx) {
     if (co_tile(Cin) == 8) {
-      if (K == 1) launch_dgrad<8, 1>(B, Cin, Cout, H, W, g, v, scale, gx, x_bs, s);
-      else launch_dgrad<8, 3>(B, Cin, Cout, H, W, g, v, scale, gx, x_bs, s);
+      if (K == 1) GB_CUDA(launch_dgrad<8, 1>(B, Cin, Cout, H, W, g, v, scale, gx, x_bs, s));
+      else GB_CUDA(launch_dgrad<8, 3>(B, Cin, Cout, H, W, g, v, scale, gx, x_bs, s));
     } else {
-      if (K == 1) launch_dgrad<4, 1>(B, Cin, Cout, H, W, g, v, scale, gx, x_bs, s);
-      else launch_dgrad<4, 3>(B, Cin, Cout, H, W, g, v, scale, gx, x_bs, s);
+      if (K == 1) GB_CUDA(launch_dgrad<4, 1>(B, Cin, Cout, H, W, g, v, scale, gx, x_bs, s));
+      else GB_CUDA(launch_dgrad<4, 3>(B, Cin, Cout, H, W, g, v, scale, gx, x_bs, s));
     }
-    ++n;
   }
   const InMap xm = plain_map(x, x_bs, H, W);
   float* part = (float*)workspace;
-  if (K == 1) launch_wgrad<1, 1>(B, Cin, Cout, 1, xm, H, W, g, gw, part, kWgradPerSM, s);
-  else launch_wgrad<3, 1>(B, Cin, Cout, 1, xm, H, W, g, gw, part, kWgradPerSM, s);
-  gb::count_launches(n + 2);
-  GB_CHECK_LAUNCH();
-  return 0;
+  if (K == 1) return launch_wgrad<1, 1>(B, Cin, Cout, 1, xm, H, W, g, gw, part, kWgradPerSM, s);
+  return launch_wgrad<3, 1>(B, Cin, Cout, 1, xm, H, W, g, gw, part, kWgradPerSM, s);
 }

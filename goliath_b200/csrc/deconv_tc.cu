@@ -372,19 +372,11 @@ PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
 }
 
 template <int NT, int NPX>
-cudaError_t launch_tc(dim3 grid, size_t smem, cudaStream_t s, const CUtensorMap& ma_hi, const CUtensorMap& ma_lo,
-                      const CUtensorMap& mb_hi, const CUtensorMap& mb_lo, const TcArgs& a) {
+[[nodiscard]] cudaError_t launch_tc(dim3 grid, size_t smem, cudaStream_t s, const CUtensorMap& ma_hi,
+                                    const CUtensorMap& ma_lo, const CUtensorMap& mb_hi, const CUtensorMap& mb_lo,
+                                    const TcArgs& a) {
   static_assert(NT * NPX <= kMaxNT, "accumulators per thread");
-  static bool configured = false;
-  if (!configured) {
-    // 227 KB per block on sm_90, less the kernel's static shared memory (barriers)
-    const cudaError_t e = cudaFuncSetAttribute(deconv_tc_kernel<NT, NPX>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               227 * 1024 - 2048);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
-  deconv_tc_kernel<NT, NPX><<<grid, kThreads, smem, s>>>(ma_hi, ma_lo, mb_hi, mb_lo, a);
-  return cudaGetLastError();
+  return gb::launch<deconv_tc_kernel<NT, NPX>>(grid, kThreads, smem, s, ma_hi, ma_lo, mb_hi, mb_lo, a);
 }
 
 }  // namespace
@@ -398,10 +390,8 @@ GB_API size_t gb_deconv_tc_weight_bytes(int Cin_pad, int Cout) {
 GB_API int gb_nchw_to_nhwc_split(int B, int C, int Cpad, int H, int W, const float* x, float* hi, float* lo, void* stream) {
   const long long total = (long long)B * H * W * Cpad;
   if (total <= 0) return 0;
-  nchw_to_nhwc_split_kernel<<<(unsigned)gb::cdiv64(total, 256), 256, 0, (cudaStream_t)stream>>>(B, C, Cpad, H * W, x, hi, lo);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<nchw_to_nhwc_split_kernel>((unsigned)gb::cdiv64(total, 256), 256, 0, (cudaStream_t)stream, B, C,
+                                               Cpad, H * W, x, hi, lo);
 }
 
 // Tensor-core forward of ConvTranspose2dWNUB(k=4,s=2,p=1) [+LeakyReLU].  x_hi/x_lo: NHWC [B,Hi,Wi,Cin_pad] (tf32 hi
@@ -422,11 +412,10 @@ GB_API int gb_deconv4x4s2_tc_fwd(int B, int Cin, int Cin_pad, int Cout, int Hi, 
   cudaStream_t s = (cudaStream_t)stream;
   float* w_hi = w_scratch;
   float* w_lo = w_scratch + (size_t)16 * Npad * Cin_pad;
-  int launches = 1;
   if (v) {  // v == NULL: w_scratch still holds the matrices prepared by an earlier call with the same weight_v
     const long long total = 16ll * Npad * Cin_pad;
-    weight_prep_kernel<<<(unsigned)gb::cdiv64(total, 256), 256, 0, s>>>(Cin, Cin_pad, Cout, Npad, v, w_hi, w_lo);
-    ++launches;
+    GB_CUDA(gb::launch<weight_prep_kernel>((unsigned)gb::cdiv64(total, 256), 256, 0, s, Cin, Cin_pad, Cout, Npad, v,
+                                           w_hi, w_lo));
   }
   // tile geometry: 128 positions = tile_r rows x tile_c columns
   int tile_c = 128;
@@ -504,8 +493,5 @@ GB_API int gb_deconv4x4s2_tc_fwd(int B, int Cin, int Cin_pad, int Cout, int Hi, 
 #undef GB_TC_CASE
     default: break;
   }
-  GB_CUDA(err);
-  gb::count_launches(launches);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return err;
 }

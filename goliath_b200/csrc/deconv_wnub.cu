@@ -317,11 +317,12 @@ __global__ void __launch_bounds__(256, 2) deconv4x4s2_fwd_wide_kernel(
 
 // The round-1 forward kernel's launch (also the stride-2 convolution's data gradient, SCALE_IN = true)
 template <bool SCALE_IN>
-int launch_deconv_fwd(int B, int Cin, int Cout, int Hi, int Wi, const float* x, const float* v, const float* scale,
-                      const float* bias, float slope, int apply_act, float* out, cudaStream_t s) {
+[[nodiscard]] int launch_deconv_fwd(int B, int Cin, int Cout, int Hi, int Wi, const float* x, const float* v,
+                                    const float* scale, const float* bias, float slope, int apply_act, float* out,
+                                    cudaStream_t s) {
   dim3 grid(gb::cdiv(Hi, TQ) * gb::cdiv(Wi, TQ), gb::cdiv(Cout, CO_T), B);
-  deconv4x4s2_fwd_kernel<SCALE_IN><<<grid, TQ * TQ, 0, s>>>(Cin, Cout, Hi, Wi, x, v, scale, bias, slope, apply_act, out);
-  return 1;
+  return gb::launch<deconv4x4s2_fwd_kernel<SCALE_IN>>(grid, TQ * TQ, 0, s, Cin, Cout, Hi, Wi, x, v, scale, bias, slope,
+                                                      apply_act, out);
 }
 
 }  // namespace
@@ -340,22 +341,11 @@ GB_API int gb_deconv4x4s2_wnub_fwd(int B, int Cin, int Cout, int Hi, int Wi, con
     int per_cta = 1;  // grow while the grid still fills the machine a few times over
     while (per_cta < nblk && (long long)tiles * B * gb::cdiv(nblk, per_cta * 2) >= 4LL * 2 * gb::kNumSMs) per_cta *= 2;
     const size_t smem = (size_t)W_CI * W_HY * W_HS * 8 + (size_t)2 * W_CI * 16 * W_CO * 4;
-    static bool configured = false;
-    if (!configured) {
-      GB_CUDA(cudaFuncSetAttribute(deconv4x4s2_fwd_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      configured = true;
-    }
     dim3 grid(tiles, gb::cdiv(nblk, per_cta), B);
-    deconv4x4s2_fwd_wide_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(Cin, Cout, Hi, Wi, per_cta, x, v, scale, bias,
-                                                                           slope, apply_act, out);
-    gb::count_launches(1);
-    GB_CHECK_LAUNCH();
-    return 0;
+    return gb::launch<deconv4x4s2_fwd_wide_kernel>(grid, 256, smem, (cudaStream_t)stream, Cin, Cout, Hi, Wi, per_cta, x,
+                                                   v, scale, bias, slope, apply_act, out);
   }
-  gb::count_launches(launch_deconv_fwd<false>(B, Cin, Cout, Hi, Wi, x, v, scale, bias, slope, apply_act, out,
-                                              (cudaStream_t)stream));
-  GB_CHECK_LAUNCH();
-  return 0;
+  return launch_deconv_fwd<false>(B, Cin, Cout, Hi, Wi, x, v, scale, bias, slope, apply_act, out, (cudaStream_t)stream);
 }
 
 // =====================================================================================================
@@ -765,24 +755,17 @@ __global__ void __launch_bounds__(256, 1) deconv4x4s2_bwd_weight_wide_kernel(
 // data gradient and whose weight gradient is this weight gradient with the roles of x and gz swapped).  `wide` picks
 // the kernels for the high-resolution layers; the caller has checked Wi % 4 == 0, Wi >= 32, Hi >= 16.
 template <bool CONV_FWD>
-int launch_bwd_data(bool wide, int B, int Cin, int Cout, int Hi, int Wi, const float* gz, const float* v,
-                    const float* scale, const float* bias, float slope, int apply_act, float* gx, cudaStream_t s) {
+[[nodiscard]] int launch_bwd_data(bool wide, int B, int Cin, int Cout, int Hi, int Wi, const float* gz, const float* v,
+                                  const float* scale, const float* bias, float slope, int apply_act, float* gx,
+                                  cudaStream_t s) {
   if (wide) {
-    static bool configured = false;
-    if (!configured) {
-      GB_CUDA(cudaFuncSetAttribute(deconv4x4s2_bwd_data_wide_kernel<CONV_FWD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   DW_SMEM));
-      configured = true;
-    }
     dim3 grid(gb::cdiv(Hi, DW_Y) * gb::cdiv(Wi, DW_X), gb::cdiv(Cin, DW_CI), B);
-    deconv4x4s2_bwd_data_wide_kernel<CONV_FWD><<<grid, 256, DW_SMEM, s>>>(Cin, Cout, Hi, Wi, gz, v, scale, bias, slope,
-                                                                          apply_act, gx);
-    return 1;
+    return gb::launch<deconv4x4s2_bwd_data_wide_kernel<CONV_FWD>>(grid, 256, DW_SMEM, s, Cin, Cout, Hi, Wi, gz, v,
+                                                                  scale, bias, slope, apply_act, gx);
   }
   dim3 grid(gb::cdiv(Hi, BD_T) * gb::cdiv(Wi, BD_T), gb::cdiv(Cin, BD_CI), B);
-  deconv4x4s2_bwd_data_kernel<CONV_FWD><<<grid, BD_T * BD_T, 0, s>>>(Cin, Cout, Hi, Wi, gz, v, scale, bias, slope,
-                                                                     apply_act, gx);
-  return 1;
+  return gb::launch<deconv4x4s2_bwd_data_kernel<CONV_FWD>>(grid, BD_T * BD_T, 0, s, Cin, Cout, Hi, Wi, gz, v, scale,
+                                                           bias, slope, apply_act, gx);
 }
 
 // The backward's kernels for a transposed convolution Cin -> Cout on an Hi x Wi input, and its weight gradient's split
@@ -811,39 +794,27 @@ BwdPlan bwd_plan(bool conv, int B, int Cin, int Cout, int Hi, int Wi) {
   return p;
 }
 
-// gw [Cin,Cout,4,4] written; two launches
-int launch_bwd_weight(const BwdPlan& p, int B, int Cin, int Cout, int Hi, int Wi, const float* x, const float* gz,
-                      float* gw, float* part, cudaStream_t s) {
+// gw [Cin,Cout,4,4] written
+[[nodiscard]] int launch_bwd_weight(const BwdPlan& p, int B, int Cin, int Cout, int Hi, int Wi, const float* x,
+                                    const float* gz, float* gw, float* part, cudaStream_t s) {
   if (p.wide) {
-    static bool configured = false;
-    if (!configured) {
-      GB_CUDA(cudaFuncSetAttribute(deconv4x4s2_bwd_weight_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WW_SMEM));
-      configured = true;
-    }
     dim3 grid(p.split, gb::cdiv(Cin, WW_CI), gb::cdiv(Cout, WW_CO));
-    deconv4x4s2_bwd_weight_wide_kernel<<<grid, 256, WW_SMEM, s>>>(B, Cin, Cout, Hi, Wi, x, gz, part);
+    GB_CUDA(gb::launch<deconv4x4s2_bwd_weight_wide_kernel>(grid, 256, WW_SMEM, s, B, Cin, Cout, Hi, Wi, x, gz, part));
   } else {
     dim3 grid(p.split, gb::cdiv(Cin, NW_CI), gb::cdiv(Cout, NW_CO));
-    deconv4x4s2_bwd_weight_kernel<<<grid, 256, 0, s>>>(B, Cin, Cout, Hi, Wi, x, gz, part);
+    GB_CUDA(gb::launch<deconv4x4s2_bwd_weight_kernel>(grid, 256, 0, s, B, Cin, Cout, Hi, Wi, x, gz, part));
   }
   const int n = Cin * Cout * 16;
-  split_sum_kernel<<<gb::cdiv(n, 256), 256, 0, s>>>(p.split, n, part, gw);
-  return 2;
+  return gb::launch<split_sum_kernel>(gb::cdiv(n, 256), 256, 0, s, p.split, n, part, gw);
 }
 
 // With an activation: gz = gout * act'(out) and the untied-bias gradient.  Without one, gz is gout and the bias
 // gradient its batch sum (NULL at B == 1, where the caller aliases it to gout).
-int launch_act_bwd(int B, long long per_item, const float* out, const float* gout, float slope, int apply_act, float* gz,
-                   float* g_bias, cudaStream_t s) {
+[[nodiscard]] int launch_act_bwd(int B, long long per_item, const float* out, const float* gout, float slope,
+                                 int apply_act, float* gz, float* g_bias, cudaStream_t s) {
   const unsigned grid = (unsigned)gb::cdiv64(per_item, 256);
-  if (apply_act) {
-    act_bwd_kernel<<<grid, 256, 0, s>>>(B, per_item, gout, nullptr, out, slope, gz, g_bias);
-    return 1;
-  }
-  if (g_bias) {
-    batch_sum_kernel<<<grid, 256, 0, s>>>(B, per_item, gout, g_bias);
-    return 1;
-  }
+  if (apply_act) return gb::launch<act_bwd_kernel>(grid, 256, 0, s, B, per_item, gout, nullptr, out, slope, gz, g_bias);
+  if (g_bias) return gb::launch<batch_sum_kernel>(grid, 256, 0, s, B, per_item, gout, g_bias);
   return 0;
 }
 
@@ -864,13 +835,11 @@ GB_API int gb_deconv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Hi, int Wi, con
                                    float* gz, float* g_bias, float* gx, float* gw, void* workspace, void* stream) {
   if (B <= 0 || Cin <= 0 || Cout <= 0 || Hi <= 0 || Wi <= 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
-  int launches = launch_act_bwd(B, (long long)Cout * 4 * Hi * Wi, out, gout, slope, apply_act, gz, g_bias, s);
+  GB_CUDA(launch_act_bwd(B, (long long)Cout * 4 * Hi * Wi, out, gout, slope, apply_act, gz, g_bias, s));
   const float* g = apply_act ? gz : gout;
   const BwdPlan p = bwd_plan(false, B, Cin, Cout, Hi, Wi);
-  if (gx) launches += launch_bwd_data<false>(p.wide, B, Cin, Cout, Hi, Wi, g, v, scale, nullptr, 1.f, 0, gx, s);
-  if (gw) launches += launch_bwd_weight(p, B, Cin, Cout, Hi, Wi, x, g, gw, (float*)workspace, s);
-  gb::count_launches(launches);
-  GB_CHECK_LAUNCH();
+  if (gx) GB_CUDA(launch_bwd_data<false>(p.wide, B, Cin, Cout, Hi, Wi, g, v, scale, nullptr, 1.f, 0, gx, s));
+  if (gw) GB_CUDA(launch_bwd_weight(p, B, Cin, Cout, Hi, Wi, x, g, gw, (float*)workspace, s));
   return 0;
 }
 
@@ -901,11 +870,8 @@ GB_API int gb_conv4x4s2_wnub_fwd(int B, int Cin, int Cout, int Ho, int Wo, const
                                  const float* scale, const float* bias, float slope, int apply_act, float* out,
                                  void* stream) {
   if (B <= 0 || Cin <= 0 || Cout <= 0 || Ho <= 0 || Wo <= 0) return 0;
-  const int n = launch_bwd_data<true>(conv_wide_fwd(B, Cout, Ho, Wo), B, Cout, Cin, Ho, Wo, x, v, scale, bias, slope,
-                                      apply_act, out, (cudaStream_t)stream);
-  gb::count_launches(n);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return launch_bwd_data<true>(conv_wide_fwd(B, Cout, Ho, Wo), B, Cout, Cin, Ho, Wo, x, v, scale, bias, slope,
+                               apply_act, out, (cudaStream_t)stream);
 }
 
 GB_API size_t gb_conv4x4s2_wnub_bwd_workspace_bytes(int B, int Cin, int Cout, int Ho, int Wo) {
@@ -922,13 +888,11 @@ GB_API int gb_conv4x4s2_wnub_bwd(int B, int Cin, int Cout, int Ho, int Wo, const
                                  float* gz, float* g_bias, float* gx, float* gw, void* workspace, void* stream) {
   if (B <= 0 || Cin <= 0 || Cout <= 0 || Ho <= 0 || Wo <= 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
-  int launches = launch_act_bwd(B, (long long)Cout * Ho * Wo, out, gout, slope, apply_act, gz, g_bias, s);
+  GB_CUDA(launch_act_bwd(B, (long long)Cout * Ho * Wo, out, gout, slope, apply_act, gz, g_bias, s));
   const float* g = apply_act ? gz : gout;
-  if (gx) launches += launch_deconv_fwd<true>(B, Cout, Cin, Ho, Wo, g, v, scale, nullptr, 1.f, 0, gx, s);
+  if (gx) GB_CUDA(launch_deconv_fwd<true>(B, Cout, Cin, Ho, Wo, g, v, scale, nullptr, 1.f, 0, gx, s));
   if (gw)
-    launches += launch_bwd_weight(bwd_plan(true, B, Cout, Cin, Ho, Wo), B, Cout, Cin, Ho, Wo, g, x, gw,
-                                  (float*)workspace, s);
-  gb::count_launches(launches);
-  GB_CHECK_LAUNCH();
+    GB_CUDA(launch_bwd_weight(bwd_plan(true, B, Cout, Cin, Ho, Wo), B, Cout, Cin, Ho, Wo, g, x, gw, (float*)workspace,
+                              s));
   return 0;
 }

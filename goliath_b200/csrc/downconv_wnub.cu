@@ -42,33 +42,34 @@ InMap x_map(const BlockArgs& a) {
 }
 
 template <int CO_T>
-void launch_conv1(const BlockArgs& a, const InMap& x, const float* v1, const float* s1, const float* b1, float slope,
-                  float* h1, cudaStream_t s) {
+[[nodiscard]] int launch_conv1(const BlockArgs& a, const InMap& x, const float* v1, const float* s1, const float* b1,
+                               float slope, float* h1, cudaStream_t s) {
   const int cin_g = a.Cin / a.groups;
   dim3 grid(gb::cdiv(a.H, TP) * gb::cdiv(a.W, TP), a.groups * gb::cdiv(cin_g, CO_T), a.B);
-  wn_conv_fwd_kernel<CO_T, 3, 1, false, 2><<<grid, TP * TP, 0, s>>>(cin_g, cin_g, a.groups, x, a.H, a.W, v1, s1, b1, 2, 1,
-                                                                  slope, x, nullptr, nullptr, nullptr, h1, nullptr);
+  return gb::launch<wn_conv_fwd_kernel<CO_T, 3, 1, false, 2>>(grid, TP * TP, 0, s, cin_g, cin_g, a.groups, x, a.H, a.W,
+                                                              v1, s1, b1, 2, 1, slope, x, nullptr, nullptr, nullptr, h1,
+                                                              nullptr);
 }
 
 template <int CO_T>
-void launch_conv2(const BlockArgs& a, const InMap& x, const float* h1, const float* v2, const float* s2,
-                  const float* b2, const float* vr, const float* sr, const float* br, float slope, float* out,
-                  unsigned char* mask, cudaStream_t s) {
+[[nodiscard]] int launch_conv2(const BlockArgs& a, const InMap& x, const float* h1, const float* v2, const float* s2,
+                               const float* b2, const float* vr, const float* sr, const float* br, float slope,
+                               float* out, unsigned char* mask, cudaStream_t s) {
   const int cin_g = a.Cin / a.groups, cout_g = a.Cout / a.groups, Ho = a.H / 2, Wo = a.W / 2;
   dim3 grid(gb::cdiv(Ho, TP) * gb::cdiv(Wo, TP), a.groups * gb::cdiv(cout_g, CO_T), a.B);
-  wn_conv_fwd_kernel<CO_T, 3, 2, true, 2><<<grid, TP * TP, 0, s>>>(
+  return gb::launch<wn_conv_fwd_kernel<CO_T, 3, 2, true, 2>>(grid, TP * TP, 0, s,
       cin_g, cout_g, a.groups, plain_map(h1, (long long)a.Cin * a.H * a.W, a.H, a.W), Ho, Wo, v2, s2, b2, 2, 1, slope,
       x, vr, sr, br, out, mask);
 }
 
 // gz1 = conv2^T(gz2) * lrelu'(h1), or (ACT = false) gx = conv1^T(gz1) + conv_resize^T(gout)
 template <int CO_T, int S, bool ACT, int SKIP>
-void launch_dgrad(int B, int Cin, int n_sum_g, int groups, int H, int W, const float* gz, const float* v,
-                  const float* scale, const float* h1, float slope, int n_skip_g, const float* gs, const float* vr,
-                  const float* sr, float* out, cudaStream_t s) {
+[[nodiscard]] int launch_dgrad(int B, int Cin, int n_sum_g, int groups, int H, int W, const float* gz, const float* v,
+                               const float* scale, const float* h1, float slope, int n_skip_g, const float* gs,
+                               const float* vr, const float* sr, float* out, cudaStream_t s) {
   const int cin_g = Cin / groups;
   dim3 grid(gb::cdiv(H, TP) * gb::cdiv(W, TP), groups * gb::cdiv(cin_g, CO_T), B);
-  wn_conv_dgrad_kernel<CO_T, 3, S, ACT, SKIP><<<grid, TP * TP, 0, s>>>(
+  return gb::launch<wn_conv_dgrad_kernel<CO_T, 3, S, ACT, SKIP>>(grid, TP * TP, 0, s,
       cin_g, n_sum_g, groups, H, W, gz, v, scale, h1, slope, n_skip_g, gs, vr, sr, out, (long long)Cin * H * W);
 }
 
@@ -86,16 +87,11 @@ GB_API int gb_downconv_block_fwd(int B, int Cin, int Cout, int groups, int H, in
   cudaStream_t s = (cudaStream_t)stream;
   const InMap xm = x_map(a);
   if ((Cin / groups) % 8 == 0)
-    launch_conv1<8>(a, xm, v1, s1, b1, slope, h1, s);
+    GB_CUDA(launch_conv1<8>(a, xm, v1, s1, b1, slope, h1, s));
   else
-    launch_conv1<4>(a, xm, v1, s1, b1, slope, h1, s);
-  if ((Cout / groups) % 8 == 0)
-    launch_conv2<8>(a, xm, h1, v2, s2, b2, vr, sr, br, slope, out, mask, s);
-  else
-    launch_conv2<4>(a, xm, h1, v2, s2, b2, vr, sr, br, slope, out, mask, s);
-  gb::count_launches(2);
-  GB_CHECK_LAUNCH();
-  return 0;
+    GB_CUDA(launch_conv1<4>(a, xm, v1, s1, b1, slope, h1, s));
+  if ((Cout / groups) % 8 == 0) return launch_conv2<8>(a, xm, h1, v2, s2, b2, vr, sr, br, slope, out, mask, s);
+  return launch_conv2<4>(a, xm, h1, v2, s2, b2, vr, sr, br, slope, out, mask, s);
 }
 
 GB_API size_t gb_downconv_block_bwd_workspace_bytes(int B, int Cin, int Cout, int groups, int H, int W) {
@@ -120,29 +116,23 @@ GB_API int gb_downconv_block_bwd(int B, int Cin, int Cout, int groups, int H, in
   const int cin_g = Cin / groups, cout_g = Cout / groups, Ho = H / 2, Wo = W / 2;
   const long long n_out = (long long)Cout * Ho * Wo, n_in = (long long)Cin * H * W;
   float* part = (float*)workspace;
-  act_bwd_kernel<<<(unsigned)gb::cdiv64(n_out, 256), 256, 0, s>>>(B, n_out, gout, mask, nullptr, slope, gz2, gb2);
-  chan_sum_kernel<<<Cout, 256, 0, s>>>(B, Cout, Ho * Wo, gout, gbr);
+  GB_CUDA(gb::launch<act_bwd_kernel>((unsigned)gb::cdiv64(n_out, 256), 256, 0, s, B, n_out, gout, mask, nullptr, slope,
+                                     gz2, gb2));
+  GB_CUDA(gb::launch<chan_sum_kernel>(Cout, 256, 0, s, B, Cout, Ho * Wo, gout, gbr));
   if (cin_g % 8 == 0)
-    launch_dgrad<8, 2, true, 0>(B, Cin, cout_g, groups, H, W, gz2, v2, s2, h1, slope, 0, nullptr, nullptr, nullptr,
-                                    gz1, s);
+    GB_CUDA(launch_dgrad<8, 2, true, 0>(B, Cin, cout_g, groups, H, W, gz2, v2, s2, h1, slope, 0, nullptr, nullptr,
+                                        nullptr, gz1, s));
   else
-    launch_dgrad<4, 2, true, 0>(B, Cin, cout_g, groups, H, W, gz2, v2, s2, h1, slope, 0, nullptr, nullptr, nullptr,
-                                    gz1, s);
-  batch_sum_kernel<<<(unsigned)gb::cdiv64(n_in, 256), 256, 0, s>>>(B, n_in, gz1, gb1);
-  launch_wgrad<3, 2>(B, Cin, Cout, groups, plain_map(h1, n_in, H, W), Ho, Wo, gz2, gw2, part, kWgradPerSM, s);
-  launch_wgrad<3, 1>(B, Cin, Cin, groups, xm, H, W, gz1, gw1, part, kWgradPerSM, s);
-  launch_wgrad<1, 2>(B, Cin, Cout, groups, xm, Ho, Wo, gout, gwr, part, kWgradPerSM, s);
-  int n = 10;
-  if (gx) {
-    if (cin_g % 8 == 0)
-      launch_dgrad<8, 1, false, 2>(B, Cin, cin_g, groups, H, W, gz1, v1, s1, nullptr, slope, cout_g, gout, vr, sr,
+    GB_CUDA(launch_dgrad<4, 2, true, 0>(B, Cin, cout_g, groups, H, W, gz2, v2, s2, h1, slope, 0, nullptr, nullptr,
+                                        nullptr, gz1, s));
+  GB_CUDA(gb::launch<batch_sum_kernel>((unsigned)gb::cdiv64(n_in, 256), 256, 0, s, B, n_in, gz1, gb1));
+  GB_CUDA(launch_wgrad<3, 2>(B, Cin, Cout, groups, plain_map(h1, n_in, H, W), Ho, Wo, gz2, gw2, part, kWgradPerSM, s));
+  GB_CUDA(launch_wgrad<3, 1>(B, Cin, Cin, groups, xm, H, W, gz1, gw1, part, kWgradPerSM, s));
+  GB_CUDA(launch_wgrad<1, 2>(B, Cin, Cout, groups, xm, Ho, Wo, gout, gwr, part, kWgradPerSM, s));
+  if (!gx) return 0;
+  if (cin_g % 8 == 0)
+    return launch_dgrad<8, 1, false, 2>(B, Cin, cin_g, groups, H, W, gz1, v1, s1, nullptr, slope, cout_g, gout, vr, sr,
+                                        gx, s);
+  return launch_dgrad<4, 1, false, 2>(B, Cin, cin_g, groups, H, W, gz1, v1, s1, nullptr, slope, cout_g, gout, vr, sr,
                                       gx, s);
-    else
-      launch_dgrad<4, 1, false, 2>(B, Cin, cin_g, groups, H, W, gz1, v1, s1, nullptr, slope, cout_g, gout, vr, sr,
-                                      gx, s);
-    ++n;
-  }
-  gb::count_launches(n);
-  GB_CHECK_LAUNCH();
-  return 0;
 }

@@ -299,10 +299,8 @@ __global__ void __launch_bounds__(256) envmap_rotate_kernel(int B, int He, int W
 GB_API int gb_envmap_rotate(int B, int He, int We, const float* image, const float* rot_mat, float* out, void* stream) {
   if (B <= 0) return 0;
   if (He < 1 || We < 1) return (int)cudaErrorInvalidValue;
-  envmap_rotate_kernel<<<dim3(gb::cdiv(He * We, 256), B), 256, 0, (cudaStream_t)stream>>>(B, He, We, image, rot_mat, out);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<envmap_rotate_kernel>(dim3(gb::cdiv(He * We, 256), B), 256, 0, (cudaStream_t)stream, B, He, We,
+                                          image, rot_mat, out);
 }
 
 GB_API int gb_envmap_compose_fwd(int B, int H, int W, int He, int We, const float* render, const float* alpha,
@@ -312,11 +310,9 @@ GB_API int gb_envmap_compose_fwd(int B, int H, int W, int He, int We, const floa
   if (H < kBall || W < kBall || He < 1 || We < 1 || rt_rows < 3 || rt_cols < 3) return (int)cudaErrorInvalidValue;
   ComposeArgs a = {B, H, W, He, We, rt_rows, rt_cols, render, alpha, envbg, K, Rt, hblur, out};
   const cudaStream_t st = (cudaStream_t)stream;
-  envmap_image_hblur_kernel<<<dim3(gb::cdiv(W, kRowTile), H, B), kRowTile, 0, st>>>(a);
-  envmap_vblur_compose_kernel<<<dim3(gb::cdiv(W, kColTile), gb::cdiv(H, kColRows), B), dim3(kColTile, 8), 0, st>>>(a);
-  gb::count_launches(2);
-  GB_CHECK_LAUNCH();
-  return 0;
+  GB_CUDA(gb::launch<envmap_image_hblur_kernel>(dim3(gb::cdiv(W, kRowTile), H, B), kRowTile, 0, st, a));
+  return gb::launch<envmap_vblur_compose_kernel>(dim3(gb::cdiv(W, kColTile), gb::cdiv(H, kColRows), B),
+                                                 dim3(kColTile, 8), 0, st, a);
 }
 
 GB_API int gb_envmap_compose_bwd(int B, int H, int W, const float* g_out, float* g_render, void* stream) {
@@ -324,8 +320,5 @@ GB_API int gb_envmap_compose_bwd(int B, int H, int W, const float* g_out, float*
   if (H < kBall || W < kBall) return (int)cudaErrorInvalidValue;
   const size_t n = (size_t)B * 3 * H * W;
   const int blocks = (int)(n < (size_t)gb::kNumSMs * 8 * 256 ? gb::cdiv64((int64_t)n, 256) : gb::kNumSMs * 8);
-  envmap_compose_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(B, H, W, g_out, g_render);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<envmap_compose_bwd_kernel>(blocks, 256, 0, (cudaStream_t)stream, B, H, W, g_out, g_render);
 }

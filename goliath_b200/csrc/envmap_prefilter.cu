@@ -276,10 +276,7 @@ GB_API int gb_envmap_prefilter_sg(int B, int q, const int32_t* level_hw, const f
   }
   const long long blocks = gb::cdiv64(a.first[q], kWarps);
   if (blocks > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
-  envmap_prefilter_sg_kernel<<<(unsigned)blocks, 32 * kWarps, 0, (cudaStream_t)stream>>>(a);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<envmap_prefilter_sg_kernel>((unsigned)blocks, 32 * kWarps, 0, (cudaStream_t)stream, a);
 }
 
 GB_API int gb_envmap_spin_table(int B, int He, int We, const float* angles, const float* image, float perc90,
@@ -293,20 +290,16 @@ GB_API int gb_envmap_spin_table(int B, int He, int We, const float* angles, cons
     RotArgs r;
     r.n = B - b0 < kMaxRotB ? B - b0 : kMaxRotB;
     for (int i = 0; i < r.n; ++i) r.angle[i] = angles[b0 + i];
-    envmap_spin_rot_kernel<<<1, kMaxRotB, 0, st>>>(r, lightrot + 9 * (size_t)b0);
-    gb::count_launches(1);
+    GB_CUDA(gb::launch<envmap_spin_rot_kernel>(1, kMaxRotB, 0, st, r, lightrot + 9 * (size_t)b0));
   }
-  GB_CHECK_LAUNCH();
   const size_t plane = (size_t)He * We;
   for (int b = 0; b < B; ++b) {  // one probe for every item: the rotation's batch stride is one image
     const int e = gb_envmap_rotate(1, He, We, image, lightrot + 9 * (size_t)b, envbg + 3 * plane * b, stream);
     if (e) return e;
   }
   const int rows = B * 3 * He;
-  envmap_spin_hpass_kernel<<<gb::cdiv(rows, kRowWarps), 32 * kRowWarps, kRowWarps * We * sizeof(float), st>>>(
-      rows, We, perc90, envbg, hpass);
-  envmap_spin_table_kernel<<<B, kOutH * kOutW, 0, st>>>(He, env_scale, hpass, envmap, light_intensity, norm_scale);
-  gb::count_launches(2);
-  GB_CHECK_LAUNCH();
-  return 0;
+  GB_CUDA(gb::launch<envmap_spin_hpass_kernel>(gb::cdiv(rows, kRowWarps), 32 * kRowWarps, kRowWarps * We * sizeof(float),
+                                               st, rows, We, perc90, envbg, hpass));
+  return gb::launch<envmap_spin_table_kernel>(B, kOutH * kOutW, 0, st, He, env_scale, hpass, envmap, light_intensity,
+                                              norm_scale);
 }

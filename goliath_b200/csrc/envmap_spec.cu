@@ -130,10 +130,7 @@ GB_API int gb_envmap_spec_fwd(int B, int G, int q, const float* const* levels, c
   if (e) return e;
   a.ref_dirs = ref_dirs; a.sigma = sigma; a.spec_vis = spec_vis; a.lightrot = lightrot; a.level_scale = level_scale;
   a.spec = spec;
-  envmap_spec_kernel<false><<<dim3(gb::cdiv(G, 256), B), 256, 0, (cudaStream_t)stream>>>(a);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<envmap_spec_kernel<false>>(dim3(gb::cdiv(G, 256), B), 256, 0, (cudaStream_t)stream, a);
 }
 
 // g_spec [B,G,3] -> g_ref_dirs [B,G,3], g_spec_vis [B,G] (both overwritten).
@@ -147,8 +144,5 @@ GB_API int gb_envmap_spec_bwd(int B, int G, int q, const float* const* levels, c
   if (e) return e;
   a.ref_dirs = ref_dirs; a.sigma = sigma; a.spec_vis = spec_vis; a.lightrot = lightrot; a.level_scale = level_scale;
   a.g_spec = g_spec; a.g_ref_dirs = g_ref_dirs; a.g_spec_vis = g_spec_vis;
-  envmap_spec_kernel<true><<<dim3(gb::cdiv(G, 256), B), 256, 0, (cudaStream_t)stream>>>(a);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<envmap_spec_kernel<true>>(dim3(gb::cdiv(G, 256), B), 256, 0, (cudaStream_t)stream, a);
 }

@@ -143,12 +143,10 @@ GB_API int gb_vert_normals_fwd(int B, int V, int F, const float* v, const int32_
                                void* stream) {
   if (B <= 0 || V <= 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
-  if (F > 0) face_normals_scatter_kernel<<<dim3(gb::cdiv(F, kThreads), B), kThreads, 0, s>>>(B, V, F, v, vi, eps, acc);
+  if (F > 0) GB_CUDA(gb::launch<face_normals_scatter_kernel>(dim3(gb::cdiv(F, kThreads), B), kThreads, 0, s, B, V, F, v,
+                                                             vi, eps, acc));
   const long long n = (long long)B * V;
-  normalize3_kernel<<<(unsigned)gb::cdiv64(n, kThreads), kThreads, 0, s>>>(n, acc, eps, vn);
-  gb::count_launches(2);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<normalize3_kernel>((unsigned)gb::cdiv64(n, kThreads), kThreads, 0, s, n, acc, eps, vn);
 }
 
 // g_vn [B,V,3] -> g_v [B,V,3] (zero-filled by the caller, accumulated); g_acc [B,V,3] scratch.
@@ -157,10 +155,10 @@ GB_API int gb_vert_normals_bwd(int B, int V, int F, const float* v, const int32_
   if (B <= 0 || V <= 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
   const long long n = (long long)B * V;
-  normalize3_bwd_kernel<<<(unsigned)gb::cdiv64(n, kThreads), kThreads, 0, s>>>(n, acc, g_vn, eps, g_acc);
-  if (F > 0) face_normals_scatter_bwd_kernel<<<dim3(gb::cdiv(F, kThreads), B), kThreads, 0, s>>>(B, V, F, v, vi, eps, g_acc, g_v);
-  gb::count_launches(2);
-  GB_CHECK_LAUNCH();
+  GB_CUDA(gb::launch<normalize3_bwd_kernel>((unsigned)gb::cdiv64(n, kThreads), kThreads, 0, s, n, acc, g_vn, eps,
+                                            g_acc));
+  if (F > 0) GB_CUDA(gb::launch<face_normals_scatter_bwd_kernel>(dim3(gb::cdiv(F, kThreads), B), kThreads, 0, s, B, V,
+                                                                 F, v, vi, eps, g_acc, g_v));
   return 0;
 }
 
@@ -168,20 +166,14 @@ GB_API int gb_vert_normals_bwd(int B, int V, int F, const float* v, const int32_
 GB_API int gb_values_to_uv_fwd(int B, int V, int C, int64_t T, const float* values, const int32_t* index, const float* bary,
                                float* out, void* stream) {
   if (B <= 0 || T <= 0 || C <= 0) return 0;
-  values_to_uv_kernel<<<dim3((unsigned)gb::cdiv64(T, kThreads), B), kThreads, 0, (cudaStream_t)stream>>>(B, V, C, T, values, index,
-                                                                                                     bary, out);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<values_to_uv_kernel>(dim3((unsigned)gb::cdiv64(T, kThreads), B), kThreads, 0, (cudaStream_t)stream,
+                                         B, V, C, T, values, index, bary, out);
 }
 
 // g_out [B,C,T] -> g_values [B,V,C] (zero-filled by the caller, accumulated)
 GB_API int gb_values_to_uv_bwd(int B, int V, int C, int64_t T, const int32_t* index, const float* bary, const float* g_out,
                                float* g_values, void* stream) {
   if (B <= 0 || T <= 0 || C <= 0) return 0;
-  values_to_uv_bwd_kernel<<<dim3((unsigned)gb::cdiv64(T, kThreads), B), kThreads, 0, (cudaStream_t)stream>>>(B, V, C, T, index, bary,
-                                                                                                         g_out, g_values);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<values_to_uv_bwd_kernel>(dim3((unsigned)gb::cdiv64(T, kThreads), B), kThreads, 0,
+                                             (cudaStream_t)stream, B, V, C, T, index, bary, g_out, g_values);
 }

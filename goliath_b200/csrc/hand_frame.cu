@@ -180,12 +180,9 @@ GB_API int gb_hand_valid_gather_fwd(int B, int K, int n_valid, int tpl_elems, co
                                     float* tpl_out, float* pos_out, float* rot_out, float* scale_out, void* stream) {
   if (B <= 0 || K <= 0 || n_valid <= 0) return 0;
   if (tpl_elems <= 0 || tpl_elems % 4 != 0 || B > 65535) return 1;
-  valid_gather_fwd_kernel<<<dim3(K, B), kGatherThreads, 0, (cudaStream_t)stream>>>(
+  return gb::launch<valid_gather_fwd_kernel>(dim3(K, B), kGatherThreads, 0, (cudaStream_t)stream,
       K, n_valid, tpl_elems / 4, slot, (const float4*)tpl, pos, rot, scale, inv_radius, (float4*)tpl_out, pos_out,
       rot_out, scale_out);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 GB_API int gb_hand_valid_gather_bwd(int B, int K, int n_valid, int tpl_elems, const int32_t* slot, const float* g_tpl,
@@ -194,12 +191,9 @@ GB_API int gb_hand_valid_gather_bwd(int B, int K, int n_valid, int tpl_elems, co
                                     void* stream) {
   if (B <= 0 || K <= 0) return 0;
   if (tpl_elems <= 0 || tpl_elems % 4 != 0 || B > 65535) return 1;
-  valid_gather_bwd_kernel<<<dim3(K, B), kGatherThreads, 0, (cudaStream_t)stream>>>(
+  return gb::launch<valid_gather_bwd_kernel>(dim3(K, B), kGatherThreads, 0, (cudaStream_t)stream,
       K, n_valid, tpl_elems / 4, slot, (const float4*)g_tpl, g_pos, g_rot, g_scale, inv_radius, (float4*)g_tpl_full,
       g_pos_full, g_rot_full, g_scale_full);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 GB_API size_t gb_hand_finish_workspace_bytes(int B, int H, int W) {
@@ -214,10 +208,7 @@ GB_API int gb_hand_finish_fwd(int B, int H, int W, const float* rayrgba, const f
   FinishArgs a = {};
   a.B = B; a.HW = H * W; a.rayrgba = (const float4*)rayrgba; a.cal_w = cal_w; a.cal_b = cal_b; a.grey = grey;
   a.bg = bg; a.rgb = rgb; a.alpha = alpha;
-  hand_finish_fwd_kernel<<<dim3(finish_blocks(a.HW), B), kFinishThreads, 0, (cudaStream_t)stream>>>(a);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<hand_finish_fwd_kernel>(dim3(finish_blocks(a.HW), B), kFinishThreads, 0, (cudaStream_t)stream, a);
 }
 
 GB_API int gb_hand_finish_bwd(int B, int H, int W, const float* rayrgba, const float* cal_w, const int32_t* grey,
@@ -229,13 +220,10 @@ GB_API int gb_hand_finish_bwd(int B, int H, int W, const float* rayrgba, const f
   a.B = B; a.HW = H * W; a.rayrgba = (const float4*)rayrgba; a.cal_w = cal_w; a.grey = grey; a.bg = bg;
   a.g_rgb = g_rgb; a.g_alpha = g_alpha; a.g_rayrgba = (float4*)g_rayrgba; a.partial = (float*)workspace;
   const int nb = finish_blocks(a.HW);
-  hand_finish_bwd_kernel<<<dim3(nb, B), kFinishThreads, 0, (cudaStream_t)stream>>>(a);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
+  GB_CUDA(gb::launch<hand_finish_bwd_kernel>(dim3(nb, B), kFinishThreads, 0, (cudaStream_t)stream, a));
   if (cal_w) {
-    hand_finish_cal_reduce_kernel<<<B, kFinishThreads, 0, (cudaStream_t)stream>>>(nb, a.partial, g_cal_w, g_cal_b);
-    gb::count_launches(1);
-    GB_CHECK_LAUNCH();
+    GB_CUDA(gb::launch<hand_finish_cal_reduce_kernel>(B, kFinishThreads, 0, (cudaStream_t)stream, nb, a.partial,
+                                                      g_cal_w, g_cal_b));
   }
   return 0;
 }

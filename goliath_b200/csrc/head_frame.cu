@@ -138,10 +138,7 @@ GB_API int gb_head_lights_fwd(int B, int L, int C, const float* head_pose, const
                               float* headrel_light_sh, float* lightrot_out, void* stream) {
   if (B <= 0) return 0;
   if (L < 0 || (C != 1 && C != 3) || ((lightrot == nullptr) != (lightrot_out == nullptr))) return 1;
-  head_lights_kernel<<<B, LT_THREADS, 0, (cudaStream_t)stream>>>(L, C, head_pose, campos, Rt, light_pos,
-                                                                 light_intensity, lightrot, headrel_Rt, headrel_campos,
-                                                                 headrel_light_pos, headrel_light_sh, lightrot_out);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<head_lights_kernel>(B, LT_THREADS, 0, (cudaStream_t)stream, L, C, head_pose, campos, Rt, light_pos,
+                                        light_intensity, lightrot, headrel_Rt, headrel_campos, headrel_light_pos,
+                                        headrel_light_sh, lightrot_out);
 }

@@ -245,10 +245,7 @@ GB_API int gb_lbs_skeleton_fwd(int B, int J, int P, int S, const float* motion, 
   if (J > kMaxJoints || P < 0 || S < 0 || n_levels < 1 || n_levels > J || scale_stride < 0) return (int)cudaErrorInvalidValue;
   SkelArgs a{B, J, P, S, scale_stride, n_levels, motion, scale, transform, transform_offsets, joint_offset,
              joint_rotation, bind_state, parents, level_order, level_start, mats, states};
-  skeleton_kernel<<<B, kSkelThreads, 0, (cudaStream_t)stream>>>(a);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<skeleton_kernel>(B, kSkelThreads, 0, (cudaStream_t)stream, a);
 }
 
 GB_API int gb_lbs_skin_fwd(int B, int V, int J, int vb, const float* mats, const float* verts, const float* templ,
@@ -257,10 +254,8 @@ GB_API int gb_lbs_skin_fwd(int B, int V, int J, int vb, const float* mats, const
   if (B <= 0 || V <= 0) return 0;
   if (J <= 0 || (vb != 1 && vb != B)) return (int)cudaErrorInvalidValue;
   SkinArgs a{B, V, J, vb, mats, verts, templ, skin_weights, global_scaling, skin_indices};
-  skin_fwd_kernel<<<(unsigned)gb::cdiv64((long long)B * V, kThreads), kThreads, 0, (cudaStream_t)stream>>>(a, out);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<skin_fwd_kernel>((unsigned)gb::cdiv64((long long)B * V, kThreads), kThreads, 0,
+                                     (cudaStream_t)stream, a, out);
 }
 
 GB_API int gb_lbs_skin_bwd(int B, int V, int J, int vb, const float* mats, const int32_t* skin_indices,
@@ -269,11 +264,8 @@ GB_API int gb_lbs_skin_bwd(int B, int V, int J, int vb, const float* mats, const
   if (B <= 0 || V <= 0) return 0;
   if (J <= 0 || (vb != 1 && vb != B)) return (int)cudaErrorInvalidValue;
   SkinArgs a{B, V, J, vb, mats, nullptr, nullptr, skin_weights, global_scaling, skin_indices};
-  skin_bwd_kernel<<<(unsigned)gb::cdiv64((long long)vb * V, kThreads), kThreads, 0, (cudaStream_t)stream>>>(a, g_out,
-                                                                                                           g_verts);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<skin_bwd_kernel>((unsigned)gb::cdiv64((long long)vb * V, kThreads), kThreads, 0,
+                                     (cudaStream_t)stream, a, g_out, g_verts);
 }
 
 GB_API int gb_lbs_unskin_fwd(int B, int V, int J, int vb, const float* mats, const float* verts, const float* templ,
@@ -282,8 +274,6 @@ GB_API int gb_lbs_unskin_fwd(int B, int V, int J, int vb, const float* mats, con
   if (B <= 0 || V <= 0) return 0;
   if (J <= 0 || (vb != 1 && vb != B)) return (int)cudaErrorInvalidValue;
   SkinArgs a{B, V, J, vb, mats, verts, templ, skin_weights, global_scaling, skin_indices};
-  unskin_fwd_kernel<<<(unsigned)gb::cdiv64((long long)B * V, kThreads), kThreads, 0, (cudaStream_t)stream>>>(a, out);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<unskin_fwd_kernel>((unsigned)gb::cdiv64((long long)B * V, kThreads), kThreads, 0,
+                                       (cudaStream_t)stream, a, out);
 }

@@ -558,15 +558,13 @@ GB_API int gb_mesh_raster(int B, int V, int F, int H, int W, const float* v_pix,
   unsigned long long* zb = (unsigned long long*)ws;
   int* n_large = (int*)(ws + align256((size_t)n * 8));
   int* large = n_large + 64;
-  raster_init_kernel<<<grid1(n), kBlock, 0, s>>>(n, zb, n_large);
+  GB_CUDA(gb::launch<raster_init_kernel>(grid1(n), kBlock, 0, s, n, zb, n_large));
   if (F > 0) {
-    raster_small_kernel<<<grid1((long long)B * F), kBlock, 0, s>>>(B, V, F, H, W, v_pix, vi, zb, n_large, large);
-    raster_large_kernel<<<gb::kNumSMs * 8, kBlock, 0, s>>>(V, F, H, W, v_pix, vi, zb, n_large, large);
+    GB_CUDA(gb::launch<raster_small_kernel>(grid1((long long)B * F), kBlock, 0, s, B, V, F, H, W, v_pix, vi, zb,
+                                            n_large, large));
+    GB_CUDA(gb::launch<raster_large_kernel>(gb::kNumSMs * 8, kBlock, 0, s, V, F, H, W, v_pix, vi, zb, n_large, large));
   }
-  raster_resolve_kernel<<<grid1(n), kBlock, 0, s>>>(n, zb, index_img);
-  gb::count_launches(F > 0 ? 4 : 2);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<raster_resolve_kernel>(grid1(n), kBlock, 0, s, n, zb, index_img);
 }
 
 GB_API int gb_mesh_render_fwd(int B, int V, int F, int H, int W, int C, int Ht, int Wt, const float* v_pix,
@@ -575,12 +573,8 @@ GB_API int gb_mesh_render_fwd(int B, int V, int F, int H, int W, int C, int Ht, 
                               float* render, void* stream) {
   if (!sizes_ok(B, H, W, F) || C < 0 || Ht <= 0 || Wt <= 0) return B == 0 ? 0 : (int)cudaErrorInvalidValue;
   const long long n = (long long)B * H * W;
-  render_fwd_kernel<<<grid1(n), kBlock, 0, (cudaStream_t)stream>>>(B, V, H, W, C, Ht, Wt, v_pix, vi, vti, vt, tex,
-                                                                    index_img, depth_img, bary_img, vt_img, mask,
-                                                                    render);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<render_fwd_kernel>(grid1(n), kBlock, 0, (cudaStream_t)stream, B, V, H, W, C, Ht, Wt, v_pix, vi, vti,
+                                       vt, tex, index_img, depth_img, bary_img, vt_img, mask, render);
 }
 
 GB_API size_t gb_mesh_render_bwd_workspace_bytes(int B, int F, int H, int W, int Ht, int Wt) {
@@ -611,33 +605,28 @@ GB_API int gb_mesh_render_bwd(int B, int V, int F, int H, int W, int C, int Ht, 
   float* face_grad = (float*)(ws + L.face_grad);
   void* sort_ws = ws + L.sort_ws;
 
-  render_bwd_record_kernel<<<grid1(n), kBlock, 0, s>>>(B, V, F, H, W, C, Ht, Wt, v_pix, vi, vti, vt, tex, index_img,
-                                                       vt_img, render, g_render, edge_grad, rec, key_face, key_tex,
-                                                       pix);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
+  GB_CUDA(gb::launch<render_bwd_record_kernel>(grid1(n), kBlock, 0, s, B, V, F, H, W, C, Ht, Wt, v_pix, vi, vti, vt,
+                                               tex, index_img, vt_img, render, g_render, edge_grad, rec, key_face,
+                                               key_tex, pix));
   // g_v_pix: pixels by face, one warp per face, then the vertex gather
   GB_CUDA(cudaMemsetAsync(bins_face, 0, (size_t)nf * 8, s));
   int err = gb_sort_intersects(n, (const int64_t*)key_face, pix, (int64_t*)key_sorted, pix_face, bits_for(nf), sort_ws, stream);
   if (err) return err;
   if (nf > 0) {
-    bin_edges_kernel<<<grid1(n), kBlock, 0, s>>>(n, key_sorted, nf, bins_face);
-    face_reduce_kernel<<<grid1(nf * 32), kBlock, 0, s>>>(nf, bins_face, pix_face, rec, face_grad);
-    gb::count_launches(2);
+    GB_CUDA(gb::launch<bin_edges_kernel>(grid1(n), kBlock, 0, s, n, key_sorted, nf, bins_face));
+    GB_CUDA(gb::launch<face_reduce_kernel>(grid1(nf * 32), kBlock, 0, s, nf, bins_face, pix_face, rec, face_grad));
   }
   if (V > 0) {
-    vertex_gather_kernel<<<grid1((long long)B * V), kBlock, 0, s>>>(B, V, F, inc_ptr, inc, face_grad, g_v_pix);
-    gb::count_launches(1);
+    GB_CUDA(gb::launch<vertex_gather_kernel>(grid1((long long)B * V), kBlock, 0, s, B, V, F, inc_ptr, inc, face_grad,
+                                             g_v_pix));
   }
   // g_tex: pixels by the texel of their top-left tap, one thread per texel
   GB_CUDA(cudaMemsetAsync(bins_tex, 0, (size_t)nt * 8, s));
   err = gb_sort_intersects(n, (const int64_t*)key_tex, pix, (int64_t*)key_sorted, pix_tex, bits_for(nt), sort_ws, stream);
   if (err) return err;
-  bin_edges_kernel<<<grid1(n), kBlock, 0, s>>>(n, key_sorted, nt, bins_tex);
+  GB_CUDA(gb::launch<bin_edges_kernel>(grid1(n), kBlock, 0, s, n, key_sorted, nt, bins_tex));
   if (C > 0)
-    texel_gather_kernel<<<grid1((long long)B * Ht * Wt), kBlock, 0, s>>>(B, H, W, C, Ht, Wt, bins_tex, pix_tex, vt_img,
-                                                                          g_render, g_tex);
-  gb::count_launches(C > 0 ? 2 : 1);
-  GB_CHECK_LAUNCH();
+    GB_CUDA(gb::launch<texel_gather_kernel>(grid1((long long)B * Ht * Wt), kBlock, 0, s, B, H, W, C, Ht, Wt, bins_tex,
+                                            pix_tex, vt_img, g_render, g_tex));
   return 0;
 }

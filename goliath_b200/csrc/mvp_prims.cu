@@ -238,11 +238,8 @@ GB_API int gb_mvp_slab_to_prims_fwd(int B, int PZ, int U, int PSX, int PSY, int 
   if (PSX <= 0 || PSY <= 0 || U % PSX || U % PSY) return (int)cudaErrorInvalidValue;
   SlabGeom g{B, PZ, U, PSX, PSY, U / PSX, U / PSY, Kout};
   const long long total = (long long)B * PZ * U * U;
-  slab_prims_kernel<false><<<(unsigned)gb::cdiv64(total, 256), 256, 0, (cudaStream_t)stream>>>(
+  return gb::launch<slab_prims_kernel<false>>((unsigned)gb::cdiv64(total, 256), 256, 0, (cudaStream_t)stream,
       g, rgb, alpha, prim_slot, rgb_mul, rgb_add, apply_relu, reinterpret_cast<float4*>(tpl), nullptr, nullptr);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 // Backward: g_tpl [B,Kout,PZ,PSY,PSX,4] -> g_rgb [B,PZ,3,U,U], g_alpha [B,PZ,1,U,U] (every element written; dropped
@@ -254,12 +251,9 @@ GB_API int gb_mvp_slab_to_prims_bwd(int B, int PZ, int U, int PSX, int PSY, int 
   if (PSX <= 0 || PSY <= 0 || U % PSX || U % PSY) return (int)cudaErrorInvalidValue;
   SlabGeom g{B, PZ, U, PSX, PSY, U / PSX, U / PSY, Kout};
   const long long total = (long long)B * PZ * U * U;
-  slab_prims_kernel<true><<<(unsigned)gb::cdiv64(total, 256), 256, 0, (cudaStream_t)stream>>>(
+  return gb::launch<slab_prims_kernel<true>>((unsigned)gb::cdiv64(total, 256), 256, 0, (cudaStream_t)stream,
       g, rgb, alpha, prim_slot, rgb_mul, rgb_add, apply_relu,
       reinterpret_cast<float4*>(const_cast<float*>(g_tpl)), g_rgb, g_alpha);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 // hand_mvp.py:317-321 + :410-425.  dec [B,9,K] = TransDecoder.dec0 output viewed [B,9,64*64]; posbase [B,K,3],
@@ -268,11 +262,8 @@ GB_API int gb_mvp_prim_transform_fwd(int B, int K, const float* dec, const float
                                      float prim_scale, int zero_delta, float* primpos, float* primrot, float* primscale,
                                      void* stream) {
   if (B <= 0 || K <= 0) return 0;
-  prim_transform_kernel<false><<<gb::cdiv(B * K, 128), 128, 0, (cudaStream_t)stream>>>(
+  return gb::launch<prim_transform_kernel<false>>(gb::cdiv(B * K, 128), 128, 0, (cudaStream_t)stream,
       B, K, dec, posbase, rotbase, prim_scale, zero_delta, primpos, primrot, primscale, nullptr);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 // hand_mvp.py:386-408 (make_postex, compute_tbn) and :230-236 (compute_view_cos + values_to_uv) on the posed mesh.
@@ -282,11 +273,8 @@ GB_API int gb_mvp_prim_frames_fwd(int B, int V, int NT, int T, const float* vert
   if (B <= 0 || T <= 0) return 0;
   if (V <= 0 || (rotbase && (NT <= 0 || !vtidx || !vt)) || (view_cos && (!vn || !campos)))
     return (int)cudaErrorInvalidValue;
-  prim_frames_kernel<<<gb::cdiv(B * T, 128), 128, 0, (cudaStream_t)stream>>>(B, V, NT, T, verts, vidx, vtidx, bary, vt,
-                                                                             vn, campos, posbase, rotbase, view_cos);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<prim_frames_kernel>(gb::cdiv(B * T, 128), 128, 0, (cudaStream_t)stream, B, V, NT, T, verts, vidx,
+                                        vtidx, bary, vt, vn, campos, posbase, rotbase, view_cos);
 }
 
 // g_primpos / g_primrot / g_primscale may be NULL (no gradient arrived); g_dec [B,9,K] is written.
@@ -294,10 +282,7 @@ GB_API int gb_mvp_prim_transform_bwd(int B, int K, const float* dec, const float
                                      float prim_scale, int zero_delta, const float* g_primpos, const float* g_primrot,
                                      const float* g_primscale, float* g_dec, void* stream) {
   if (B <= 0 || K <= 0) return 0;
-  prim_transform_kernel<true><<<gb::cdiv(B * K, 128), 128, 0, (cudaStream_t)stream>>>(
+  return gb::launch<prim_transform_kernel<true>>(gb::cdiv(B * K, 128), 128, 0, (cudaStream_t)stream,
       B, K, dec, posbase, rotbase, prim_scale, zero_delta, const_cast<float*>(g_primpos), const_cast<float*>(g_primrot),
       const_cast<float*>(g_primscale), g_dec);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }

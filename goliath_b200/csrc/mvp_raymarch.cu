@@ -953,11 +953,8 @@ GB_API int gb_mvp_compute_aabb(int N, int K, const float* primpos, const float* 
   cudaStream_t s = (cudaStream_t)stream;
   GB_CUDA(cudaMemsetAsync(workspace, 0, gb_mvp_aabb_workspace_bytes(N, K), s));
   const int blocks = min(gb::cdiv(N * K, 256), gb::kNumSMs * 8);
-  compute_aabb_kernel<<<blocks, 256, 0, s>>>(N, K, primpos, primrot, primscale, sortedobjid, (const int2*)nodechildren,
-                                             nodeparent, nodeaabb, (int*)workspace);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<compute_aabb_kernel>(blocks, 256, 0, s, N, K, primpos, primrot, primscale, sortedobjid,
+                                         (const int2*)nodechildren, nodeparent, nodeaabb, (int*)workspace);
 }
 
 // replaces mvpraymarchlib.raymarch_forward (mvpraymarch.cpp:179-283 -> mvpraymarch_kernel.cu:41-130).
@@ -983,24 +980,14 @@ GB_API int gb_mvp_raymarch_fwd(int N, int H, int W, int K, const float* raypos, 
   const int nwarps = (blocksizex * blocksizey + 31) / 32;
   const size_t smem = (size_t)nwarps * kMaxHit * (sizeof(int) + sizeof(float2));
   cudaStream_t s = (cudaStream_t)stream;
-#define GB_RM_FWD(WP, SH)                                                                                         \
-  do {                                                                                                            \
-    if (smem > 48 * 1024)                                                                                         \
-      GB_CUDA(cudaFuncSetAttribute(raymarch_fwd_kernel<WP, SH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    raymarch_fwd_kernel<WP, SH><<<grid, block, smem, s>>>(a);                                                      \
-  } while (0)
-  if (algo == 1) { if (shadow) GB_RM_FWD(true, true); else GB_RM_FWD(true, false); }
-  else if (shadow) GB_RM_FWD(false, true);
-  else if (raymarch_mode() & 1) {  // lane-compacted sampling (option, algo 0 without the shadow splat)
-    const size_t smem_q = smem + (size_t)nwarps * sizeof(RMQueue);
-    if (smem_q > 48 * 1024)
-      GB_CUDA(cudaFuncSetAttribute(raymarch_fwd_queue_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_q));
-    raymarch_fwd_queue_kernel<<<grid, block, smem_q, s>>>(a);
-  } else GB_RM_FWD(false, false);
-#undef GB_RM_FWD
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  if (algo == 1) {
+    if (shadow) return gb::launch<raymarch_fwd_kernel<true, true>>(grid, block, smem, s, a);
+    return gb::launch<raymarch_fwd_kernel<true, false>>(grid, block, smem, s, a);
+  }
+  if (shadow) return gb::launch<raymarch_fwd_kernel<false, true>>(grid, block, smem, s, a);
+  if (raymarch_mode() & 1)  // lane-compacted sampling (option, algo 0 without the shadow splat)
+    return gb::launch<raymarch_fwd_queue_kernel>(grid, block, smem + (size_t)nwarps * sizeof(RMQueue), s, a);
+  return gb::launch<raymarch_fwd_kernel<false, false>>(grid, block, smem, s, a);
 }
 
 // replaces mvpraymarchlib.raymarch_backward (mvpraymarch.cpp:285-399 -> mvpraymarch_kernel.cu:132-221).
@@ -1029,23 +1016,10 @@ GB_API int gb_mvp_raymarch_bwd(int N, int H, int W, int K, const float* raypos, 
   const int nwarps = (blocksizex * blocksizey + 31) / 32;
   const size_t smem = (size_t)nwarps * kMaxHit * (sizeof(int) + sizeof(float2));
   cudaStream_t s = (cudaStream_t)stream;
-  if (algo == 1) {
-    if (smem > 48 * 1024)
-      GB_CUDA(cudaFuncSetAttribute(raymarch_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    raymarch_bwd_kernel<true><<<grid, block, smem, s>>>(a);
-  } else if (raymarch_mode() & 2) {  // lane-compacted backward (option, algo 0)
-    const size_t smem_q = smem + (size_t)nwarps * sizeof(RMQueueB);
-    if (smem_q > 48 * 1024)
-      GB_CUDA(cudaFuncSetAttribute(raymarch_bwd_queue_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_q));
-    raymarch_bwd_queue_kernel<<<grid, block, smem_q, s>>>(a);
-  } else {
-    if (smem > 48 * 1024)
-      GB_CUDA(cudaFuncSetAttribute(raymarch_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    raymarch_bwd_kernel<false><<<grid, block, smem, s>>>(a);
-  }
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  if (algo == 1) return gb::launch<raymarch_bwd_kernel<true>>(grid, block, smem, s, a);
+  if (raymarch_mode() & 2)  // lane-compacted backward (option, algo 0)
+    return gb::launch<raymarch_bwd_queue_kernel>(grid, block, smem + (size_t)nwarps * sizeof(RMQueueB), s, a);
+  return gb::launch<raymarch_bwd_kernel<false>>(grid, block, smem, s, a);
 }
 
 // Deep shadow march of the relightable hand teacher (hand_teacher_mvp.py:274-358 with mvpraymarch(with_shadow=True)):
@@ -1073,10 +1047,5 @@ GB_API int gb_mvp_shadow_march(int N, int L, int H, int W, int K, const float* r
   const int nwarps = (blocksizex * blocksizey + 31) / 32;
   const size_t smem = (size_t)nwarps * kMaxHit * (sizeof(int) + sizeof(float2));
   cudaStream_t s = (cudaStream_t)stream;
-  if (smem > 48 * 1024)
-    GB_CUDA(cudaFuncSetAttribute(shadow_march_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  shadow_march_kernel<<<grid, block, smem, s>>>(a);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<shadow_march_kernel>(grid, block, smem, s, a);
 }

@@ -178,12 +178,9 @@ GB_API int gb_olat_features(int B, int L, int K, int TD, int TH, int TW, int U, 
   if (B <= 0 || L <= 0 || U <= 0) return 0;
   if (TD < 1 || TH < 1 || TW < 1 || U % TW || U % TH || (U / TW) * (U / TH) != K) return (int)cudaErrorInvalidValue;
   const size_t total = (size_t)B * TD * U * U;
-  olat_features_kernel<<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(
+  return gb::launch<olat_features_kernel>(grid_for(total), 256, 0, (cudaStream_t)stream,
       B, L, K, TD, TH, TW, U, volradius, primpos, primrot, primscale, valid, light_pos, campos, (const float2*)shadow,
       feat, primshadow, accumulate, shadow_feat);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 // replaces the compose of OLATRGBDecoder.forward_rgb (hand_teacher_mvp.py:468-479): tex [B*L,4Z,U,U], intensity
@@ -193,11 +190,8 @@ GB_API int gb_olat_compose_fwd(int B, int L, int Z, int U, const float* tex, con
                                const float* shadow_feat, float* rgb, int accumulate, float* texolat, void* stream) {
   if (B <= 0 || L <= 0 || Z <= 0 || U <= 0) return 0;
   const size_t total = (size_t)B * Z * U * U;
-  olat_compose_fwd_kernel<<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(B, L, Z, U, tex, intensity, shadow_feat,
-                                                                             rgb, accumulate, texolat);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<olat_compose_fwd_kernel>(grid_for(total), 256, 0, (cudaStream_t)stream, B, L, Z, U, tex, intensity,
+                                             shadow_feat, rgb, accumulate, texolat);
 }
 
 // gradient of gb_olat_compose_fwd w.r.t. tex: g_tex [B*L,4Z,U,U] (written) from g_rgb [B,Z,3,U,U] and g_texolat
@@ -207,9 +201,6 @@ GB_API int gb_olat_compose_bwd(int B, int L, int Z, int U, const float* tex, con
                                void* stream) {
   if (B <= 0 || L <= 0 || Z <= 0 || U <= 0) return 0;
   const size_t total = (size_t)B * Z * U * U;
-  olat_compose_bwd_kernel<<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(B, L, Z, U, tex, intensity, shadow_feat,
-                                                                             g_rgb, g_texolat, g_tex);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<olat_compose_bwd_kernel>(grid_for(total), 256, 0, (cudaStream_t)stream, B, L, Z, U, tex, intensity,
+                                             shadow_feat, g_rgb, g_texolat, g_tex);
 }

@@ -147,10 +147,8 @@ GB_API int gb_optim_row_bytes(void) { return (int)sizeof(TensorRow); }
 // gradients after non-finite entries were zeroed in place (rows with g == NULL are skipped).
 GB_API int gb_grad_sanitize_sqnorm(const void* rows, const int32_t* chunks, int n_chunks, double* sqnorm, void* stream) {
   if (n_chunks <= 0) return 0;
-  grad_sanitize_sqnorm_kernel<<<n_chunks, kThreads, 0, (cudaStream_t)stream>>>((const TensorRow*)rows, (const int2*)chunks, sqnorm);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<grad_sanitize_sqnorm_kernel>(n_chunks, kThreads, 0, (cudaStream_t)stream, (const TensorRow*)rows,
+                                                 (const int2*)chunks, sqnorm);
 }
 
 // One Adam (adamw = 0) / AdamW (adamw = 1) step over every row; gradients are scaled by clamp(max_norm / (sqrt(*sqnorm)
@@ -163,8 +161,5 @@ GB_API int gb_adam_step(const void* rows, const int32_t* chunks, int n_chunks, c
   a.rows = (const TensorRow*)rows; a.chunks = (const int2*)chunks; a.sqnorm = sqnorm; a.max_norm = max_norm;
   a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.step = step; a.adamw = adamw;
   a.write_grads = write_grads;
-  adam_step_kernel<<<n_chunks, kThreads, 0, (cudaStream_t)stream>>>(a);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<adam_step_kernel>(n_chunks, kThreads, 0, (cudaStream_t)stream, a);
 }

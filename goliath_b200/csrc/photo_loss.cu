@@ -405,10 +405,8 @@ GB_API int gb_post_render_fwd(int B, int H, int W, const float* rgb, const float
   a.blur_w = blur_w; a.pred = pred;
   Taps t;
   make_taps(t);
-  post_render_fwd_kernel<<<dim3(gb::cdiv(W, kTile), gb::cdiv(H, kTile), B), kThreads, 0, (cudaStream_t)stream>>>(a, t);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<post_render_fwd_kernel>(dim3(gb::cdiv(W, kTile), gb::cdiv(H, kTile), B), kThreads, 0,
+                                            (cudaStream_t)stream, a, t);
 }
 
 // g_pred [B,3,H,W] -> g_rgb [B,3,H,W] (overwritten); g_cal_w / g_cal_b / g_blur_w [B,3] accumulated (caller zero-fills;
@@ -423,10 +421,8 @@ GB_API int gb_post_render_bwd(int B, int H, int W, const float* rgb, const float
   a.blur_w = blur_w; a.g_pred = g_pred; a.g_rgb = g_rgb; a.g_cal_w = g_cal_w; a.g_cal_b = g_cal_b; a.g_blur_w = g_blur_w;
   Taps t;
   make_taps(t);
-  post_render_bwd_kernel<<<dim3(gb::cdiv(W, kTile), gb::cdiv(H, kTile), B), kThreads, 0, (cudaStream_t)stream>>>(a, t);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<post_render_bwd_kernel>(dim3(gb::cdiv(W, kTile), gb::cdiv(H, kTile), B), kThreads, 0,
+                                            (cudaStream_t)stream, a, t);
 }
 
 // Masked L1 and SSIM sums of pred vs target (ca_code/loss/__init__.py:391-410, 479-494): sums[0] = sum |(pred - target) * mask|,
@@ -440,10 +436,8 @@ GB_API int gb_ssim_l1_fwd(int B, int H, int W, const float* pred, const float* t
   a.sums = sums;
   Taps t;
   make_taps(t);
-  ssim_l1_fwd_kernel<<<dim3(gb::cdiv(W, kTile), gb::cdiv(H, kTile), 3 * B), kThreads, 0, (cudaStream_t)stream>>>(a, t);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<ssim_l1_fwd_kernel>(dim3(gb::cdiv(W, kTile), gb::cdiv(H, kTile), 3 * B), kThreads, 0,
+                                        (cudaStream_t)stream, a, t);
 }
 
 // Gradient of loss = l1_weight * l1 + ssim_weight * (1 - ssim) w.r.t. pred, times the upstream gradient *g_loss (device
@@ -459,8 +453,6 @@ GB_API int gb_ssim_l1_bwd(int B, int H, int W, const float* pred, const float* t
   a.ssim_w = ssim_weight; a.g_pred = g_pred;
   Taps t;
   make_taps(t);
-  ssim_l1_bwd_kernel<<<dim3(gb::cdiv(W, kTile), gb::cdiv(H, kTile), 3 * B), kThreads, 0, (cudaStream_t)stream>>>(a, t);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<ssim_l1_bwd_kernel>(dim3(gb::cdiv(W, kTile), gb::cdiv(H, kTile), 3 * B), kThreads, 0,
+                                        (cudaStream_t)stream, a, t);
 }

@@ -53,12 +53,9 @@ GB_API int gb_compute_raydirs_fwd(int N, int H, int W, const float* viewpos, con
   if (N <= 0 || H <= 0 || W <= 0) return 0;
   dim3 block(32, 8);
   dim3 grid(gb::cdiv(W, 32), gb::cdiv(N * H, 8));
-  raydirs_fwd_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(N, H, W, viewpos, viewrot, (const float2*)focal,
-                                                               (const float2*)princpt, (const float2*)pixelcoords,
-                                                               volradius, raypos, raydir, (float2*)tminmax);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<raydirs_fwd_kernel>(grid, block, 0, (cudaStream_t)stream, N, H, W, viewpos, viewrot,
+                                        (const float2*)focal, (const float2*)princpt, (const float2*)pixelcoords,
+                                        volradius, raypos, raydir, (float2*)tminmax);
 }
 
 // replaces utilslib.compute_raydirs_backward (utils.cpp:84-132): the reference computes nothing here.

@@ -39,11 +39,8 @@ GB_API int gb_render_finish_fwd(int img_h, int img_w, const float* out4, const f
                                 float* alpha_img, float* depth, void* stream) {
   const int P = img_h * img_w;
   if (P <= 0) return 0;
-  finish_fwd_kernel<<<gb::cdiv(P, 256), 256, 0, (cudaStream_t)stream>>>(P, reinterpret_cast<const float4*>(out4), alpha,
-                                                                        rgb, alpha_img, depth);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<finish_fwd_kernel>(gb::cdiv(P, 256), 256, 0, (cudaStream_t)stream, P,
+                                       reinterpret_cast<const float4*>(out4), alpha, rgb, alpha_img, depth);
 }
 
 // g_rgb [3,H,W] / g_depth [1,H,W] (either may be NULL) -> g_out4 [H,W,4]; alpha receives no gradient (detached upstream).
@@ -51,9 +48,6 @@ GB_API int gb_render_finish_bwd(int img_h, int img_w, const float* alpha, const 
                                 float* g_out4, void* stream) {
   const int P = img_h * img_w;
   if (P <= 0) return 0;
-  finish_bwd_kernel<<<gb::cdiv(P, 256), 256, 0, (cudaStream_t)stream>>>(P, alpha, g_rgb, g_depth,
-                                                                        reinterpret_cast<float4*>(g_out4));
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<finish_bwd_kernel>(gb::cdiv(P, 256), 256, 0, (cudaStream_t)stream, P, alpha, g_rgb, g_depth,
+                                       reinterpret_cast<float4*>(g_out4));
 }

@@ -265,11 +265,9 @@ GB_API int gb_rgca_heads_fwd(int B, int G, const float* f_vnocond, const float* 
   a.light_sh2 = light_sh2; a.shsum2 = shsum2;
   if ((light_sh2 == nullptr) != (shsum2 == nullptr)) return (int)cudaErrorInvalidValue;
   if (light_sh2)
-    heads_fwd_kernel<true><<<dim3(gb::cdiv(G, kBlock), B), kBlock, 0, (cudaStream_t)stream>>>(a);
+    GB_CUDA(gb::launch<heads_fwd_kernel<true>>(dim3(gb::cdiv(G, kBlock), B), kBlock, 0, (cudaStream_t)stream, a));
   else
-    heads_fwd_kernel<false><<<dim3(gb::cdiv(G, kBlock), B), kBlock, 0, (cudaStream_t)stream>>>(a);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
+    GB_CUDA(gb::launch<heads_fwd_kernel<false>>(dim3(gb::cdiv(G, kBlock), B), kBlock, 0, (cudaStream_t)stream, a));
   return 0;
 }
 
@@ -296,10 +294,8 @@ GB_API int gb_rgca_heads_bwd(int B, int G, const float* f_vnocond, const float* 
   a.g_tn = g_tn; a.g_albedo = g_albedo;
   a.light_sh2 = light_sh2; a.g_shsum2 = g_shsum2;
   if (light_sh2 && g_shsum2)
-    heads_bwd_kernel<true><<<dim3(gb::cdiv(G, kBlock), B), kBlock, 0, (cudaStream_t)stream>>>(a);
+    GB_CUDA(gb::launch<heads_bwd_kernel<true>>(dim3(gb::cdiv(G, kBlock), B), kBlock, 0, (cudaStream_t)stream, a));
   else
-    heads_bwd_kernel<false><<<dim3(gb::cdiv(G, kBlock), B), kBlock, 0, (cudaStream_t)stream>>>(a);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
+    GB_CUDA(gb::launch<heads_bwd_kernel<false>>(dim3(gb::cdiv(G, kBlock), B), kBlock, 0, (cudaStream_t)stream, a));
   return 0;
 }

@@ -338,8 +338,9 @@ GB_API int gb_sg_evaluate_fwd(const float* lobe_dirs, const float* lobe_sigmas, 
   if (w_type < 0 || w_type > 3) return (int)cudaErrorInvalidValue;
   dim3 grid(gb::cdiv(D, kBlock), N);
   cudaStream_t s = (cudaStream_t)stream;
-#define GB_SG_FWD(WT) \
-  sg_fwd_kernel<WT, false><<<grid, kBlock, 0, s>>>(lobe_dirs, lobe_sigmas, light_values, light_pts, prim_pts, n_lights, integral, D, L, Compose{})
+#define GB_SG_FWD(WT)                                                                                                  \
+  GB_CUDA(gb::launch<sg_fwd_kernel<WT, false>>(grid, kBlock, 0, s, lobe_dirs, lobe_sigmas, light_values, light_pts,    \
+                                               prim_pts, n_lights, integral, D, L, Compose{}))
   switch (w_type) {
     case 0: GB_SG_FWD(0); break;
     case 1: GB_SG_FWD(1); break;
@@ -347,8 +348,6 @@ GB_API int gb_sg_evaluate_fwd(const float* lobe_dirs, const float* lobe_sigmas, 
     default: GB_SG_FWD(3); break;
   }
 #undef GB_SG_FWD
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
   return 0;
 }
 
@@ -362,10 +361,10 @@ GB_API int gb_sg_evaluate_bwd(const float* lobe_dirs, const float* lobe_sigmas, 
   if (w_type < 0 || w_type > 3) return (int)cudaErrorInvalidValue;
   dim3 grid(gb::cdiv(D, kBlock), N);
   cudaStream_t s = (cudaStream_t)stream;
-#define GB_SG_BWD(WT, LG)                                                                                   \
-  sg_bwd_kernel<WT, LG, false><<<grid, kBlock, 0, s>>>(lobe_dirs, lobe_sigmas, light_values, light_pts, prim_pts, \
-                                                       n_lights, grad_integral, grad_dirs, grad_sigmas,          \
-                                                       grad_light_values, D, L, Compose{})
+#define GB_SG_BWD(WT, LG)                                                                                              \
+  GB_CUDA(gb::launch<sg_bwd_kernel<WT, LG, false>>(grid, kBlock, 0, s, lobe_dirs, lobe_sigmas, light_values,           \
+                                                   light_pts, prim_pts, n_lights, grad_integral, grad_dirs,            \
+                                                   grad_sigmas, grad_light_values, D, L, Compose{}))
   if (grad_light_values) {
     switch (w_type) {
       case 0: GB_SG_BWD(0, true); break;
@@ -382,8 +381,6 @@ GB_API int gb_sg_evaluate_bwd(const float* lobe_dirs, const float* lobe_sigmas, 
     }
   }
 #undef GB_SG_BWD
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
   return 0;
 }
 
@@ -400,8 +397,9 @@ GB_API int gb_sg_shade_compose_fwd(const float* lobe_dirs, const float* lobe_sig
   cudaStream_t s = (cudaStream_t)stream;
   Compose cz{};
   cz.diff_color = diff_color; cz.spec_vis = spec_vis; cz.color = color; cz.spec_color = spec_color;
-#define GB_SG_FWD(WT) \
-  sg_fwd_kernel<WT, true><<<grid, kBlock, 0, s>>>(lobe_dirs, lobe_sigmas, light_values, light_pts, prim_pts, n_lights, nullptr, D, L, cz)
+#define GB_SG_FWD(WT)                                                                                                  \
+  GB_CUDA(gb::launch<sg_fwd_kernel<WT, true>>(grid, kBlock, 0, s, lobe_dirs, lobe_sigmas, light_values, light_pts,     \
+                                              prim_pts, n_lights, nullptr, D, L, cz))
   switch (w_type) {
     case 0: GB_SG_FWD(0); break;
     case 1: GB_SG_FWD(1); break;
@@ -409,8 +407,6 @@ GB_API int gb_sg_shade_compose_fwd(const float* lobe_dirs, const float* lobe_sig
     default: GB_SG_FWD(3); break;
   }
 #undef GB_SG_FWD
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
   return 0;
 }
 
@@ -430,9 +426,10 @@ GB_API int gb_sg_shade_compose_bwd(const float* lobe_dirs, const float* lobe_sig
   Compose cz{};
   cz.diff_color = diff_color; cz.spec_vis = spec_vis; cz.color = const_cast<float*>(color);
   cz.g_color = g_color; cz.g_spec_color = g_spec_color; cz.g_diff = g_diff; cz.g_vis = g_vis;
-#define GB_SG_BWD(WT, LG)                                                                                          \
-  sg_bwd_kernel<WT, LG, true><<<grid, kBlock, 0, s>>>(lobe_dirs, lobe_sigmas, light_values, light_pts, prim_pts, \
-                                                      n_lights, nullptr, g_dirs, g_sigmas, g_light_values, D, L, cz)
+#define GB_SG_BWD(WT, LG)                                                                                              \
+  GB_CUDA(gb::launch<sg_bwd_kernel<WT, LG, true>>(grid, kBlock, 0, s, lobe_dirs, lobe_sigmas, light_values,            \
+                                                  light_pts, prim_pts, n_lights, nullptr, g_dirs, g_sigmas,            \
+                                                  g_light_values, D, L, cz))
   if (g_light_values) {
     switch (w_type) {
       case 0: GB_SG_BWD(0, true); break;
@@ -449,7 +446,5 @@ GB_API int gb_sg_shade_compose_bwd(const float* lobe_dirs, const float* lobe_sig
     }
   }
 #undef GB_SG_BWD
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
   return 0;
 }

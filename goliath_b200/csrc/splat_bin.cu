@@ -289,12 +289,9 @@ GB_API int gb_cumsum_i32(int n, const int32_t* in, int32_t* out, void* workspace
   cudaStream_t s = (cudaStream_t)stream;
   const int tiles = gb::cdiv(n, kScanTile);
   int* tile_sums = (int*)workspace;
-  scan_tile_sums_kernel<<<tiles, kScanBlock, 0, s>>>(n, in, tile_sums);
-  scan_small_kernel<<<1, kScanBlock, 0, s>>>(tiles, tile_sums);
-  scan_apply_kernel<<<tiles, kScanBlock, 0, s>>>(n, in, tile_sums, out);
-  gb::count_launches(3);
-  GB_CHECK_LAUNCH();
-  return 0;
+  GB_CUDA(gb::launch<scan_tile_sums_kernel>(tiles, kScanBlock, 0, s, n, in, tile_sums));
+  GB_CUDA(gb::launch<scan_small_kernel>(1, kScanBlock, 0, s, tiles, tile_sums));
+  return gb::launch<scan_apply_kernel>(tiles, kScanBlock, 0, s, n, in, tile_sums, out);
 }
 
 // replaces gsplat._C.map_gaussian_to_intersects
@@ -303,11 +300,8 @@ static int map_impl(int G, const float* xys, const float* depths, const int32_t*
                     void* stream) {
   if (G <= 0) return 0;
   const int tbx = gb::cdiv(img_w, block_width), tby = gb::cdiv(img_h, block_width);
-  map_to_intersects_kernel<<<gb::cdiv(G, 256), 256, 0, (cudaStream_t)stream>>>(
+  return gb::launch<map_to_intersects_kernel>(gb::cdiv(G, 256), 256, 0, (cudaStream_t)stream,
       G, (const float2*)xys, depths, radii, cum_tiles_hit, tbx, tby, block_width, (long long*)isect_ids, gaussian_ids, cap);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 GB_API int gb_map_gaussian_to_intersects(int G, const float* xys, const float* depths, const int32_t* radii,
@@ -361,14 +355,13 @@ static int sort_impl(int64_t n, const int* n_dev, const int64_t* isect_ids, cons
     unsigned long long* dst_k = to_out ? (unsigned long long*)isect_sorted : alt_k;
     int* dst_v = to_out ? gids_sorted : alt_v;
     const int shift = 8 * p;
-    sort_hist_kernel<<<tiles, kSortBlock, 0, s>>>(n, n_dev, src_k, shift, tiles, hist);
-    sort_scan_kernel<<<kRadix, kScanBlock, 0, s>>>(hist, tiles, totals);
-    sort_scatter_kernel<<<tiles, kSortBlock, 0, s>>>(n, n_dev, src_k, src_v, dst_k, dst_v, shift, tiles, hist, totals);
+    GB_CUDA(gb::launch<sort_hist_kernel>(tiles, kSortBlock, 0, s, n, n_dev, src_k, shift, tiles, hist));
+    GB_CUDA(gb::launch<sort_scan_kernel>(kRadix, kScanBlock, 0, s, hist, tiles, totals));
+    GB_CUDA(gb::launch<sort_scatter_kernel>(tiles, kSortBlock, 0, s, n, n_dev, src_k, src_v, dst_k, dst_v, shift, tiles,
+                                            hist, totals));
     src_k = dst_k;
     src_v = dst_v;
   }
-  gb::count_launches(3 * passes);
-  GB_CHECK_LAUNCH();
   return 0;
 }
 
@@ -387,11 +380,8 @@ GB_API int gb_sort_intersects_dn(int64_t cap, const int32_t* n_dev, const int64_
 static int edges_impl(int64_t n, const int* n_dev, const int64_t* isect_sorted, int32_t* tile_bins, int* overflow,
                       void* stream) {
   if (n <= 0) return 0;
-  tile_bin_edges_kernel<<<(unsigned)gb::cdiv64(n, 256), 256, 0, (cudaStream_t)stream>>>(
+  return gb::launch<tile_bin_edges_kernel>((unsigned)gb::cdiv64(n, 256), 256, 0, (cudaStream_t)stream,
       n, n_dev, (const long long*)isect_sorted, (int2*)tile_bins, overflow);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 // replaces gsplat._C.get_tile_bin_edges; tile_bins [T,2] int32 must be zeroed by the caller

@@ -393,18 +393,6 @@ int num_sms() {
   return s_sms[dev];
 }
 
-// opt in to a dynamic shared-memory window above 48 KB, once per device and kernel
-template <typename K>
-int opt_in_smem(K kernel, size_t bytes, bool* done) {
-  int dev = 0;
-  GB_CUDA(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64 || !done[dev]) {
-    GB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    if (dev >= 0 && dev < 64) done[dev] = true;
-  }
-  return 0;
-}
-
 }  // namespace
 
 // There is one formulation of the binning; these report it as mode 0 and accept (and ignore) any setting, so callers
@@ -511,60 +499,37 @@ static int bin_tiles_impl(int G, const float* xys, const float* depths, const in
   const int smem_tiles = (T <= kMaxSmemTiles) ? T : 0;
   const int stage_cap = scatter_stage_cap(smem_tiles);
   const size_t scat_smem = scatter_smem_bytes(smem_tiles);
-  static bool s_opt_c2[64] = {}, s_opt_c4[64] = {}, s_opt_scat[64] = {}, s_opt_sort[64] = {};
-  if ((size_t)smem_tiles * 4 > 40 * 1024) {
-    constexpr size_t kCountSmem = (size_t)kMaxSmemTiles * 4;
-    const int e = (items == 2) ? opt_in_smem(tile_count_kernel<2>, kCountSmem, s_opt_c2)
-                               : opt_in_smem(tile_count_kernel<4>, kCountSmem, s_opt_c4);
-    if (e) return e;
-  }
-  {  // the largest window any grid asks for: the tile arrays of kMaxSmemTiles, or those of kStageMaxTiles + staging
-    const size_t a = scatter_smem_bytes(kMaxSmemTiles), b = scatter_smem_bytes(kStageMaxTiles);
-    const int e = opt_in_smem(tile_scatter_kernel, a > b ? a : b, s_opt_scat);
-    if (e) return e;
-  }
-  const size_t sort_smem = (size_t)kSortCap * 8;
-  {
-    const int e = opt_in_smem(tile_sort_kernel, sort_smem, s_opt_sort);
-    if (e) return e;
-  }
 
   GB_CUDA(cudaMemsetAsync(ws, 0, l.zero_bytes, s));
   const int ctas = gb::cdiv(G, kGaussBlock * items);
   if (items == 2)
-    tile_count_kernel<2><<<ctas, kGaussBlock, (size_t)smem_tiles * 4, s>>>(G, (const float2*)xys, radii, tbx, tby,
-                                                                          block_width, smem_tiles, counts, rects, ext_identity);
+    GB_CUDA(gb::launch<tile_count_kernel<2>>(ctas, kGaussBlock, (size_t)smem_tiles * 4, s, G, (const float2*)xys, radii,
+                                             tbx, tby, block_width, smem_tiles, counts, rects, ext_identity));
   else
-    tile_count_kernel<4><<<ctas, kGaussBlock, (size_t)smem_tiles * 4, s>>>(G, (const float2*)xys, radii, tbx, tby,
-                                                                          block_width, smem_tiles, counts, rects, ext_identity);
+    GB_CUDA(gb::launch<tile_count_kernel<4>>(ctas, kGaussBlock, (size_t)smem_tiles * 4, s, G, (const float2*)xys, radii,
+                                             tbx, tby, block_width, smem_tiles, counts, rects, ext_identity));
   int* n_total = n_out ? n_out : (int*)(ws + l.sync);  // the record gather below needs the count on the device
-  tile_scan_kernel<<<1, 1024, 0, s>>>(T, (long long)cap, counts, (int2*)tile_bins, cursor, n_total, overflow);
-  gb::count_launches(2);
-  GB_CHECK_LAUNCH();
+  GB_CUDA(gb::launch<tile_scan_kernel>(1, 1024, 0, s, T, (long long)cap, counts, (int2*)tile_bins, cursor, n_total,
+                                       overflow));
   const int e = tile_sched ? gb_tile_schedule(T, tile_bins, tile_order, stream)
                            : gb_tile_order(T, tile_bins, tile_order, stream);
   if (e) return e;
   const bool late = colors_ready != nullptr;  // the colour quarter of the by-id records is filled after the tile sort
   const int per_cta = scatter_per_cta(G, num_sms());
-  tile_scatter_kernel<<<gb::cdiv(G, per_cta), kGaussBlock, scat_smem, s>>>(
+  GB_CUDA(gb::launch<tile_scatter_kernel>(gb::cdiv(G, per_cta), kGaussBlock, scat_smem, s,
       G, rects, (const float2*)xys, conics, late ? nullptr : colors3, depths, opacity, compensation, tbx, (long long)cap,
-      per_cta, smem_tiles, stage_cap, cursor, bucket, (unsigned*)ids_sorted, rec_by_id);
-  gb::count_launches(1);
+      per_cta, smem_tiles, stage_cap, cursor, bucket, (unsigned*)ids_sorted, rec_by_id));
   if (!ext_bucket) {  // else the caller's forward sorts each bucket
-    tile_sort_kernel<<<T, kSortThreads, sort_smem, s>>>(tile_order, (const int2*)tile_bins, (const unsigned*)depths, bucket,
-                                                        ids_sorted);
-    gb::count_launches(1);
+    GB_CUDA(gb::launch<tile_sort_kernel>(T, kSortThreads, (size_t)kSortCap * 8, s, tile_order, (const int2*)tile_bins,
+                                         (const unsigned*)depths, bucket, ids_sorted));
   }
   if (late) {
     GB_CUDA(cudaStreamWaitEvent(s, (cudaEvent_t)colors_ready, 0));
-    rec_colors_kernel<<<gb::cdiv(G, 256), 256, 0, s>>>(G, radii, colors3, depths, rec_by_id);
-    gb::count_launches(1);
+    GB_CUDA(gb::launch<rec_colors_kernel>(gb::cdiv(G, 256), 256, 0, s, G, radii, colors3, depths, rec_by_id));
   }
   if (cap > 0 && !ranked) {
-    gather_records_kernel<<<(unsigned)gb::cdiv64(3 * cap, 256), 256, 0, s>>>((long long)cap, n_total, gids_sorted,
-                                                                           rec_by_id, (float4*)records);
-    gb::count_launches(1);
+    GB_CUDA(gb::launch<gather_records_kernel>((unsigned)gb::cdiv64(3 * cap, 256), 256, 0, s, (long long)cap, n_total,
+                                              gids_sorted, rec_by_id, (float4*)records));
   }
-  GB_CHECK_LAUNCH();
   return 0;
 }

@@ -314,15 +314,13 @@ GB_API int gb_rasterize_fwd(int img_h, int img_w, int block_width, int channels,
   const int threads = ((block_width * block_width + 31) / 32) * 32;
   cudaStream_t s = (cudaStream_t)stream;
   if (channels == 3)
-    rasterize_fwd_kernel<3><<<grid, threads, 0, s>>>(img_w, img_h, block_width, gids_sorted, (const int2*)tile_bins,
-                                                     (const float2*)xys, conics, colors, opacities, background,
-                                                     final_Ts, final_idx, out_img);
+    GB_CUDA(gb::launch<rasterize_fwd_kernel<3>>(grid, threads, 0, s, img_w, img_h, block_width, gids_sorted,
+                                                (const int2*)tile_bins, (const float2*)xys, conics, colors, opacities,
+                                                background, final_Ts, final_idx, out_img));
   else
-    rasterize_fwd_kernel<4><<<grid, threads, 0, s>>>(img_w, img_h, block_width, gids_sorted, (const int2*)tile_bins,
-                                                     (const float2*)xys, conics, colors, opacities, background,
-                                                     final_Ts, final_idx, out_img);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
+    GB_CUDA(gb::launch<rasterize_fwd_kernel<4>>(grid, threads, 0, s, img_w, img_h, block_width, gids_sorted,
+                                                (const int2*)tile_bins, (const float2*)xys, conics, colors, opacities,
+                                                background, final_Ts, final_idx, out_img));
   return 0;
 }
 
@@ -339,16 +337,14 @@ GB_API int gb_rasterize_bwd(int img_h, int img_w, int block_width, int channels,
   const int threads = ((block_width * block_width + 31) / 32) * 32;
   cudaStream_t s = (cudaStream_t)stream;
   if (channels == 3)
-    rasterize_bwd_kernel<3><<<grid, threads, 0, s>>>(img_w, img_h, block_width, gids_sorted, (const int2*)tile_bins,
-                                                     (const float2*)xys, conics, colors, opacities, background,
-                                                     final_Ts, final_idx, v_output, v_output_alpha, v_xy, v_conic,
-                                                     v_colors, v_opacity);
+    GB_CUDA(gb::launch<rasterize_bwd_kernel<3>>(grid, threads, 0, s, img_w, img_h, block_width, gids_sorted,
+                                                (const int2*)tile_bins, (const float2*)xys, conics, colors, opacities,
+                                                background, final_Ts, final_idx, v_output, v_output_alpha, v_xy,
+                                                v_conic, v_colors, v_opacity));
   else
-    rasterize_bwd_kernel<4><<<grid, threads, 0, s>>>(img_w, img_h, block_width, gids_sorted, (const int2*)tile_bins,
-                                                     (const float2*)xys, conics, colors, opacities, background,
-                                                     final_Ts, final_idx, v_output, v_output_alpha, v_xy, v_conic,
-                                                     v_colors, v_opacity);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
+    GB_CUDA(gb::launch<rasterize_bwd_kernel<4>>(grid, threads, 0, s, img_w, img_h, block_width, gids_sorted,
+                                                (const int2*)tile_bins, (const float2*)xys, conics, colors, opacities,
+                                                background, final_Ts, final_idx, v_output, v_output_alpha, v_xy,
+                                                v_conic, v_colors, v_opacity));
   return 0;
 }

@@ -1528,10 +1528,6 @@ __global__ void __launch_bounds__(256) colors12_unpack_kernel(long long G, int n
   v12[3 * g] = z; v12[3 * g + 1] = z; v12[3 * g + 2] = z;
 }
 
-bool g_multi_attr_set[64] = {};
-
-bool g_attr_set[64] = {};  // per device: the > 48 KB dynamic shared memory opt-in of the backward kernel
-
 }  // namespace
 
 namespace gbblend {
@@ -1552,9 +1548,9 @@ static int launch_fwd_any(int img_h, int img_w, int channels, const int32_t* til
   if (sched && !tile_order) return (int)cudaErrorInvalidValue;
   static const bool list = fwd_list_variant();
 #define GB_FWD_MOM(CC, LL, RR, ...)                                                                                     \
-  blend_fwd_ilp_kernel<CC, LL, RR, ##__VA_ARGS__><<<tbx * tby, kFwdThreads, 0, s>>>(                                   \
+  GB_CUDA(gb::launch<blend_fwd_ilp_kernel<CC, LL, RR, ##__VA_ARGS__>>(tbx * tby, kFwdThreads, 0, s,                     \
       img_w, img_h, tbx, tile_order, sched, (const int2*)tile_bins, (const float4*)records, ranks, background, final_Ts, \
-      final_idx, out_img, hit_list, hit_count)
+      final_idx, out_img, hit_list, hit_count))
   if (ranks && hit_list) {
     if (channels == 3) GB_FWD_MOM(3, true, true, true); else GB_FWD_MOM(4, true, true, true);
   } else if (ranks) {
@@ -1565,8 +1561,6 @@ static int launch_fwd_any(int img_h, int img_w, int channels, const int32_t* til
     if (list) GB_FWD_MOM(4, true, false); else GB_FWD_MOM(4, false, false);
   }
 #undef GB_FWD_MOM
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
   return 0;
 }
 
@@ -1579,13 +1573,11 @@ static int launch_fwd_sort(int img_h, int img_w, int channels, const int32_t* ti
                            float* depth_img = nullptr) {
   const int tbx = gb::cdiv(img_w, 16), tby = gb::cdiv(img_h, 16);
 #define GB_FWD_SORT(CC, FF)                                                                                             \
-  blend_fwd_sort_kernel<CC, FF><<<tbx * tby, kFwdThreads, 0, s>>>(                                                     \
-      img_w, img_h, tbx, tile_order, (const int2*)tile_bins, (const float4*)records, background, final_Ts, final_idx,  \
-      out_img, hit_list, hit_count, (const unsigned*)depths, bucket, ranks, alpha_img, depth_img)
+  GB_CUDA(gb::launch<blend_fwd_sort_kernel<CC, FF>>(tbx * tby, kFwdThreads, 0, s,                                       \
+      img_w, img_h, tbx, tile_order, (const int2*)tile_bins, (const float4*)records, background, final_Ts, final_idx,   \
+      out_img, hit_list, hit_count, (const unsigned*)depths, bucket, ranks, alpha_img, depth_img))
   if (alpha_img) GB_FWD_SORT(4, true); else if (channels == 3) GB_FWD_SORT(3, false); else GB_FWD_SORT(4, false);
 #undef GB_FWD_SORT
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
   return 0;
 }
 
@@ -1596,27 +1588,16 @@ static int launch_bwd_any(int img_h, int img_w, int channels, const int32_t* gid
                           cudaStream_t s) {
   const int tbx = gb::cdiv(img_w, 16), tby = gb::cdiv(img_h, 16);
   if (sched && !tile_order) return (int)cudaErrorInvalidValue;
-  int dev = 0;
-  GB_CUDA(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64 || !g_attr_set[dev]) {
-    GB_CUDA(cudaFuncSetAttribute(blend_bwd_mom_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmem));
-    GB_CUDA(cudaFuncSetAttribute(blend_bwd_mom_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmem));
-    GB_CUDA(cudaFuncSetAttribute(blend_bwd_mom_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmem));
-    GB_CUDA(cudaFuncSetAttribute(blend_bwd_mom_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmem));
-    if (dev >= 0 && dev < 64) g_attr_set[dev] = true;
-  }
 #define GB_BWD_MOM(CC, RR)                                                                                              \
-  blend_bwd_mom_kernel<CC, RR><<<tbx * tby, kBwdThreads, kBwdSmem, s>>>(                                                \
+  GB_CUDA(gb::launch<blend_bwd_mom_kernel<CC, RR>>(tbx * tby, kBwdThreads, kBwdSmem, s,                                 \
       img_w, img_h, tbx, tile_order, sched, gids_sorted, ranks, (const int2*)tile_bins, (const float4*)records, background, \
-      final_Ts, final_idx, v_output, v_output_alpha, v_xy, v_conic, v_colors, v_opacity)
+      final_Ts, final_idx, v_output, v_output_alpha, v_xy, v_conic, v_colors, v_opacity))
   if (ranks) {
     if (channels == 3) GB_BWD_MOM(3, true); else GB_BWD_MOM(4, true);
   } else {
     if (channels == 3) GB_BWD_MOM(3, false); else GB_BWD_MOM(4, false);
   }
 #undef GB_BWD_MOM
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
   return 0;
 }
 
@@ -1646,16 +1627,14 @@ static int launch_bwd_lists(int img_h, int img_w, int channels, const int32_t* r
     per_sm = max(1, n) * sms;
   }
   const int grid = min(per_sm, gb::cdiv(n_items, kListWarps));
-  order_items_kernel<<<1, 1024, 0, s>>>(n_items, hit_count);
+  GB_CUDA(gb::launch<order_items_kernel>(1, 1024, 0, s, n_items, hit_count));
 #define GB_BWD_LISTS(CC, FF)                                                                                            \
-  blend_bwd_lists_kernel<CC, FF><<<grid, kListThreads, 0, s>>>(                                                         \
+  GB_CUDA(gb::launch<blend_bwd_lists_kernel<CC, FF>>(grid, kListThreads, 0, s,                                          \
       img_w, img_h, tbx, n_items, (const int2*)tile_bins, hit_list, hit_count, hit_count + n_items, ranks,              \
       (const float4*)records, background, final_Ts, final_idx, v_output, v_output_alpha, v_xy, v_conic, v_colors,       \
-      v_opacity, g_depth, alpha_img)
+      v_opacity, g_depth, alpha_img))
   if (finish) GB_BWD_LISTS(4, true); else if (channels == 3) GB_BWD_LISTS(3, false); else GB_BWD_LISTS(4, false);
 #undef GB_BWD_LISTS
-  gb::count_launches(2);
-  GB_CHECK_LAUNCH();
   return 0;
 }
 
@@ -1777,22 +1756,16 @@ GB_API int gb_rasterize_ranked_bwd_lists_finish(int img_h, int img_w, const int3
 // wide records [cap, 20] fp32: geometry of the 48-byte records + 4 x rgb.
 GB_API int gb_records_widen(int64_t cap, const int32_t* n_dev, const float* records, float* records_wide, void* stream) {
   if (cap <= 0) return 0;
-  records_widen_kernel<<<(unsigned)gb::cdiv64(cap, 256), 256, 0, (cudaStream_t)stream>>>(cap, n_dev, (const float4*)records,
-                                                                                         (float4*)records_wide);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<records_widen_kernel>((unsigned)gb::cdiv64(cap, 256), 256, 0, (cudaStream_t)stream, cap, n_dev,
+                                          (const float4*)records, (float4*)records_wide);
 }
 // colors: nk (1..4) consecutive [G,3] tables; missing conditions are blended as black.
 GB_API int gb_records_set_colors4(int64_t cap, const int32_t* n_dev, const int32_t* gids_sorted, const float* colors, int nk,
                                   int64_t G, float* records_wide, void* stream) {
   if (cap <= 0) return 0;
   if (nk < 1 || nk > 4) return (int)cudaErrorInvalidValue;
-  records_set_colors4_kernel<<<(unsigned)gb::cdiv64(cap, 256), 256, 0, (cudaStream_t)stream>>>(cap, n_dev, gids_sorted, colors, nk,
-                                                                                               G, (float4*)records_wide);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<records_set_colors4_kernel>((unsigned)gb::cdiv64(cap, 256), 256, 0, (cudaStream_t)stream, cap,
+                                                n_dev, gids_sorted, colors, nk, G, (float4*)records_wide);
 }
 // out_planes [4][H][W][3]: the four conditions' images (background added); same tile_bins / order as the single pass.
 GB_API int gb_rasterize_multi_fwd(int img_h, int img_w, const int32_t* tile_bins, const int32_t* tile_order, int sched,
@@ -1800,11 +1773,8 @@ GB_API int gb_rasterize_multi_fwd(int img_h, int img_w, const int32_t* tile_bins
   if (img_h <= 0 || img_w <= 0) return 0;
   if (sched && !tile_order) return (int)cudaErrorInvalidValue;
   const int tbx = gb::cdiv(img_w, 16), tby = gb::cdiv(img_h, 16);
-  blend_fwd_multi_kernel<<<tbx * tby, kFwdThreads, 0, (cudaStream_t)stream>>>(
+  return gb::launch<blend_fwd_multi_kernel>(tbx * tby, kFwdThreads, 0, (cudaStream_t)stream,
       img_w, img_h, tbx, tile_order, sched, (const int2*)tile_bins, (const float4*)records_wide, background, out_planes);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 // v_planes [4][H][W][3]; final_Ts / final_idx of the view (from the single-condition pass); v_xy / v_conic / v_opacity are
 // accumulated into; v_colors12 [G,12] (zero-filled) receives the four colour gradients interleaved per Gaussian.
@@ -1814,26 +1784,15 @@ GB_API int gb_rasterize_multi_bwd(int img_h, int img_w, const int32_t* gids_sort
                                   float* v_conic, float* v_colors12, float* v_opacity, void* stream) {
   if (img_h <= 0 || img_w <= 0) return 0;
   if (sched && !tile_order) return (int)cudaErrorInvalidValue;
-  int dev = 0;
-  GB_CUDA(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64 || !g_multi_attr_set[dev]) {
-    GB_CUDA(cudaFuncSetAttribute(blend_bwd_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMBwdSmem));
-    if (dev >= 0 && dev < 64) g_multi_attr_set[dev] = true;
-  }
   const int tbx = gb::cdiv(img_w, 16), tby = gb::cdiv(img_h, 16);
-  blend_bwd_multi_kernel<<<tbx * tby, kBwdThreads, kMBwdSmem, (cudaStream_t)stream>>>(
+  return gb::launch<blend_bwd_multi_kernel>(tbx * tby, kBwdThreads, kMBwdSmem, (cudaStream_t)stream,
       img_w, img_h, tbx, tile_order, sched, gids_sorted, (const int2*)tile_bins, (const float4*)records_wide, background, final_Ts,
       final_idx, v_planes, v_xy, v_conic, v_colors12, v_opacity);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 // v_colors12 [G,12] -> nk consecutive [G,3] tables (overwritten); clears v_colors12 for the next group.
 GB_API int gb_colors12_unpack(int64_t G, int nk, float* v_colors12, float* v_colors, void* stream) {
   if (G <= 0) return 0;
   if (nk < 1 || nk > 4) return (int)cudaErrorInvalidValue;
-  colors12_unpack_kernel<<<(unsigned)gb::cdiv64(G, 256), 256, 0, (cudaStream_t)stream>>>(G, nk, (float4*)v_colors12, v_colors);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<colors12_unpack_kernel>((unsigned)gb::cdiv64(G, 256), 256, 0, (cudaStream_t)stream, G, nk,
+                                            (float4*)v_colors12, v_colors);
 }

@@ -436,11 +436,11 @@ GB_API int gb_pack_records(int64_t n, int channels, const int32_t* gids_sorted, 
   cudaStream_t s = (cudaStream_t)stream;
   const unsigned blocks = (unsigned)gb::cdiv64(n, 256);
   if (channels == 3)
-    pack_records_kernel<3><<<blocks, 256, 0, s>>>(n, gids_sorted, (const float2*)xys, conics, colors, opacities, (float4*)records);
+    GB_CUDA(gb::launch<pack_records_kernel<3>>(blocks, 256, 0, s, n, gids_sorted, (const float2*)xys, conics, colors,
+                                               opacities, (float4*)records));
   else
-    pack_records_kernel<4><<<blocks, 256, 0, s>>>(n, gids_sorted, (const float2*)xys, conics, colors, opacities, (float4*)records);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
+    GB_CUDA(gb::launch<pack_records_kernel<4>>(blocks, 256, 0, s, n, gids_sorted, (const float2*)xys, conics, colors,
+                                               opacities, (float4*)records));
   return 0;
 }
 
@@ -449,11 +449,8 @@ static int pack_fused_impl(int64_t n, const int32_t* n_dev, const int32_t* gids_
                            const float* conics, const float* colors3, const float* depths, const float* opacity,
                            const float* compensation, float* records, void* stream) {
   if (n <= 0) return 0;
-  pack_records_fused_kernel<<<(unsigned)gb::cdiv64(n, 256), 256, 0, (cudaStream_t)stream>>>(
+  return gb::launch<pack_records_fused_kernel>((unsigned)gb::cdiv64(n, 256), 256, 0, (cudaStream_t)stream,
       n, n_dev, gids_sorted, (const float2*)xys, conics, colors3, depths, opacity, compensation, (float4*)records);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 GB_API int gb_pack_records_fused(int64_t n, const int32_t* gids_sorted, const float* xys, const float* conics,
                                  const float* colors3, const float* depths, const float* opacity,
@@ -472,11 +469,8 @@ GB_API int gb_pack_records_fused_dn(int64_t cap, const int32_t* n_dev, const int
 GB_API int gb_records_set_colors(int64_t cap, const int32_t* n_dev, const int32_t* gids_sorted, const float* colors3,
                                  const float* depths, float* records, void* stream) {
   if (cap <= 0) return 0;
-  records_set_colors_kernel<<<(unsigned)gb::cdiv64(cap, 256), 256, 0, (cudaStream_t)stream>>>(
+  return gb::launch<records_set_colors_kernel>((unsigned)gb::cdiv64(cap, 256), 256, 0, (cudaStream_t)stream,
       cap, n_dev, gids_sorted, colors3, depths, (float4*)records);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 // Backward glue of the fused render (all outputs overwritten): v_colors3 [G,3], v_opacity [G], v_comp [G], v_depth [G].
@@ -484,20 +478,14 @@ GB_API int gb_splat_grad_unpack(int G, const float* v_colors4, const float* v_op
                                 const float* compensation, float* v_colors3, float* v_opacity, float* v_comp,
                                 float* v_depth, void* stream) {
   if (G <= 0) return 0;
-  splat_grad_unpack_kernel<<<gb::cdiv(G, 256), 256, 0, (cudaStream_t)stream>>>(
+  return gb::launch<splat_grad_unpack_kernel>(gb::cdiv(G, 256), 256, 0, (cudaStream_t)stream,
       G, (const float4*)v_colors4, v_opac_eff, opacity, compensation, v_colors3, v_opacity, v_comp, v_depth);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 // Launch order of the tiles: longest list first.  order: [T] int32.
 GB_API int gb_tile_order(int num_tiles, const int32_t* tile_bins, int32_t* order, void* stream) {
   if (num_tiles <= 0) return 0;
-  tile_order_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(num_tiles, (const int2*)tile_bins, order, 0);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<tile_order_kernel>(1, 1024, 0, (cudaStream_t)stream, num_tiles, (const int2*)tile_bins, order, 0);
 }
 
 // SM-affine schedule of the tiles: `sched` holds gb_tile_schedule_ints(num_tiles) int32.  One queue per SM, filled
@@ -506,11 +494,8 @@ GB_API int gb_tile_order(int num_tiles, const int32_t* tile_bins, int32_t* order
 GB_API int gb_tile_schedule_ints(int num_tiles) { return (num_tiles > 0 ? num_tiles : 0) + gbblend::kSchedQueues + 1; }
 GB_API int gb_tile_schedule(int num_tiles, const int32_t* tile_bins, int32_t* sched, void* stream) {
   if (num_tiles <= 0) return 0;
-  tile_order_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(num_tiles, (const int2*)tile_bins, sched,
-                                                          gbblend::kSchedQueues);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
+  return gb::launch<tile_order_kernel>(1, 1024, 0, (cudaStream_t)stream, num_tiles, (const int2*)tile_bins, sched,
+                                       gbblend::kSchedQueues);
 }
 
 // Blend forward over packed records (block_width == 16).  tile_order may be NULL (row-major launch order).
@@ -528,13 +513,13 @@ GB_API int gb_rasterize_packed_fwd(int img_h, int img_w, int channels, const int
     return gbblend::launch_fwd_pipe(img_h, img_w, channels, tile_bins, tile_order, 0, records, background, out_img,
                                     final_Ts, final_idx, s);
   if (channels == 3)
-    blend_fwd_packed_kernel<3><<<tbx * tby, kThreads, 0, s>>>(img_w, img_h, tbx, tile_order, (const int2*)tile_bins,
-                                                              (const float4*)records, background, final_Ts, final_idx, out_img);
+    GB_CUDA(gb::launch<blend_fwd_packed_kernel<3>>(tbx * tby, kThreads, 0, s, img_w, img_h, tbx, tile_order,
+                                                   (const int2*)tile_bins, (const float4*)records, background, final_Ts,
+                                                   final_idx, out_img));
   else
-    blend_fwd_packed_kernel<4><<<tbx * tby, kThreads, 0, s>>>(img_w, img_h, tbx, tile_order, (const int2*)tile_bins,
-                                                              (const float4*)records, background, final_Ts, final_idx, out_img);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
+    GB_CUDA(gb::launch<blend_fwd_packed_kernel<4>>(tbx * tby, kThreads, 0, s, img_w, img_h, tbx, tile_order,
+                                                   (const int2*)tile_bins, (const float4*)records, background, final_Ts,
+                                                   final_idx, out_img));
   return 0;
 }
 
@@ -556,14 +541,14 @@ GB_API int gb_rasterize_packed_bwd(int img_h, int img_w, int channels, const int
                                     final_Ts, final_idx, v_output, v_output_alpha, v_xy, v_conic, v_colors, v_opacity,
                                     s);
   if (channels == 3)
-    blend_bwd_packed_kernel<3><<<tbx * tby, kThreads, 0, s>>>(img_w, img_h, tbx, tile_order, gids_sorted, (const int2*)tile_bins,
-                                                              (const float4*)records, background, final_Ts, final_idx,
-                                                              v_output, v_output_alpha, v_xy, v_conic, v_colors, v_opacity);
+    GB_CUDA(gb::launch<blend_bwd_packed_kernel<3>>(tbx * tby, kThreads, 0, s, img_w, img_h, tbx, tile_order,
+                                                   gids_sorted, (const int2*)tile_bins, (const float4*)records,
+                                                   background, final_Ts, final_idx, v_output, v_output_alpha, v_xy,
+                                                   v_conic, v_colors, v_opacity));
   else
-    blend_bwd_packed_kernel<4><<<tbx * tby, kThreads, 0, s>>>(img_w, img_h, tbx, tile_order, gids_sorted, (const int2*)tile_bins,
-                                                              (const float4*)records, background, final_Ts, final_idx,
-                                                              v_output, v_output_alpha, v_xy, v_conic, v_colors, v_opacity);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
+    GB_CUDA(gb::launch<blend_bwd_packed_kernel<4>>(tbx * tby, kThreads, 0, s, img_w, img_h, tbx, tile_order,
+                                                   gids_sorted, (const int2*)tile_bins, (const float4*)records,
+                                                   background, final_Ts, final_idx, v_output, v_output_alpha, v_xy,
+                                                   v_conic, v_colors, v_opacity));
   return 0;
 }

@@ -439,15 +439,13 @@ int launch_fwd_pipe(int img_h, int img_w, int channels, const int32_t* tile_bins
   const int tbx = gb::cdiv(img_w, 16), tby = gb::cdiv(img_h, 16);
   if (sched && !tile_order) return (int)cudaErrorInvalidValue;
   if (channels == 3)
-    blend_fwd_pipe_kernel<3><<<tbx * tby, kFwdThreads, 0, s>>>(img_w, img_h, tbx, tile_order, sched, (const int2*)tile_bins,
-                                                               (const float4*)records, background, final_Ts, final_idx,
-                                                               out_img);
+    GB_CUDA(gb::launch<blend_fwd_pipe_kernel<3>>(tbx * tby, kFwdThreads, 0, s, img_w, img_h, tbx, tile_order, sched,
+                                                 (const int2*)tile_bins, (const float4*)records, background, final_Ts,
+                                                 final_idx, out_img));
   else
-    blend_fwd_pipe_kernel<4><<<tbx * tby, kFwdThreads, 0, s>>>(img_w, img_h, tbx, tile_order, sched, (const int2*)tile_bins,
-                                                               (const float4*)records, background, final_Ts, final_idx,
-                                                               out_img);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
+    GB_CUDA(gb::launch<blend_fwd_pipe_kernel<4>>(tbx * tby, kFwdThreads, 0, s, img_w, img_h, tbx, tile_order, sched,
+                                                 (const int2*)tile_bins, (const float4*)records, background, final_Ts,
+                                                 final_idx, out_img));
   return 0;
 }
 
@@ -458,15 +456,13 @@ int launch_bwd_pipe(int img_h, int img_w, int channels, const int32_t* gids_sort
   const int tbx = gb::cdiv(img_w, 16), tby = gb::cdiv(img_h, 16);
   if (sched && !tile_order) return (int)cudaErrorInvalidValue;
   if (channels == 3)
-    blend_bwd_pipe_kernel<3><<<tbx * tby, kBwdThreads, 0, s>>>(
+    GB_CUDA(gb::launch<blend_bwd_pipe_kernel<3>>(tbx * tby, kBwdThreads, 0, s,
         img_w, img_h, tbx, tile_order, sched, gids_sorted, (const int2*)tile_bins, (const float4*)records, background, final_Ts,
-        final_idx, v_output, v_output_alpha, v_xy, v_conic, v_colors, v_opacity);
+        final_idx, v_output, v_output_alpha, v_xy, v_conic, v_colors, v_opacity));
   else
-    blend_bwd_pipe_kernel<4><<<tbx * tby, kBwdThreads, 0, s>>>(
+    GB_CUDA(gb::launch<blend_bwd_pipe_kernel<4>>(tbx * tby, kBwdThreads, 0, s,
         img_w, img_h, tbx, tile_order, sched, gids_sorted, (const int2*)tile_bins, (const float4*)records, background, final_Ts,
-        final_idx, v_output, v_output_alpha, v_xy, v_conic, v_colors, v_opacity);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
+        final_idx, v_output, v_output_alpha, v_xy, v_conic, v_colors, v_opacity));
   return 0;
 }
 

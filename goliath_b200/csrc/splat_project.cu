@@ -321,12 +321,9 @@ GB_API int gb_project_gaussians_fwd(int G, const float* means3d, const float* sc
                                     int32_t* num_tiles_hit, void* stream) {
   if (G <= 0) return 0;
   if (block_width < 2 || block_width > 16) return (int)cudaErrorInvalidValue;
-  project_fwd_kernel<<<gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream>>>(
+  return gb::launch<project_fwd_kernel>(gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream,
       G, means3d, scales, glob_scale, (const float4*)quats, viewmat, fx, fy, cx, cy, img_h, img_w, block_width,
       clip_thresh, cov3d, (float2*)xys, depths, radii, conics, compensation, num_tiles_hit, nullptr);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 // gb_project_gaussians_fwd that also zeroes grad_acc [10 G] fp32, the accumulator the fused render's blend backward
@@ -339,12 +336,9 @@ GB_API int gb_project_gaussians_fwd_acc(int G, const float* means3d, const float
                                         float* compensation, int32_t* num_tiles_hit, float* grad_acc, void* stream) {
   if (G <= 0) return 0;
   if (block_width < 2 || block_width > 16 || !grad_acc) return (int)cudaErrorInvalidValue;
-  project_fwd_kernel<<<gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream>>>(
+  return gb::launch<project_fwd_kernel>(gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream,
       G, means3d, scales, glob_scale, (const float4*)quats, viewmat, fx, fy, cx, cy, img_h, img_w, block_width,
       clip_thresh, cov3d, (float2*)xys, depths, radii, conics, compensation, num_tiles_hit, grad_acc);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 // replaces gsplat._C.project_gaussians_backward (autograd of the call at render_gsplat.py:49-63)
@@ -355,12 +349,9 @@ GB_API int gb_project_gaussians_bwd(int G, const float* means3d, const float* sc
                                     const float* v_conic, const float* v_compensation, float* v_cov2d,
                                     float* v_cov3d, float* v_mean3d, float* v_scale, float* v_quat, void* stream) {
   if (G <= 0) return 0;
-  project_bwd_kernel<<<gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream>>>(
+  return gb::launch<project_bwd_kernel>(gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream,
       G, means3d, scales, glob_scale, (const float4*)quats, viewmat, fx, fy, cov3d, radii, conics, compensation,
       (const float2*)v_xy, v_depth, v_conic, v_compensation, v_cov2d, v_cov3d, v_mean3d, v_scale, (float4*)v_quat);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }
 
 // Backward of the fused render per Gaussian, after its blend backward: grad_acc as gb_project_gaussians_fwd_acc left it
@@ -372,10 +363,7 @@ GB_API int gb_splat_project_bwd(int G, const float* means3d, const float* scales
                                 const float* grad_acc, float* v_colors, float* v_opacity, float* v_mean3d,
                                 float* v_scale, float* v_quat, void* stream) {
   if (G <= 0) return 0;
-  splat_project_bwd_kernel<<<gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream>>>(
+  return gb::launch<splat_project_bwd_kernel>(gb::cdiv(G, kBlock), kBlock, 0, (cudaStream_t)stream,
       G, means3d, scales, glob_scale, (const float4*)quats, viewmat, fx, fy, cov3d, radii, conics, compensation, opacity,
       grad_acc, v_colors, v_opacity, v_mean3d, v_scale, (float4*)v_quat);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }

@@ -88,28 +88,28 @@ __global__ void __launch_bounds__(256)
 }
 
 template <int CO_T>
-void launch_fwd_pair(int B, int Cin, int Cout, int groups, const InMap& u, const float* v1,
-                     const float* s1, const float* b1, const float* v2, const float* s2, const float* b2,
-                     const float* vr, const float* sr, const float* br, float slope, float* h1, float* out,
-                     unsigned char* mask, cudaStream_t s) {
+[[nodiscard]] int launch_fwd_pair(int B, int Cin, int Cout, int groups, const InMap& u, const float* v1,
+                                  const float* s1, const float* b1, const float* v2, const float* s2, const float* b2,
+                                  const float* vr, const float* sr, const float* br, float slope, float* h1,
+                                  float* out, unsigned char* mask, cudaStream_t s) {
   const int cin_g = Cin / groups, cout_g = Cout / groups;
   const int tiles = gb::cdiv(u.H, TP) * gb::cdiv(u.W, TP);
   dim3 g1(tiles, groups * gb::cdiv(cin_g, CO_T), B), g2(tiles, groups * gb::cdiv(cout_g, CO_T), B);
-  wn_conv_fwd_kernel<CO_T, 3, 1, false, 2, IN_UP2, IN_UP2><<<g1, TP * TP, 0, s>>>(cin_g, cin_g, groups, u, u.H, u.W, v1, s1, b1, 2, 1,
-                                                                slope, u, nullptr, nullptr, nullptr, h1, nullptr);
-  wn_conv_fwd_kernel<CO_T, 3, 1, true, 2, IN_PLAIN, IN_UP2><<<g2, TP * TP, 0, s>>>(
+  GB_CUDA(gb::launch<wn_conv_fwd_kernel<CO_T, 3, 1, false, 2, IN_UP2, IN_UP2>>(g1, TP * TP, 0, s,
+      cin_g, cin_g, groups, u, u.H, u.W, v1, s1, b1, 2, 1, slope, u, nullptr, nullptr, nullptr, h1, nullptr));
+  return gb::launch<wn_conv_fwd_kernel<CO_T, 3, 1, true, 2, IN_PLAIN, IN_UP2>>(g2, TP * TP, 0, s,
       cin_g, cout_g, groups, plain_map(h1, (long long)Cin * u.H * u.W, u.H, u.W), u.H, u.W, v2, s2, b2, 2, 1, slope, u,
       vr, sr, br, out, mask);
 }
 
 // gz1 = conv2^T(gz2) * lrelu'(h1), or (ACT = false) gu = conv1^T(gz1) + conv_resize^T(gout)
 template <int CO_T, bool ACT, int SKIP>
-void launch_dgrad(int B, int Cin, int n_sum_g, int groups, int H, int W, const float* gz, const float* v,
-                  const float* scale, const float* h1, float slope, int n_skip_g, const float* gs, const float* vr,
-                  const float* sr, float* out, cudaStream_t s) {
+[[nodiscard]] int launch_dgrad(int B, int Cin, int n_sum_g, int groups, int H, int W, const float* gz, const float* v,
+                               const float* scale, const float* h1, float slope, int n_skip_g, const float* gs,
+                               const float* vr, const float* sr, float* out, cudaStream_t s) {
   const int cin_g = Cin / groups;
   dim3 grid(gb::cdiv(H, TP) * gb::cdiv(W, TP), groups * gb::cdiv(cin_g, CO_T), B);
-  wn_conv_dgrad_kernel<CO_T, 3, 1, ACT, SKIP><<<grid, TP * TP, 0, s>>>(
+  return gb::launch<wn_conv_dgrad_kernel<CO_T, 3, 1, ACT, SKIP>>(grid, TP * TP, 0, s,
       cin_g, n_sum_g, groups, H, W, gz, v, scale, h1, slope, n_skip_g, gs, vr, sr, out, (long long)Cin * H * W);
 }
 
@@ -129,12 +129,8 @@ GB_API int gb_upconv_block_fwd(int B, int Cin, int Cout, int groups, int Hi, int
   cudaStream_t s = (cudaStream_t)stream;
   const InMap u = up2_map(x, Cin, Hi, Wi);
   if ((Cin / groups) % 8 == 0 && (Cout / groups) % 8 == 0)
-    launch_fwd_pair<8>(B, Cin, Cout, groups, u, v1, s1, b1, v2, s2, b2, vr, sr, br, slope, h1, out, mask, s);
-  else
-    launch_fwd_pair<4>(B, Cin, Cout, groups, u, v1, s1, b1, v2, s2, b2, vr, sr, br, slope, h1, out, mask, s);
-  gb::count_launches(2);
-  GB_CHECK_LAUNCH();
-  return 0;
+    return launch_fwd_pair<8>(B, Cin, Cout, groups, u, v1, s1, b1, v2, s2, b2, vr, sr, br, slope, h1, out, mask, s);
+  return launch_fwd_pair<4>(B, Cin, Cout, groups, u, v1, s1, b1, v2, s2, b2, vr, sr, br, slope, h1, out, mask, s);
 }
 
 GB_API size_t gb_upconv_block_bwd_workspace_bytes(int B, int Cin, int Cout, int groups, int Hi, int Wi) {
@@ -158,33 +154,28 @@ GB_API int gb_upconv_block_bwd(int B, int Cin, int Cout, int groups, int Hi, int
   const int cin_g = Cin / groups, cout_g = Cout / groups;
   const long long n_out = (long long)Cout * HW, n_in = (long long)Cin * HW;
   float* part = (float*)workspace;
-  act_bwd_kernel<<<(unsigned)gb::cdiv64(n_out, 256), 256, 0, s>>>(B, n_out, gout, mask, nullptr, slope, gz2, gb2);
-  chan_sum_kernel<<<Cout, 256, 0, s>>>(B, Cout, HW, gout, gbr);
+  GB_CUDA(gb::launch<act_bwd_kernel>((unsigned)gb::cdiv64(n_out, 256), 256, 0, s, B, n_out, gout, mask, nullptr, slope,
+                                     gz2, gb2));
+  GB_CUDA(gb::launch<chan_sum_kernel>(Cout, 256, 0, s, B, Cout, HW, gout, gbr));
   if (cin_g % 8 == 0)
-    launch_dgrad<8, true, 0>(B, Cin, cout_g, groups, H, W, gz2, v2, s2, h1, slope, 0, nullptr, nullptr, nullptr,
-                                 gz1, s);
+    GB_CUDA(launch_dgrad<8, true, 0>(B, Cin, cout_g, groups, H, W, gz2, v2, s2, h1, slope, 0, nullptr, nullptr,
+                                     nullptr, gz1, s));
   else
-    launch_dgrad<4, true, 0>(B, Cin, cout_g, groups, H, W, gz2, v2, s2, h1, slope, 0, nullptr, nullptr, nullptr,
-                                 gz1, s);
-  batch_sum_kernel<<<(unsigned)gb::cdiv64(n_in, 256), 256, 0, s>>>(B, n_in, gz1, gb1);
-  launch_wgrad<3, 1>(B, Cin, Cout, groups, plain_map(h1, n_in, H, W), H, W, gz2, gw2, part, kWgradPerSM, s);
-  launch_wgrad<3, 1>(B, Cin, Cin, groups, u, H, W, gz1, gw1, part, kWgradPerSM, s);
-  launch_wgrad<1, 1>(B, Cin, Cout, groups, u, H, W, gout, gwr, part, kWgradPerSM, s);
-  int n = 10;
-  if (gx) {
-    if (cin_g % 8 == 0)
-      launch_dgrad<8, false, 1>(B, Cin, cin_g, groups, H, W, gz1, v1, s1, nullptr, slope, cout_g, gout, vr, sr, gu,
-                                   s);
-    else
-      launch_dgrad<4, false, 1>(B, Cin, cin_g, groups, H, W, gz1, v1, s1, nullptr, slope, cout_g, gout, vr, sr, gu,
-                                   s);
-    const long long nx = (long long)B * Cin * Hi * Wi;
-    up_transpose_kernel<<<(unsigned)gb::cdiv64(nx, 256), 256, 0, s>>>(nx, u, gu, gx);
-    n += 2;
-  }
-  gb::count_launches(n);
-  GB_CHECK_LAUNCH();
-  return 0;
+    GB_CUDA(launch_dgrad<4, true, 0>(B, Cin, cout_g, groups, H, W, gz2, v2, s2, h1, slope, 0, nullptr, nullptr,
+                                     nullptr, gz1, s));
+  GB_CUDA(gb::launch<batch_sum_kernel>((unsigned)gb::cdiv64(n_in, 256), 256, 0, s, B, n_in, gz1, gb1));
+  GB_CUDA(launch_wgrad<3, 1>(B, Cin, Cout, groups, plain_map(h1, n_in, H, W), H, W, gz2, gw2, part, kWgradPerSM, s));
+  GB_CUDA(launch_wgrad<3, 1>(B, Cin, Cin, groups, u, H, W, gz1, gw1, part, kWgradPerSM, s));
+  GB_CUDA(launch_wgrad<1, 1>(B, Cin, Cout, groups, u, H, W, gout, gwr, part, kWgradPerSM, s));
+  if (!gx) return 0;
+  if (cin_g % 8 == 0)
+    GB_CUDA(launch_dgrad<8, false, 1>(B, Cin, cin_g, groups, H, W, gz1, v1, s1, nullptr, slope, cout_g, gout, vr, sr,
+                                      gu, s));
+  else
+    GB_CUDA(launch_dgrad<4, false, 1>(B, Cin, cin_g, groups, H, W, gz1, v1, s1, nullptr, slope, cout_g, gout, vr, sr,
+                                      gu, s));
+  const long long nx = (long long)B * Cin * Hi * Wi;
+  return gb::launch<up_transpose_kernel>((unsigned)gb::cdiv64(nx, 256), 256, 0, s, nx, u, gu, gx);
 }
 
 GB_API int gb_sparse_rows_apply(int B, int C, int n_rows, const int* row_ptr, const int* col, const float* coef,
@@ -192,9 +183,6 @@ GB_API int gb_sparse_rows_apply(int B, int C, int n_rows, const int* row_ptr, co
                                 long long out_bs, long long out_cs, long long out_rs, void* stream) {
   if (B <= 0 || C <= 0 || n_rows <= 0) return 0;
   const long long n = (long long)B * n_rows;
-  sparse_rows_kernel<<<(unsigned)gb::cdiv64(n, 256), 256, 0, (cudaStream_t)stream>>>(
+  return gb::launch<sparse_rows_kernel>((unsigned)gb::cdiv64(n, 256), 256, 0, (cudaStream_t)stream,
       B, C, n_rows, row_ptr, col, coef, in, in_bs, in_cs, in_rs, out, out_bs, out_cs, out_rs);
-  gb::count_launches(1);
-  GB_CHECK_LAUNCH();
-  return 0;
 }

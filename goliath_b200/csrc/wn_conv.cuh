@@ -459,16 +459,16 @@ size_t wgrad_part_floats(int B, int Cin, int Cout, int groups, int K, int Ho, in
   return (size_t)wgrad_split(B, cin_g, cout_g, groups, Ho, Wo, per_sm) * Cout * cin_g * K * K;
 }
 
-// gw [Cout, Cin/groups, K, K] written; two launches
+// gw [Cout, Cin/groups, K, K] written
 template <int K, int S>
-void launch_wgrad(int B, int Cin, int Cout, int groups, const InMap& in, int Ho, int Wo, const float* gz, float* gw,
+[[nodiscard]] int launch_wgrad(int B, int Cin, int Cout, int groups, const InMap& in, int Ho, int Wo, const float* gz, float* gw,
                   float* part, int per_sm, cudaStream_t s) {
   const int cin_g = Cin / groups, cout_g = Cout / groups;
   const int split = wgrad_split(B, cin_g, cout_g, groups, Ho, Wo, per_sm);
   dim3 grid(split, gb::cdiv(cin_g, BW_CI), groups * gb::cdiv(cout_g, BW_CO));
-  wn_conv_wgrad_kernel<K, S><<<grid, 256, 0, s>>>(B, cin_g, cout_g, groups, in, Ho, Wo, gz, part);
+  GB_CUDA(gb::launch<wn_conv_wgrad_kernel<K, S>>(grid, 256, 0, s, B, cin_g, cout_g, groups, in, Ho, Wo, gz, part));
   const int n = Cout * cin_g * K * K;
-  split_sum_kernel<<<gb::cdiv(n, 256), 256, 0, s>>>(split, n, part, gw);
+  return gb::launch<split_sum_kernel>(gb::cdiv(n, 256), 256, 0, s, split, n, part, gw);
 }
 
 }  // namespace
