@@ -163,3 +163,36 @@ def body_mesh(n_faces: int, img_h: int = 2048, img_w: int = 1334, batch: int = 4
         Rt[b, :, :3] = torch.tensor([[c, 0.0, s], [0.0, 1.0, 0.0], [-s, 0.0, c]])
         Rt[b, :, 3] = torch.tensor([0.0, 0.0, 2.3 + 0.4 * torch.rand(1, generator=g).item()])
     return dict(verts=verts, vi=vi, vti=vi.clone(), vt=vt, K=K, Rt=Rt)
+
+
+def uv_layout(n_charts: int = 64, quads: int = 16, seed: int = SEED + 11) -> Dict[str, torch.Tensor]:
+    """A seeded UV layout of real-avatar size for the UV-image builders (goliath_b200.geom): n_charts jittered grid
+    charts of quads x quads quads (2 quads^2 faces each, 32768 faces by default, windings mixed at random) packed in
+    u < 0.45, and one large face covering about 9 % of the map; about half the map is uncovered, and its far corner is
+    more than 100 texels from any chart at 1024^2.  Returns vt [N,2] fp32, vti [F,3] and vi [F,3] int64 (vi maps the
+    UV corners to mesh vertices through a permutation), v2uv [V,1] int64."""
+    g = torch.Generator().manual_seed(seed)
+    side = int(math.ceil(math.sqrt(n_charts)))
+    cell_u, cell_v = 0.43 / side, 0.96 / side
+    vts, faces, base = [], [], 0
+    for c in range(n_charts):
+        u0, v0 = 0.02 + (c % side) * cell_u, 0.02 + (c // side) * cell_v
+        a = torch.linspace(0.0, 1.0, quads + 1)
+        uu, vv = torch.meshgrid(a * 0.9 * cell_u, a * 0.9 * cell_v, indexing="ij")
+        jit = (torch.rand(quads + 1, quads + 1, 2, generator=g) - 0.5) * torch.tensor([cell_u, cell_v]) * (0.3 / quads)
+        jit[0, :], jit[-1, :], jit[:, 0], jit[:, -1] = 0, 0, 0, 0
+        vts.append(torch.stack([u0 + uu, v0 + vv], -1).add(jit).reshape(-1, 2))
+        k = torch.arange((quads + 1) ** 2).reshape(quads + 1, quads + 1)
+        q00, q10, q01, q11 = k[:-1, :-1], k[1:, :-1], k[:-1, 1:], k[1:, 1:]
+        f = torch.cat([torch.stack([q00, q10, q11], -1).reshape(-1, 3), torch.stack([q00, q11, q01], -1).reshape(-1, 3)])
+        flip = torch.rand(f.shape[0], generator=g) < 0.5
+        f[flip] = f[flip][:, [0, 2, 1]]
+        faces.append(f + base)
+        base += (quads + 1) ** 2
+    vts.append(torch.tensor([[0.46, 0.02], [0.78, 0.02], [0.46, 0.6]]))
+    faces.append(torch.tensor([[base, base + 1, base + 2]]))
+    vt = torch.cat(vts).float()
+    vti = torch.cat(faces).long()
+    V = vt.shape[0]
+    perm = torch.randperm(V, generator=g)
+    return {"vt": vt, "vti": vti, "vi": perm[vti], "v2uv": torch.arange(V)[:, None]}

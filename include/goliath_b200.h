@@ -946,6 +946,33 @@ int gb_hand_finish_bwd(int B, int H, int W, const float* rayrgba, const float* c
                        const float* bg, const float* g_rgb, const float* g_alpha, float* g_rayrgba, float* g_cal_w,
                        float* g_cal_b, void* workspace, void* stream);
 
+/* UV layout images (csrc/uv_layout.cu; the rasteriser's conventions are this project's, DESIGN.md R12).
+ * bytes of the workspace gb_uv_index_images needs: an int32 [U,U] face image and the large-face list */
+size_t gb_uv_raster_workspace_bytes(int F, int U);
+/* replaces make_uv_face_index, make_uv_vert_index and make_uv_barys (ca_code/utils/geom.py:31-142, pytorch3d's
+ * rasterize_meshes with one face per pixel): vt [N,2] fp32, vti [F,3] int32, flip = flip_uv.  Writes, each optional
+ * (NULL: skipped), face [U,U] int64 (-1 uncovered, the lowest covering face id otherwise), vert_index [U,U,3] int64 =
+ * vi[face] (-1 uncovered; needs vi [F,3] int32 when F > 0), bary [U,U,3] fp32 = bary_coords on the UV triangle at (grid[j],
+ * grid[i]) (0 uncovered; grid [U] fp32 = torch.linspace(0.5, U - 0.5, U) / U) and valid [U,U] uint8 = face >= 0. */
+int gb_uv_index_images(int F, int U, int flip, const float* vt, const int32_t* vti, const int32_t* vi,
+                       const float* grid, void* workspace, int64_t* face, int64_t* vert_index, float* bary,
+                       uint8_t* valid, void* stream);
+/* bytes of the workspace gb_uv_impaint_sources needs: the int32 [H,W] column distances */
+size_t gb_uv_impaint_workspace_bytes(int H, int W);
+/* replaces the KDTree query of index_image_impaint (geom.py:145-178): index [H,W,C] int64, a texel is valid when any
+ * channel is not -1.  Writes d2 [H,W] int32 = the exact squared distance to the nearest valid texel ((H + W)^2 or more
+ * when there is none) and src [H,W] int32 = the row-major index of the impaint source, -1 for valid texels and for
+ * d2 > d2max.  offsets [n,2] int32 (di, dj) sorted by (di^2 + dj^2, di, dj) with group_start [d2max + 2] int32 (the
+ * first offset of each squared length) pick, among equidistant valid texels, the smallest row-major index.
+ * W <= 14528. */
+int gb_uv_impaint_sources(int H, int W, int C, const int64_t* index, int d2max, const int32_t* offsets,
+                          const int32_t* group_start, void* workspace, int32_t* d2, int32_t* src, void* stream);
+/* replaces the indexed copies of index_image_impaint (geom.py:180-194) and its second call on the face image
+ * (GeometryModule.__init__, geom.py:238-244): for up to three images of T texels (in/out NULL: skipped) of words_k
+ * 32-bit words per texel, out[t] = in[src[t]] where src[t] >= 0 and in[t] elsewhere; every texel is written. */
+int gb_uv_impaint_gather(int64_t T, const int32_t* src, const void* in0, void* out0, int words0, const void* in1,
+                         void* out1, int words1, const void* in2, void* out2, int words2, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
